@@ -183,11 +183,52 @@ __device__ __forceinline__ uint64_t cg_home_slot(int64_t key, int hash_shift)
 	return ((uint64_t) key * 0x9E3779B97F4A7C15ull) >> hash_shift;
 }
 
-/* order-preserving map of float8 bits to unsigned (for min/max words) */
-__device__ __forceinline__ uint64_t f8_ordered(int64_t bits)
+/* order-preserving map of float8 bits to unsigned (for min/max words), in [PG] float8 btree order: every NaN,
+ * whatever its sign bit, is the one largest code (above +inf) */
+__host__ __device__ __forceinline__ uint64_t f8_ordered(int64_t bits)
 {
 	uint64_t u = (uint64_t) bits;
+	if ((u & 0x7fffffffffffffffull) > 0x7ff0000000000000ull) return ~0ull;
 	return (u >> 63) ? ~u : (u | 0x8000000000000000ull);
+}
+
+/* int64 multiply / add that set `ovf` when the exact result does not fit */
+__device__ __forceinline__ int64_t mul_ovf(int64_t x, int64_t y, bool &ovf)
+{
+	int64_t lo = (int64_t) ((uint64_t) x * (uint64_t) y);
+	ovf |= __mul64hi(x, y) != (lo >> 63);
+	return lo;
+}
+__device__ __forceinline__ int64_t add_ovf(int64_t x, int64_t y, bool &ovf)
+{
+	int64_t s = (int64_t) ((uint64_t) x + (uint64_t) y);
+	ovf |= ((x ^ s) & (y ^ s)) < 0;
+	return s;
+}
+
+/* integer term prod (a + b*x) of one aggregate; factor f reads column value x[f].  Without a proven bound
+ * (g.ovchk) a term that leaves int64 raises CG_ERRFLAG_TERM_OVERFLOW unless an input is NULL */
+template <int NCC>
+__device__ __forceinline__ int64_t int_term(const KAgg &g, const int64_t (&v)[NCC], bool isnull, unsigned long long *stats)
+{
+	int64_t it = 1;
+	if (!g.ovchk)
+	{
+#pragma unroll
+		for (int f = 0; f < 3; f++)
+			if (f < g.nfactors) it *= g.a[f] + g.b[f] * pick<NCC>(v, g.pcol[f]);
+		return it;
+	}
+	bool ovf = false;
+#pragma unroll
+	for (int f = 0; f < 3; f++)
+		if (f < g.nfactors)
+		{
+			int64_t t = add_ovf(g.a[f], mul_ovf(g.b[f], pick<NCC>(v, g.pcol[f]), ovf), ovf);
+			it = f ? mul_ovf(it, t, ovf) : t;
+		}
+	if (ovf && !isnull) atomicOr(stats + 2, CG_ERRFLAG_TERM_OVERFLOW);
+	return it;
 }
 
 __device__ __forceinline__ void word_apply_global(uint64_t *p, int op, uint64_t val)

@@ -882,6 +882,9 @@ static int check_error_flags(CgPartial *p, unsigned long long flags)
 	if (flags & CG_ERRFLAG_VARLENA)
 		return cg_set_error(CG_EUNSUPPORTED, "a numeric value is NaN, has more fractional digits than the column's scale or does not fit 64 bits, "
 											 "or a varlena stream is malformed");
+	if (flags & CG_ERRFLAG_TERM_OVERFLOW)
+		return cg_set_error(CG_EUNSUPPORTED, "an integer aggregate argument is out of the 64-bit range: "
+											 "the row-at-a-time executor computes it (bigint out of range, or exact numeric)");
 	return CG_OK;
 }
 
@@ -1657,8 +1660,10 @@ extern "C" int cg_partial_ngroups(CgPartial *p, int64_t *ngroups)
 	return export_rows(ctx, p, 0, nullptr, nullptr, nullptr, ngroups);
 }
 
+/* inverse of f8_ordered (cg_device.cuh); the one NaN code comes back as the default quiet NaN */
 static inline uint64_t f8_unordered(uint64_t u)
 {
+	if (u == ~0ull) return 0x7ff8000000000000ull;
 	return (u >> 63) ? (u & 0x7fffffffffffffffull) : ~u;
 }
 
@@ -1699,6 +1704,17 @@ extern "C" int cg_partial_fetch(CgPartial *p, int64_t capacity, int64_t *keys, u
 	CG_CUDA(cudaMemcpyAsync((void *) hw, p->d_out_words, wbytes, cudaMemcpyDeviceToHost, ctx->compute));
 	CG_CUDA(cudaStreamSynchronize(ctx->compute));
 	const int na = p->desc.naggs;
+	/* a two-limb sum's low word grows by < 2^32 per row of the group (scanned, or merged with its carry folded):
+	 * it is exact while the group has fewer than 2^32 rows */
+	for (int a = 0; a < na; a++)
+		if (p->aggs[a].kind == CG_AGG_SUM && !p->aggs[a].is_float && p->aggs[a].nlimbs == 2)
+		{
+			for (unsigned long long i = 0; i < n; i++)
+				if (hw[i * p->nwords] >> 32)
+					return cg_set_error(CG_EUNSUPPORTED, "a group of %llu rows: its two-limb sum may have wrapped",
+										(unsigned long long) hw[i * p->nwords]);
+			break;
+		}
 	const int nthreads = n >= 65536 ? std::max(1, std::min(ctx->stage_threads, 16)) : 1;
 #pragma omp parallel for schedule(static) num_threads(nthreads)
 	for (int64_t i = 0; i < (int64_t) n; i++)

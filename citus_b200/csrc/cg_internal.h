@@ -164,7 +164,9 @@ struct KAgg
 	int8_t word0;       /* first accumulator word (count(x): its NULL-count word) */
 	int8_t nullword;    /* word counting NULL inputs among the group's rows:
 						 * non-NULL inputs = rows in group (word 0) - this word */
-	int8_t pad[3];
+	int8_t ovchk;       /* integer term with no proven bound: every factor and product is checked for int64
+						 * overflow (CG_ERRFLAG_TERM_OVERFLOW) */
+	int8_t pad[2];
 	int64_t a[3];
 	int64_t b[3];
 	int64_t bound;      /* nlimbs == 1: every |term| must be <= bound */
@@ -286,6 +288,7 @@ static inline void cg_choose_slices(uint32_t nselected, uint32_t grid_full, uint
 #define CG_ERRFLAG_SUM_BOUND 8ull
 #define CG_ERRFLAG_DECOMPRESS 16ull
 #define CG_ERRFLAG_VARLENA 32ull
+#define CG_ERRFLAG_TERM_OVERFLOW 64ull   /* an integer aggregate argument left int64 */
 #define CG_COMM_TAIL 16           /* words behind an accumulator array that travel with it in a combine (cg_comm.cu) */
 #define CG_STAT_PACKED_ADDED 3
 #define CG_STAT_PACKED_DRAINED 4

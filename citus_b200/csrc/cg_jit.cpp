@@ -296,7 +296,7 @@ static void gen_prelude(std::string &s)
 		"typedef unsigned long long uint64_t; typedef long long int64_t; typedef unsigned int uint32_t; typedef int int32_t;\n"
 		"typedef unsigned short uint16_t; typedef short int16_t; typedef unsigned char uint8_t; typedef signed char int8_t;\n"
 		"struct DevChunkCol { uint64_t values_off; uint64_t exists_off; uint64_t rank_off; uint32_t value_count; uint32_t row_count; };\n"
-		"struct KAgg { int8_t kind; int8_t nfactors; int8_t is_float; int8_t nlimbs; int8_t pcol[3]; int8_t word0; int8_t nullword; int8_t pad[3];\n"
+		"struct KAgg { int8_t kind; int8_t nfactors; int8_t is_float; int8_t nlimbs; int8_t pcol[3]; int8_t word0; int8_t nullword; int8_t ovchk; int8_t pad[2];\n"
 		"  int64_t a[3]; int64_t b[3]; int64_t bound; int64_t tbound; };\n";
 	addf(s,
 		 "struct KPlan { const uint8_t *arena; const DevChunkCol *chunkcols; const uint32_t *selected; uint32_t nselected; int32_t nstaged;\n"
@@ -329,7 +329,13 @@ static void gen_prelude(std::string &s)
 		/* [PG] float8 btree order: NaN equals NaN and is greater than everything */
 		"__device__ __forceinline__ int fcmp(int64_t a, int64_t b) { double x = __longlong_as_double(a), y = __longlong_as_double(b);\n"
 		"  bool xn = x != x, yn = y != y; return (xn || yn) ? ((int) xn - (int) yn) : ((x > y) - (x < y)); }\n"
-		"__device__ __forceinline__ uint64_t f8_ordered(int64_t bits) { uint64_t u = (uint64_t) bits; return (u >> 63) ? ~u : (u | 0x8000000000000000ull); }\n"
+		/* every NaN is the one largest code, above +inf */
+		"__device__ __forceinline__ uint64_t f8_ordered(int64_t bits) { uint64_t u = (uint64_t) bits;\n"
+		"  if ((u & 0x7fffffffffffffffull) > 0x7ff0000000000000ull) return ~0ull; return (u >> 63) ? ~u : (u | 0x8000000000000000ull); }\n"
+		"__device__ __forceinline__ int64_t mul_ovf(int64_t x, int64_t y, bool &o) { int64_t l = (int64_t) ((uint64_t) x * (uint64_t) y);\n"
+		"  o |= __mul64hi(x, y) != (l >> 63); return l; }\n"
+		"__device__ __forceinline__ int64_t add_ovf(int64_t x, int64_t y, bool &o) { int64_t r = (int64_t) ((uint64_t) x + (uint64_t) y);\n"
+		"  o |= ((x ^ r) & (y ^ r)) < 0; return r; }\n"
 		"__device__ __noinline__ void raise_flag(unsigned long long *stats, unsigned long long flag) { atomicOr(stats + 2, flag); }\n"
 		"__device__ __forceinline__ uint64_t wsum(uint64_t x) { for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o); return x; }\n"
 		"__device__ __noinline__ uint64_t hash_slot_slow(const KPlan &P, int64_t key, uint64_t h) {\n"
@@ -422,6 +428,14 @@ static std::string term_expr(const KAgg &g, int a)
 			if (g.a[f] == 0 && fb == 1.0) snprintf(buf, sizeof buf, "__longlong_as_double(v%d)", g.pcol[f]);
 			else snprintf(buf, sizeof buf, "(__longlong_as_double(P.aggs[%d].a[%d]) + __longlong_as_double(P.aggs[%d].b[%d]) * __longlong_as_double(v%d))",
 						  a, f, a, f, g.pcol[f]);
+		}
+		else if (g.ovchk)
+		{
+			/* no proven bound: every factor and product is checked (mul_ovf / add_ovf set ov<a>) */
+			if (g.a[f] == 0 && g.b[f] == 1) snprintf(buf, sizeof buf, "v%d", g.pcol[f]);
+			else snprintf(buf, sizeof buf, "add_ovf(P.aggs[%d].a[%d], mul_ovf(P.aggs[%d].b[%d], v%d, ov%d), ov%d)", a, f, a, f, g.pcol[f], a, a);
+			e = f ? "mul_ovf(" + e + ", " + buf + ", ov" + std::to_string(a) + ")" : std::string(buf);
+			continue;
 		}
 		else if (g.a[f] == 0 && g.b[f] == 1) snprintf(buf, sizeof buf, "v%d", g.pcol[f]);
 		else snprintf(buf, sizeof buf, "(P.aggs[%d].a[%d] + P.aggs[%d].b[%d] * v%d)", a, f, a, f, g.pcol[f]);
@@ -610,7 +624,11 @@ static void gen_row(std::string &s, const KPlan &plan, const JitShape &sh, int u
 		if (g.is_float) addf(s, "%sconst double ft%d = %s;\n", C, a, e.c_str());
 		else
 		{
+			if (g.ovchk) addf(s, "%sbool ov%d = false;\n", C, a);
 			addf(s, "%sconst int64_t it%d = %s;\n", C, a, e.c_str());
+			if (g.ovchk)
+				addf(s, "%sif (%sov%d) raise_flag(P.stats, %lluull);\n", C, an[a].empty() ? "" : ("!an" + std::to_string(a) + " && ").c_str(),
+					 a, (unsigned long long) CG_ERRFLAG_TERM_OVERFLOW);
 			if (g.kind == CG_AGG_SUM && g.nlimbs == 1)
 				addf(s, "%sif (%s(it%d > P.aggs[%d].bound || it%d < -P.aggs[%d].bound)) raise_flag(P.stats, %lluull);\n", C,
 					 an[a].empty() ? "" : ("!an" + std::to_string(a) + " && ").c_str(), a, a, a, a, (unsigned long long) CG_ERRFLAG_SUM_BOUND);

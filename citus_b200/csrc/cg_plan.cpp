@@ -130,6 +130,10 @@ static int layout_partial(CgPartial *p, const CgColumnDesc *columns)
 		for (int f = 0; f < 3; f++) { k.a[f] = s.a[f]; k.b[f] = s.b[f]; }
 		k.nlimbs = 1;
 		k.tbound = (s.kind == CG_AGG_SUM && !s.is_float && s.term_abs_bound > 0) ? s.term_abs_bound : 0;
+		/* an integer argument other than a bare column can leave int64 ([PG] int8mul / int8pl raise "bigint out of
+		 * range", numeric is exact): unless the caller proved a bound, the kernels check every factor and product */
+		k.ovchk = (int8_t) (!s.is_float && (s.kind == CG_AGG_SUM || s.kind == CG_AGG_MIN || s.kind == CG_AGG_MAX) &&
+							k.tbound == 0 && !(s.nfactors == 1 && s.a[0] == 0 && s.b[0] == 1));
 		switch (s.kind)
 		{
 			case CG_AGG_COUNT_STAR:
@@ -189,7 +193,7 @@ int cg_partial_shape(CgPartial *p, const CgScanDesc *desc, const CgColumnDesc *c
 		p->mode = CG_MODE_GLOBAL;
 		p->capacity = 1; p->entries = 1; p->stride = p->nwords;
 	}
-	else if (desc->ngroup_cols == 2 && key_min <= key_max &&
+	else if (desc->ngroup_cols == 2 &&
 			 (int32_t) (uint32_t) key_min <= (int32_t) (uint32_t) key_max &&
 			 (int32_t) ((uint64_t) key_min >> 32) <= (int32_t) ((uint64_t) key_max >> 32) &&
 			 ((uint64_t) ((int64_t) (int32_t) (uint32_t) key_max - (int32_t) (uint32_t) key_min) + 1) *

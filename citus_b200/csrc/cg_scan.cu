@@ -138,13 +138,11 @@ __device__ __forceinline__ void process_row(const KPlan &P, const int64_t (&v)[N
 				{
 					int c = g.pcol[f];
 					isnull = isnull || ((nullmask >> c) & 1u);
-					int64_t x = pick<NCC>(v, c);
 					if (g.is_float)
-						ft *= __longlong_as_double(g.a[f]) + __longlong_as_double(g.b[f]) * __longlong_as_double(x);
-					else
-						it *= g.a[f] + g.b[f] * x;
+						ft *= __longlong_as_double(g.a[f]) + __longlong_as_double(g.b[f]) * __longlong_as_double(pick<NCC>(v, c));
 				}
 			}
+			if (!g.is_float) it = int_term<NCC>(g, v, isnull, P.stats);
 			if (isnull)
 			{
 				/* strict transition function: a NULL input is skipped, only counted */
@@ -832,6 +830,11 @@ int cg_launch_export_packed(CgPartial *p, uint64_t out_capacity, int64_t *d_keys
 __global__ void cg_merge_kernel(const __grid_constant__ KPlan P, const int64_t *keys, const uint8_t *nulls,
 								const uint64_t *words, int64_t nrows)
 {
+	/* low words of two-limb sums: a row's low word may hold up to 64 bits of summed low halves; its carry
+	 * (bits 32..63) moves to the high word, so the table's low word grows by < 2^32 per merged row */
+	uint32_t lo_words = 0;
+	for (int a = 0; a < P.naggs; a++)
+		if (P.aggs[a].kind == CG_AGG_SUM && !P.aggs[a].is_float && P.aggs[a].nlimbs == 2) lo_words |= 1u << P.aggs[a].word0;
 	for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < nrows; i += (int64_t) gridDim.x * blockDim.x)
 	{
 		uint64_t *entry;
@@ -843,9 +846,12 @@ __global__ void cg_merge_kernel(const __grid_constant__ KPlan P, const int64_t *
 											  : find_entry<CG_MODE_HASH>(P, keys[i], kn);
 			if (entry == nullptr) continue;
 		}
+		uint64_t carry = 0;
 		for (int w = 0; w < P.nwords; w++)
 		{
 			uint64_t val = words[i * (int64_t) P.nwords + w];
+			if ((lo_words >> w) & 1u) { carry = val >> 32; val &= 0xffffffffull; }
+			else if (w > 0 && ((lo_words >> (w - 1)) & 1u)) val += carry;
 			if (val != word_identity(P.wordop[w])) word_apply_global(entry + w, P.wordop[w], val);
 		}
 	}
@@ -863,6 +869,8 @@ int cg_launch_merge(CgPartial *p, const int64_t *d_keys, const uint8_t *d_nulls,
 	plan.hash_shift = 64;
 	for (uint64_t c = p->capacity; c > 1; c >>= 1) plan.hash_shift--;
 	for (int i = 0; i < CG_KMAX_WORDS; i++) plan.wordop[i] = p->wordop[i];
+	plan.naggs = p->desc.naggs;
+	for (int a = 0; a < p->desc.naggs; a++) plan.aggs[a] = p->aggs[a];
 	unsigned blocks = (unsigned) ((nrows + 255) / 256);
 	if (blocks > (unsigned) cg_ctx()->sm_count * 8) blocks = (unsigned) cg_ctx()->sm_count * 8;
 	cg_merge_kernel<<<blocks, 256, 0, stream>>>(plan, d_keys, d_nulls, d_words, nrows);

@@ -209,6 +209,8 @@ __device__ __forceinline__ void fast_row(const FPlan &P, const int64_t *v, FastA
 		for (int s = 0; s < NS; s++)
 		{
 			int64_t x = v[SUMPOS + s];
+			/* the limbs are exact whatever the bound; a violated bound is still the caller's error */
+			if (P.slimbs[s] == 1 && (x > P.sbound[s] || x < -P.sbound[s])) raise_flag(P.stats, CG_ERRFLAG_SUM_BOUND);
 			acc.lo[s] += (uint64_t) (uint32_t) x;
 			acc.hi[s] += x >> 32;
 		}

@@ -90,10 +90,9 @@ __device__ __forceinline__ void eval_terms(const KPlan &P, const int64_t (&v)[NC
 				{
 					int c = g.pcol[f];
 					isnull = isnull || ((nullmask >> c) & 1u);
-					int64_t x = pick<NCC>(v, c);
-					if (g.is_float) ft *= __longlong_as_double(g.a[f]) + __longlong_as_double(g.b[f]) * __longlong_as_double(x);
-					else it *= g.a[f] + g.b[f] * x;
+					if (g.is_float) ft *= __longlong_as_double(g.a[f]) + __longlong_as_double(g.b[f]) * __longlong_as_double(pick<NCC>(v, c));
 				}
+			if (!g.is_float) it = int_term<NCC>(g, v, isnull, P.stats);
 			if (isnull) { t.nullbits |= 1u << a; continue; }
 			if (g.kind == CG_AGG_COUNT) continue;
 			if (g.kind == CG_AGG_SUM)

@@ -89,7 +89,7 @@ extern "C" int cg_partial_merge_values(CgPartial *p, int64_t nrows, const int64_
 			{
 				if (!minmax) return cg_set_error(CG_EINVAL, "NULL minmax array");
 				uint64_t u = (uint64_t) minmax[i * na + a];
-				if (k.is_float) u = (u >> 63) ? ~u : (u | 0x8000000000000000ull);     /* order-preserving encoding of the words */
+				if (k.is_float) u = f8_ordered((int64_t) u);     /* order-preserving encoding of the words */
 				w[k.word0] = u;
 			}
 		}
@@ -190,7 +190,7 @@ extern "C" int cg_agg_column(int32_t attlen, int32_t is_float, const void *value
 	if (sum_lo) *sum_lo = (uint64_t) s;
 	if (is_float)
 	{
-		auto unorder = [](uint64_t u) { return (int64_t) ((u >> 63) ? (u & 0x7fffffffffffffffull) : ~u); };
+		auto unorder = [](uint64_t u) { return (int64_t) (u == ~0ull ? 0x7ff8000000000000ull : (u >> 63) ? (u & 0x7fffffffffffffffull) : ~u); };
 		if (min_value) *min_value = h.count ? unorder(h.fmin) : 0;
 		if (max_value) *max_value = h.count ? unorder(h.fmax) : 0;
 	}

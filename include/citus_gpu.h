@@ -191,7 +191,9 @@ typedef struct CgAggSpec
 	int64_t term_abs_bound; /* integer SUM: caller-proven bound on |argument| (from the skip lists'
 							 * min/max), 0 = unknown.  When bound * max_rows < 2^63 the sum is kept in
 							 * one 64-bit word instead of two; a row that violates the bound fails the
-							 * scan with CG_EINVAL (never a wrong answer). */
+							 * scan with CG_EINVAL (never a wrong answer).  Without a bound, an integer
+							 * sum / min / max argument that leaves int64 (in b*x, a + b*x or a product)
+							 * fails the scan with CG_EUNSUPPORTED, like PostgreSQL's "bigint out of range". */
 } CgAggSpec;
 
 #define CG_MAX_QUALS 8

@@ -835,6 +835,14 @@ static int orc_datum_cmp(int atttype, int64_t a, int64_t b)
 	return (a > b) - (a < b);
 }
 
+/* float8_cmp_internal on doubles (min/max transition and combine functions, float8smaller / float8larger) */
+static int orc_float8_cmp(double x, double y)
+{
+	int64_t a, b;
+	memcpy(&a, &x, 8); memcpy(&b, &y, 8);
+	return orc_datum_cmp(ORC_T_FLOAT, a, b);
+}
+
 /* columnar_storage.c:117-126 LogicalToPhysical + ColumnarStorageWrite (WriteToBlock
  * keeps pd_lower at the end of the written payload, :698-744) */
 static void orc_storage_write(OrcTable *t, uint64_t logical, const uint8_t *data, uint64_t amount)
@@ -1502,7 +1510,7 @@ int orc_scan_aggregate(const OrcTable *t, const OrcQual *quals, int nquals,
 			}
 			if (rc) break;
 
-			for (uint32_t i = 0; i < rowCount; i++)
+			for (uint32_t i = 0; i < rowCount && rc == 0; i++)
 			{
 				res->rows_scanned++;
 				int pass = orc_row_passes(t, quals, nquals, exists, values, i);
@@ -1527,7 +1535,7 @@ int orc_scan_aggregate(const OrcTable *t, const OrcQual *quals, int nquals,
 					const OrcAggSpec *sp = &aggs[a];
 					OrcAggState *st = &res->states[g * nagg + a];
 					if (sp->kind == ORC_AGG_COUNT_STAR) { st->count++; continue; }
-					int isnull = 0;
+					int isnull = 0, overflow = 0;
 					int128 iv = 1; double fv = 1.0;
 					for (int f = 0; f < sp->nfactors; f++)
 					{
@@ -1540,9 +1548,23 @@ int orc_scan_aggregate(const OrcTable *t, const OrcQual *quals, int nquals,
 							fv *= (da + db * d);
 						}
 						else
-							iv *= ((int128) sp->a[f] + (int128) sp->b[f] * (int128) values[c][i]);
+						{
+							/* [PG] int8mul / int8pl: b*x, a + b*x and every partial product must fit int64 */
+							int128 m = (int128) sp->b[f] * (int128) values[c][i];
+							int128 t = (int128) sp->a[f] + m;
+							if (m > INT64_MAX || m < INT64_MIN || t > INT64_MAX || t < INT64_MIN) overflow = 1;
+							iv *= t;
+							if (iv > INT64_MAX || iv < INT64_MIN) overflow = 1;
+							if (overflow) iv = 0;
+						}
 					}
 					if (isnull) continue;
+					if (overflow && (sp->kind == ORC_AGG_SUM || sp->kind == ORC_AGG_MIN || sp->kind == ORC_AGG_MAX))
+					{
+						rc = -1;
+						snprintf(orc_errbuf, sizeof orc_errbuf, "bigint out of range");
+						break;
+					}
 					switch (sp->kind)
 					{
 						case ORC_AGG_COUNT: st->count++; break;
@@ -1551,12 +1573,12 @@ int orc_scan_aggregate(const OrcTable *t, const OrcQual *quals, int nquals,
 							st->count++;
 							break;
 						case ORC_AGG_MIN:
-							if (sp->is_float) { if (st->count == 0 || fv < st->fmin) st->fmin = fv; }
+							if (sp->is_float) { if (st->count == 0 || orc_float8_cmp(fv, st->fmin) < 0) st->fmin = fv; }
 							else { if (st->count == 0 || (int64_t) iv < st->imin) st->imin = (int64_t) iv; }
 							st->count++;
 							break;
 						case ORC_AGG_MAX:
-							if (sp->is_float) { if (st->count == 0 || fv > st->fmax) st->fmax = fv; }
+							if (sp->is_float) { if (st->count == 0 || orc_float8_cmp(fv, st->fmax) > 0) st->fmax = fv; }
 							else { if (st->count == 0 || (int64_t) iv > st->imax) st->imax = (int64_t) iv; }
 							st->count++;
 							break;
@@ -1593,12 +1615,12 @@ int orc_combine(OrcScanResult *dst, const OrcScanResult *src, const OrcAggSpec *
 			if (aggs[a].kind == ORC_AGG_MIN)
 			{
 				if (!had || s->imin < o->imin) o->imin = s->imin;
-				if (!had || s->fmin < o->fmin) o->fmin = s->fmin;
+				if (!had || orc_float8_cmp(s->fmin, o->fmin) < 0) o->fmin = s->fmin;
 			}
 			if (aggs[a].kind == ORC_AGG_MAX)
 			{
 				if (!had || s->imax > o->imax) o->imax = s->imax;
-				if (!had || s->fmax > o->fmax) o->fmax = s->fmax;
+				if (!had || orc_float8_cmp(s->fmax, o->fmax) > 0) o->fmax = s->fmax;
 			}
 			o->count += s->count;
 		}
