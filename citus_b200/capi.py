@@ -24,6 +24,7 @@ CG_WORD_ADD, CG_WORD_MIN, CG_WORD_MAX, CG_WORD_FADD, CG_WORD_FMIN, CG_WORD_FMAX 
 CG_GEN_UNIFORM, CG_GEN_SEQUENCE = 0, 1
 CG_MAX_QUALS, CG_MAX_AGGS, CG_MAX_GROUP_COLS = 8, 8, 2
 CG_MAX_QEXPR, CG_QX_AND, CG_QX_OR = 16, -1, -2
+CG_MAX_FILTER_QUALS = 8
 
 
 class CgSkipNode(C.Structure):
@@ -73,7 +74,9 @@ class CgScanDesc(C.Structure):
                 ("enable_qual_pushdown", C.c_int32), ("ngroup_cols", C.c_int32),
                 ("group_cols", C.c_int32 * CG_MAX_GROUP_COLS), ("naggs", C.c_int32),
                 ("aggs", CgAggSpec * CG_MAX_AGGS), ("expected_groups", C.c_int64),
-                ("nqual_expr", C.c_int32), ("qual_expr", C.c_int8 * CG_MAX_QEXPR), ("reserved", C.c_int32)]
+                ("nqual_expr", C.c_int32), ("qual_expr", C.c_int8 * CG_MAX_QEXPR), ("reserved", C.c_int32),
+                ("nfilter_quals", C.c_int32), ("filter_quals", CgQual * CG_MAX_FILTER_QUALS),
+                ("nfilter_expr", C.c_int32 * CG_MAX_AGGS), ("filter_expr", (C.c_int8 * CG_MAX_QEXPR) * CG_MAX_AGGS)]
 
 
 class CgScanStats(C.Structure):

@@ -197,26 +197,27 @@ class Agg:
     factors: list = field(default_factory=list)    # [(column, a, b)]
     is_float: bool = False
     term_abs_bound: int = 0
+    filter: object = None        # FILTER (WHERE ...): a WHERE-style tree of (column, op, constant) atoms, None = none
 
 
-def count_star():
-    return Agg(CG_AGG_COUNT_STAR)
+def count_star(filter=None):
+    return Agg(CG_AGG_COUNT_STAR, filter=filter)
 
 
-def count(col):
-    return Agg(CG_AGG_COUNT, [(col, 0, 1)])
+def count(col, filter=None):
+    return Agg(CG_AGG_COUNT, [(col, 0, 1)], filter=filter)
 
 
-def sum_(col, is_float=False):
-    return Agg(CG_AGG_SUM, [(col, 0, 1)], is_float)
+def sum_(col, is_float=False, filter=None):
+    return Agg(CG_AGG_SUM, [(col, 0, 1)], is_float, filter=filter)
 
 
-def min_(col, is_float=False):
-    return Agg(CG_AGG_MIN, [(col, 0, 1)], is_float)
+def min_(col, is_float=False, filter=None):
+    return Agg(CG_AGG_MIN, [(col, 0, 1)], is_float, filter=filter)
 
 
-def max_(col, is_float=False):
-    return Agg(CG_AGG_MAX, [(col, 0, 1)], is_float)
+def max_(col, is_float=False, filter=None):
+    return Agg(CG_AGG_MAX, [(col, 0, 1)], is_float, filter=filter)
 
 
 def flatten_where(where):
@@ -242,6 +243,31 @@ def flatten_where(where):
     return atoms, tokens
 
 
+def _filter_tokens(tree, pool):
+    """one aggregate's FILTER tree -> postfix tokens over the shared filter atom pool (new atoms are appended to it; an
+    atom already in the pool, e.g. the same filter on several aggregates, is reused).  A list of atoms is their AND; a
+    bare atom is a tree of one atom."""
+    if isinstance(tree, list):
+        tree = ("and", *tree) if len(tree) > 1 else tree[0]
+    if isinstance(tree, tuple) and tree and tree[0] in ("and", "or"):
+        atoms, tokens = flatten_where(tree)
+    else:
+        atoms, tokens = [tuple(tree)], [0]
+    index = []
+    for atom in atoms:
+        if atom not in pool:
+            pool.append(atom)
+        index.append(pool.index(atom))
+    return [index[t] if t >= 0 else t for t in tokens]
+
+
+def _set_atom(q, atom, float_cols):
+    col, op, k = atom
+    q.column = col
+    q.op = capi.CG_OP[op]
+    q.konst = int(np.float64(k).view(np.int64)) if col in float_cols else int(k)
+
+
 def make_desc(quals=(), group_cols=(), aggs=(), qual_pushdown=True, expected_groups=0, float_cols=()):
     d = CgScanDesc()
     quals, tokens = flatten_where(quals)
@@ -251,10 +277,21 @@ def make_desc(quals=(), group_cols=(), aggs=(), qual_pushdown=True, expected_gro
     for i, t in enumerate(tokens):
         d.qual_expr[i] = t
     d.nquals = len(quals)
-    for i, (col, op, k) in enumerate(quals):
-        d.quals[i].column = col
-        d.quals[i].op = capi.CG_OP[op]
-        d.quals[i].konst = int(np.float64(k).view(np.int64)) if col in float_cols else int(k)
+    for i, atom in enumerate(quals):
+        _set_atom(d.quals[i], atom, float_cols)
+    pool = []
+    for i, a in enumerate(aggs):
+        if a.filter is None:
+            continue
+        ftok = _filter_tokens(a.filter, pool)
+        if len(pool) > capi.CG_MAX_FILTER_QUALS or len(ftok) > capi.CG_MAX_QEXPR:
+            raise capi.CitusGpuError(capi.CG_EUNSUPPORTED, "FILTER trees too large")
+        d.nfilter_expr[i] = len(ftok)
+        for j, t in enumerate(ftok):
+            d.filter_expr[i][j] = t
+    d.nfilter_quals = len(pool)
+    for i, atom in enumerate(pool):
+        _set_atom(d.filter_quals[i], atom, float_cols)
     d.enable_qual_pushdown = 1 if qual_pushdown else 0
     d.ngroup_cols = len(group_cols)
     for i, c in enumerate(group_cols):

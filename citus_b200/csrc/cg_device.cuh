@@ -146,25 +146,30 @@ __device__ __forceinline__ bool qual_true(int64_t v, int op, int64_t k, bool isf
  * are an AND-list.
  */
 template <int NCC>
-__device__ __forceinline__ bool eval_where(const KPlan &P, const int64_t (&v)[NCC], uint32_t nullmask)
+__device__ __forceinline__ uint32_t eval_atoms(const KPlan &P, const int64_t (&v)[NCC], uint32_t nullmask, int n, const uint8_t *col,
+											   const uint8_t *op, const int64_t *k, const int64_t *lo, const int64_t *hi, const uint8_t *neg)
 {
 	uint32_t truth = 0;
 #pragma unroll 1
-	for (int q = 0; q < P.nquals; q++)
+	for (int q = 0; q < n; q++)
 	{
-		int c = P.qcol[q];
+		int c = col[q];
 		bool isnull = (nullmask >> c) & 1u;
 		int64_t x = pick<NCC>(v, c);
-		bool t = P.isfloat[c] ? qual_true(x, P.qop[q], P.qk[q], true)
-							  : (((x >= P.qlo[q]) && (x <= P.qhi[q])) != (bool) P.qneg[q]);
+		bool t = P.isfloat[c] ? qual_true(x, op[q], k[q], true) : (((x >= lo[q]) && (x <= hi[q])) != (bool) neg[q]);
 		truth |= (uint32_t) (t && !isnull) << q;
 	}
-	if (P.nqexpr == 0) return truth == (1u << P.nquals) - 1u;
+	return truth;
+}
+
+/* a postfix tree over "is TRUE" bits of atoms */
+__device__ __forceinline__ bool eval_postfix(uint32_t truth, int n, const int8_t *expr)
+{
 	uint32_t st = 0;
 #pragma unroll 1
-	for (int i = 0; i < P.nqexpr; i++)
+	for (int i = 0; i < n; i++)
 	{
-		int t = P.qexpr[i];
+		int t = expr[i];
 		if (t >= 0) st = (st << 1) | ((truth >> t) & 1u);
 		else
 		{
@@ -173,6 +178,28 @@ __device__ __forceinline__ bool eval_where(const KPlan &P, const int64_t (&v)[NC
 		}
 	}
 	return st & 1u;
+}
+
+template <int NCC>
+__device__ __forceinline__ bool eval_where(const KPlan &P, const int64_t (&v)[NCC], uint32_t nullmask)
+{
+	uint32_t truth = eval_atoms<NCC>(P, v, nullmask, P.nquals, P.qcol, P.qop, P.qk, P.qlo, P.qhi, P.qneg);
+	if (P.nqexpr == 0) return truth == (1u << P.nquals) - 1u;
+	return eval_postfix(truth, P.nqexpr, P.qexpr);
+}
+
+/* aggregate FILTERs of a row that passed WHERE, same three-valued logic: bit a set = aggregate a has a filter and
+ * it is not TRUE, so the row is no input of a */
+template <int NCC>
+__device__ __forceinline__ uint32_t eval_filters(const KPlan &P, const int64_t (&v)[NCC], uint32_t nullmask)
+{
+	if (P.nfquals == 0) return 0u;
+	uint32_t truth = eval_atoms<NCC>(P, v, nullmask, P.nfquals, P.fcol, P.fop, P.fk, P.flo, P.fhi, P.fneg);
+	uint32_t rejected = 0;
+#pragma unroll 1
+	for (int a = 0; a < P.naggs; a++)
+		if (P.nfexpr[a] > 0 && !eval_postfix(truth, P.nfexpr[a], P.fexpr[a])) rejected |= 1u << a;
+	return rejected;
 }
 
 /* home slot of a key in the open-addressing table: Fibonacci (multiply-shift) hashing, one

@@ -1281,6 +1281,9 @@ extern "C" int cg_scan_relation(const CgRelation *rel, const CgScanDesc *desc, C
 	for (int a = 0; a < desc->naggs; a++)
 		for (int f = 0; f < desc->aggs[a].nfactors && f < 3; f++)
 			if (desc->aggs[a].column[f] >= 0 && desc->aggs[a].column[f] < rel->natts) need(desc->aggs[a].column[f]);
+	if (cg_desc_has_filters(desc))
+		for (int q = 0; q < desc->nfilter_quals && q < CG_MAX_FILTER_QUALS; q++)
+			if (desc->filter_quals[q].column >= 0 && desc->filter_quals[q].column < rel->natts) need(desc->filter_quals[q].column);
 	if (staged.empty()) need(0);   /* count(*) only: the reference still reads the first column's skip nodes; we read its chunk row counts */
 
 	KPlan plan;
@@ -1730,7 +1733,7 @@ extern "C" int cg_partial_fetch(CgPartial *p, int64_t capacity, int64_t *keys, u
 			int64_t hi = 0; uint64_t lo = 0; int64_t cnt = 0; int64_t mm = 0; double fs = 0;
 			switch (k.kind)
 			{
-				case CG_AGG_COUNT_STAR: cnt = rows; break;
+				case CG_AGG_COUNT_STAR: cnt = k.filt ? rows - (int64_t) w[k.nullword] : rows; break;
 				case CG_AGG_COUNT: cnt = rows - (int64_t) w[k.nullword]; break;
 				case CG_AGG_SUM:
 					cnt = rows - (int64_t) w[k.nullword];

@@ -166,7 +166,9 @@ struct KAgg
 						 * non-NULL inputs = rows in group (word 0) - this word */
 	int8_t ovchk;       /* integer term with no proven bound: every factor and product is checked for int64
 						 * overflow (CG_ERRFLAG_TERM_OVERFLOW) */
-	int8_t pad[2];
+	int8_t filt;        /* the aggregate has a FILTER: nullword counts the rows that gave no input (NULL input or
+						 * filter not TRUE); count(*) then gets a nullword of its own (count = rows - it) */
+	int8_t pad;
 	int64_t a[3];
 	int64_t b[3];
 	int64_t bound;      /* nlimbs == 1: every |term| must be <= bound */
@@ -232,7 +234,25 @@ struct KPlan
 	int32_t slices;
 	uint32_t slice_rows;
 	uint32_t max_cg_rows;         /* largest chunk group of the launch (host-known; 0 = unknown: no slicing) */
+	/* aggregate FILTER atoms in the form of the WHERE atoms (0 when no aggregate has a filter), and per aggregate
+	 * its postfix tree over them (0 tokens = no filter) */
+	int32_t nfquals;
+	uint8_t fcol[CG_MAX_FILTER_QUALS];
+	uint8_t fop[CG_MAX_FILTER_QUALS];
+	int64_t fk[CG_MAX_FILTER_QUALS];
+	int64_t flo[CG_MAX_FILTER_QUALS];
+	int64_t fhi[CG_MAX_FILTER_QUALS];
+	uint8_t fneg[CG_MAX_FILTER_QUALS];
+	int32_t nfexpr[CG_MAX_AGGS];
+	int8_t fexpr[CG_MAX_AGGS][CG_MAX_QEXPR];
 };
+
+static inline bool cg_desc_has_filters(const CgScanDesc *d)
+{
+	for (int a = 0; a < d->naggs && a < CG_MAX_AGGS; a++)
+		if (d->nfilter_expr[a] > 0) return true;
+	return false;
+}
 
 /* plan of the specialised kernel (cg_scan_fast.cu): column roles in fixed order
  * [range quals..., group key, summed columns...] */

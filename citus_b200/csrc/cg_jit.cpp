@@ -138,6 +138,7 @@ struct JitShape
 	int half[CG_MAX_AGGS];
 	int64_t bias[CG_MAX_AGGS];
 	int rows_partner = -1;            /* aggregate in the high half of cell 0 (whose low half counts the rows), -1 = none */
+	int ncell[CG_MAX_AGGS];           /* SMALL: cell of a filtered aggregate's no-input counter, -1 = none */
 	long long lane_rows_cap = (1ll << 22);
 	int min_blocks = 0;               /* __launch_bounds__ second argument, 0 = none */
 	size_t smem = 0;
@@ -161,6 +162,7 @@ static bool agg_has_value(const KAgg &g) { return g.kind != CG_AGG_COUNT_STAR &&
 static bool agg_two_limbs(const KAgg &g) { return g.kind == CG_AGG_SUM && !g.is_float && g.nlimbs == 2; }
 
 static std::string agg_null_expr(const KAgg &g, const JitShape &sh);
+static std::string agg_noinput_expr(const KPlan &plan, int a, const JitShape &sh);
 
 static void choose_shape(const KPlan &plan, uint32_t nullable, JitShape *sh)
 {
@@ -175,7 +177,7 @@ static void choose_shape(const KPlan &plan, uint32_t nullable, JitShape *sh)
 		if (r && (atoi(r) == 2 || atoi(r) == 4)) sh->R = atoi(r);
 		if (u && atoi(u) >= 1 && atoi(u) <= 4) sh->U = atoi(u);
 	}
-	for (int a = 0; a < CG_MAX_AGGS; a++) { sh->hot0[a] = -1; sh->lane1[a] = false; sh->half[a] = -1; sh->bias[a] = 0; }
+	for (int a = 0; a < CG_MAX_AGGS; a++) { sh->hot0[a] = -1; sh->lane1[a] = false; sh->half[a] = -1; sh->bias[a] = 0; sh->ncell[a] = -1; }
 	if (plan.mode == CG_MODE_DENSE)
 	{
 		static int narrow_on = -1;
@@ -197,7 +199,7 @@ static void choose_shape(const KPlan &plan, uint32_t nullable, JitShape *sh)
 			for (int i = 1; i < ncand; i++)
 			{
 				const int x = cand[i];
-				if (taken[x] || !agg_null_expr(plan.aggs[x], *sh).empty()) continue;
+				if (taken[x] || !agg_noinput_expr(plan, x, *sh).empty()) continue;
 				int y = -1;
 				for (int j = 1; j < ncand; j++) if (j != i && !taken[cand[j]]) { y = cand[j]; break; }
 				if (y < 0) break;
@@ -223,6 +225,9 @@ static void choose_shape(const KPlan &plan, uint32_t nullable, JitShape *sh)
 			else
 				nhot += 1;
 		}
+		/* rejected rows are common, not rare like NULL inputs: a filtered aggregate's no-input counter gets a cell too */
+		for (int a = 0; a < plan.naggs; a++)
+			if (plan.nfexpr[a] > 0) sh->ncell[a] = nhot++;
 		size_t bytes = (size_t) plan.capacity * nhot * sizeof(uint64_t) * JIT_THREADS;
 		if (plan.capacity <= 4096 && bytes <= 200 * 1024)
 		{
@@ -237,8 +242,8 @@ static void choose_shape(const KPlan &plan, uint32_t nullable, JitShape *sh)
 		}
 		else
 		{
-			/* not the shared-memory kind after all: no narrow cells */
-			for (int a = 0; a < CG_MAX_AGGS; a++) { sh->half[a] = -1; sh->bias[a] = 0; }
+			/* not the shared-memory kind after all: no narrow cells, the no-input counters stay in the table */
+			for (int a = 0; a < CG_MAX_AGGS; a++) { sh->half[a] = -1; sh->bias[a] = 0; sh->ncell[a] = -1; }
 			sh->rows_partner = -1;
 		}
 	}
@@ -296,7 +301,7 @@ static void gen_prelude(std::string &s)
 		"typedef unsigned long long uint64_t; typedef long long int64_t; typedef unsigned int uint32_t; typedef int int32_t;\n"
 		"typedef unsigned short uint16_t; typedef short int16_t; typedef unsigned char uint8_t; typedef signed char int8_t;\n"
 		"struct DevChunkCol { uint64_t values_off; uint64_t exists_off; uint64_t rank_off; uint32_t value_count; uint32_t row_count; };\n"
-		"struct KAgg { int8_t kind; int8_t nfactors; int8_t is_float; int8_t nlimbs; int8_t pcol[3]; int8_t word0; int8_t nullword; int8_t ovchk; int8_t pad[2];\n"
+		"struct KAgg { int8_t kind; int8_t nfactors; int8_t is_float; int8_t nlimbs; int8_t pcol[3]; int8_t word0; int8_t nullword; int8_t ovchk; int8_t filt; int8_t pad;\n"
 		"  int64_t a[3]; int64_t b[3]; int64_t bound; int64_t tbound; };\n";
 	addf(s,
 		 "struct KPlan { const uint8_t *arena; const DevChunkCol *chunkcols; const uint32_t *selected; uint32_t nselected; int32_t nstaged;\n"
@@ -306,9 +311,12 @@ static void gen_prelude(std::string &s)
 		 "  int32_t mode; int32_t nwords; int32_t stride; uint64_t *table; int64_t *hkeys; uint64_t capacity; int32_t hash_shift;\n"
 		 "  int64_t key_min; int64_t key_min1; uint64_t range1; uint8_t wordop[%d]; unsigned long long *stats;\n"
 		 "  int8_t hot_of_word[%d]; int32_t nhot; uint64_t *packed; int32_t pack_shift; int32_t pack_word;\n"
-		 "  int32_t nqexpr; int8_t qexpr[%d]; int32_t slices; uint32_t slice_rows; uint32_t max_cg_rows; };\n",
+		 "  int32_t nqexpr; int8_t qexpr[%d]; int32_t slices; uint32_t slice_rows; uint32_t max_cg_rows;\n"
+		 "  int32_t nfquals; uint8_t fcol[%d]; uint8_t fop[%d]; int64_t fk[%d]; int64_t flo[%d]; int64_t fhi[%d]; uint8_t fneg[%d];\n"
+		 "  int32_t nfexpr[%d]; int8_t fexpr[%d][%d]; };\n",
 		 CG_KMAX_COLS, CG_KMAX_COLS, CG_KMAX_COLS, CG_MAX_QUALS, CG_MAX_QUALS, CG_MAX_QUALS, CG_MAX_QUALS, CG_MAX_QUALS, CG_MAX_QUALS,
-		 CG_MAX_GROUP_COLS, CG_MAX_AGGS, CG_KMAX_WORDS, CG_KMAX_WORDS, CG_MAX_QEXPR);
+		 CG_MAX_GROUP_COLS, CG_MAX_AGGS, CG_KMAX_WORDS, CG_KMAX_WORDS, CG_MAX_QEXPR, CG_MAX_FILTER_QUALS, CG_MAX_FILTER_QUALS,
+		 CG_MAX_FILTER_QUALS, CG_MAX_FILTER_QUALS, CG_MAX_FILTER_QUALS, CG_MAX_FILTER_QUALS, CG_MAX_AGGS, CG_MAX_AGGS, CG_MAX_QEXPR);
 	/* the text above must describe the host's structs exactly */
 	addf(s, "static_assert(sizeof(DevChunkCol) == %zu, \"DevChunkCol\");\n", sizeof(DevChunkCol));
 	addf(s, "static_assert(sizeof(KAgg) == %zu, \"KAgg\");\n", sizeof(KAgg));
@@ -464,6 +472,51 @@ static std::string agg_null_expr(const KAgg &g, const JitShape &sh)
 	return e;
 }
 
+/* "aggregate a gives no input on this row" (NULL input, or its FILTER is not TRUE: f<a>), or "" when it always does */
+static std::string agg_noinput_expr(const KPlan &plan, int a, const JitShape &sh)
+{
+	const KAgg &g = plan.aggs[a];
+	std::string e = g.kind == CG_AGG_COUNT_STAR ? std::string() : agg_null_expr(g, sh);
+	if (plan.nfexpr[a] > 0) e += (e.empty() ? "!f" : " || !f") + std::to_string(a);
+	return e;
+}
+
+/* a postfix tree over the atoms <prefix><q> */
+static std::string tree_expr(int n, const int8_t *expr, const char *prefix)
+{
+	std::vector<std::string> st;
+	for (int i = 0; i < n; i++)
+	{
+		int t = expr[i];
+		if (t >= 0) st.push_back(prefix + std::to_string(t));
+		else
+		{
+			std::string b = st.back(); st.pop_back();
+			std::string a = st.back(); st.pop_back();
+			st.push_back("(" + a + (t == CG_QX_AND ? " && " : " || ") + b + ")");
+		}
+	}
+	return st.back();
+}
+
+/* one atom "column <op> constant" on plan column c, its constants in P.<arr>k / <arr>lo / <arr>hi / <arr>neg [q]; an atom
+ * on a NULL input is not TRUE (three-valued logic) */
+static std::string atom_expr(const KPlan &plan, const JitShape &sh, int c, int op, bool neg, const char *arr, int q)
+{
+	char buf[256], nn[32] = "";
+	if (col_nullable(sh, c)) snprintf(nn, sizeof nn, "!z%d && ", c);
+	if (plan.isfloat[c])
+	{
+		const char *ops[] = {"<", "<=", "==", ">=", ">", "!="};
+		snprintf(buf, sizeof buf, "%s(fcmp(v%d, P.%sk[%d]) %s 0)", nn, c, arr, q, ops[op]);
+	}
+	else if (neg)
+		snprintf(buf, sizeof buf, "%s!((v%d >= P.%slo[%d]) && (v%d <= P.%shi[%d]))", nn, c, arr, q, c, arr, q);
+	else
+		snprintf(buf, sizeof buf, "%s(v%d >= P.%slo[%d]) && (v%d <= P.%shi[%d])", nn, c, arr, q, c, arr, q);
+	return buf;
+}
+
 /* the WHERE tree over the atoms t<q> (an AND-list without a tree) */
 static std::string where_expr(const KPlan &plan)
 {
@@ -475,19 +528,7 @@ static std::string where_expr(const KPlan &plan)
 		for (int q = 0; q < plan.nquals; q++) { snprintf(buf, sizeof buf, "%st%d", q ? " && " : "", q); e += buf; }
 		return e;
 	}
-	std::vector<std::string> st;
-	for (int i = 0; i < plan.nqexpr; i++)
-	{
-		int t = plan.qexpr[i];
-		if (t >= 0) { snprintf(buf, sizeof buf, "t%d", t); st.push_back(buf); }
-		else
-		{
-			std::string b = st.back(); st.pop_back();
-			std::string a = st.back(); st.pop_back();
-			st.push_back("(" + a + (t == CG_QX_AND ? " && " : " || ") + b + ")");
-		}
-	}
-	return st.back();
+	return tree_expr(plan.nqexpr, plan.qexpr, "t");
 }
 
 /* updates of a group entry in global memory (`e` = its word pointer): the TABLE kind, and the NULL-key group of
@@ -510,7 +551,7 @@ static void gen_table_updates(std::string &s, const KPlan &plan, const JitShape 
 	for (int a = 0; a < plan.naggs; a++)
 	{
 		const KAgg &g = plan.aggs[a];
-		if (g.kind == CG_AGG_COUNT_STAR || (with_packed && a == sh.pack_agg)) continue;
+		if ((g.kind == CG_AGG_COUNT_STAR && an[a].empty()) || (with_packed && a == sh.pack_agg)) continue;
 		if (!an[a].empty()) addf(s, "%sif (an%d) red_add(e + %d, 1ull);\n", C, a, g.nullword);
 		if (!agg_has_value(g)) continue;
 		char p[32];
@@ -536,20 +577,12 @@ static void gen_row(std::string &s, const KPlan &plan, const JitShape &sh, int u
 	}
 	/* K3: the WHERE tree; an atom on a NULL input is not TRUE (three-valued logic) */
 	for (int q = 0; q < plan.nquals; q++)
-	{
-		int c = plan.qcol[q];
-		char nn[32] = "";
-		if (col_nullable(sh, c)) snprintf(nn, sizeof nn, "!z%d && ", c);
-		if (plan.isfloat[c])
-		{
-			const char *ops[] = {"<", "<=", "==", ">=", ">", "!="};
-			addf(s, "%sconst bool t%d = %s(fcmp(v%d, P.qk[%d]) %s 0);\n", T, q, nn, c, q, ops[plan.qop[q]]);
-		}
-		else if (plan.qneg[q])
-			addf(s, "%sconst bool t%d = %s!((v%d >= P.qlo[%d]) && (v%d <= P.qhi[%d]));\n", T, q, nn, c, q, c, q);
-		else
-			addf(s, "%sconst bool t%d = %s(v%d >= P.qlo[%d]) && (v%d <= P.qhi[%d]);\n", T, q, nn, c, q, c, q);
-	}
+		addf(s, "%sconst bool t%d = %s;\n", T, q, atom_expr(plan, sh, plan.qcol[q], plan.qop[q], plan.qneg[q], "q", q).c_str());
+	/* aggregate FILTERs: atoms u<q> of their own pool, f<a> = aggregate a's tree is TRUE */
+	for (int q = 0; q < plan.nfquals; q++)
+		addf(s, "%sconst bool u%d = %s;\n", T, q, atom_expr(plan, sh, plan.fcol[q], plan.fop[q], plan.fneg[q], "f", q).c_str());
+	for (int a = 0; a < plan.naggs; a++)
+		if (plan.nfexpr[a] > 0) addf(s, "%sconst bool f%d = %s;\n", T, a, tree_expr(plan.nfexpr[a], plan.fexpr[a], "u").c_str());
 	addf(s, "%sconst bool pass = %s;\n", T, where_expr(plan).c_str());
 	addf(s, "%sif (!pass) removed++;\n%selse {\n", T, T);
 	const char *B = "\t\t\t\t\t\t\t";
@@ -611,13 +644,12 @@ static void gen_row(std::string &s, const KPlan &plan, const JitShape &sh, int u
 		addf(s, "%sconst bool ok = true;\n", B);
 	addf(s, "%sif (ok) {\n", B);
 	const char *C = "\t\t\t\t\t\t\t\t";
-	/* NULL-input flags and terms */
+	/* no-input flags (NULL input, or FILTER not TRUE) and terms; a rejected row raises no error of its term */
 	std::vector<std::string> an(plan.naggs), w0v(plan.naggs);
 	for (int a = 0; a < plan.naggs; a++)
 	{
 		const KAgg &g = plan.aggs[a];
-		if (g.kind == CG_AGG_COUNT_STAR) continue;
-		an[a] = agg_null_expr(g, sh);
+		an[a] = agg_noinput_expr(plan, a, sh);
 		if (!an[a].empty()) addf(s, "%sconst bool an%d = %s;\n", C, a, an[a].c_str());
 		if (!agg_has_value(g)) continue;
 		std::string e = term_expr(g, a);
@@ -651,7 +683,6 @@ static void gen_row(std::string &s, const KPlan &plan, const JitShape &sh, int u
 		for (int a = 0; a < plan.naggs; a++)
 		{
 			const KAgg &g = plan.aggs[a];
-			if (g.kind == CG_AGG_COUNT_STAR) continue;
 			if (!an[a].empty()) addf(s, "%sif (an%d) g_n%d++;\n", C, a, a);
 			if (!agg_has_value(g)) continue;
 			char acc[32];
@@ -685,9 +716,14 @@ static void gen_row(std::string &s, const KPlan &plan, const JitShape &sh, int u
 		for (int a = 0; a < plan.naggs; a++)
 		{
 			const KAgg &g = plan.aggs[a];
-			if (g.kind == CG_AGG_COUNT_STAR) continue;
-			/* NULL-input counters stay on global reductions (rare) */
-			if (!an[a].empty()) addf(s, "%sif (an%d) red_add(P.table + slot * %dull + %d, 1ull);\n", D, a, plan.stride, g.nullword);
+			/* a filtered aggregate's no-input counter has a cell; the NULL-input counters of the others stay on global
+			 * reductions (rare) */
+			if (sh.ncell[a] >= 0)
+			{
+				std::string &ce = cellexpr[sh.ncell[a]];
+				ce = ce.empty() ? "(uint64_t) an" + std::to_string(a) : ce + " + (uint64_t) an" + std::to_string(a);
+			}
+			else if (!an[a].empty()) addf(s, "%sif (an%d) red_add(P.table + slot * %dull + %d, 1ull);\n", D, a, plan.stride, g.nullword);
 			if (!agg_has_value(g)) continue;
 			if (sh.half[a] >= 0)
 			{
@@ -738,7 +774,7 @@ static std::string gen_source(const KPlan &plan, const JitShape &sh)
 		for (int a = 0; a < plan.naggs; a++)
 		{
 			const KAgg &g = plan.aggs[a];
-			if (g.kind != CG_AGG_COUNT_STAR && !agg_null_expr(g, sh).empty()) addf(s, "\tuint64_t g_n%d = 0;\n", a);
+			if (!agg_noinput_expr(plan, a, sh).empty()) addf(s, "\tuint64_t g_n%d = 0;\n", a);
 			if (!agg_has_value(g)) continue;
 			addf(s, "\tuint64_t g_a%d_0 = %s, g_a%d_1 = 0;\n", a, op_identity(plan.wordop[g.word0]), a);
 		}
@@ -853,7 +889,7 @@ static std::string gen_source(const KPlan &plan, const JitShape &sh)
 		for (int a = 0; a < plan.naggs; a++)
 		{
 			const KAgg &g = plan.aggs[a];
-			if (g.kind != CG_AGG_COUNT_STAR && !agg_null_expr(g, sh).empty())
+			if (!agg_noinput_expr(plan, a, sh).empty())
 				addf(s, "\t{ uint64_t n = wsum(g_n%d); if ((tid & 31) == 0 && n) red_add(P.table + %d, n); }\n", a, g.nullword);
 			if (!agg_has_value(g)) continue;
 			int op = plan.wordop[g.word0];
@@ -907,6 +943,9 @@ static std::string gen_source(const KPlan &plan, const JitShape &sh)
 		for (int a = 0; a < plan.naggs; a++)
 		{
 			const KAgg &g = plan.aggs[a];
+			if (sh.ncell[a] >= 0)
+				addf(s, "\t\t\tcase %d: { uint64_t x = 0; for (uint32_t k = 0; k < %d; k++) x += col[(k + tid) %% %d]; if (x) red_add(ge + %d, x); break; }\n",
+					 sh.ncell[a], JIT_THREADS, JIT_THREADS, g.nullword);
 			if (!agg_has_value(g) || sh.half[a] >= 0) continue;
 			int op = plan.wordop[g.word0];
 			char p[32];
@@ -1096,7 +1135,7 @@ int cg_launch_scan_jit(CgContext *ctx, const KPlan &plan, uint32_t nullable, cud
 		/* nothing but the packed word is written when the plan is count(*) + the packed sum over NULL-free inputs */
 		bool only = true;
 		for (int a = 0; a < plan.naggs; a++)
-			if (plan.aggs[a].kind != CG_AGG_COUNT_STAR && a != sh.pack_agg) only = false;
+			if ((plan.aggs[a].kind != CG_AGG_COUNT_STAR && a != sh.pack_agg) || plan.nfexpr[a] > 0) only = false;
 		if (!agg_null_expr(plan.aggs[sh.pack_agg], sh).empty()) only = false;
 		*packed_only = only;
 	}

@@ -29,6 +29,33 @@ int cg_set_error(int code, const char *fmt, ...)
 
 extern "C" const char *cg_last_error(void) { return g_errbuf; }
 
+/* a postfix tree over atoms [0, natoms): every operator finds two operands, one value is left */
+static int validate_postfix(const char *what, const int8_t *expr, int n, int natoms)
+{
+	int depth = 0;
+	for (int i = 0; i < n; i++)
+	{
+		int t = expr[i];
+		if (t >= 0) { if (t >= natoms) return cg_set_error(CG_EINVAL, "%s refers to atom %d of %d", what, t, natoms); depth++; }
+		else if (t == CG_QX_AND || t == CG_QX_OR) { if (depth < 2) return cg_set_error(CG_EINVAL, "%s: operator without operands", what); depth--; }
+		else return cg_set_error(CG_EINVAL, "%s: bad token %d", what, t);
+	}
+	if (depth != 1) return cg_set_error(CG_EINVAL, "%s leaves %d values", what, depth);
+	return CG_OK;
+}
+
+static int validate_atoms(const char *what, const CgQual *quals, int n, int natts)
+{
+	for (int q = 0; q < n; q++)
+	{
+		if (quals[q].column < 0 || quals[q].column >= natts)
+			return cg_set_error(CG_EINVAL, "%s %d: column %d out of range", what, q, quals[q].column);
+		if (quals[q].op < CG_OP_LT || quals[q].op > CG_OP_NE)
+			return cg_set_error(CG_EINVAL, "%s %d: bad operator", what, q);
+	}
+	return CG_OK;
+}
+
 static int validate_desc(const CgScanDesc *d, const CgColumnDesc *columns, int natts)
 {
 	if (d->nquals < 0 || d->nquals > CG_MAX_QUALS) return cg_set_error(CG_EINVAL, "nquals %d out of range", d->nquals);
@@ -53,26 +80,19 @@ static int validate_desc(const CgScanDesc *d, const CgColumnDesc *columns, int n
 		if (columns[c].type_class == CG_TYPE_FLOAT && l != 4 && l != 8)
 			return cg_set_error(CG_EINVAL, "column %d: float with attlen %d", c, l);
 	}
-	for (int q = 0; q < d->nquals; q++)
-	{
-		if (d->quals[q].column < 0 || d->quals[q].column >= natts)
-			return cg_set_error(CG_EINVAL, "qual %d: column %d out of range", q, d->quals[q].column);
-		if (d->quals[q].op < CG_OP_LT || d->quals[q].op > CG_OP_NE)
-			return cg_set_error(CG_EINVAL, "qual %d: bad operator", q);
-	}
+	int rc = validate_atoms("qual", d->quals, d->nquals, natts);
+	if (rc) return rc;
 	if (d->nqual_expr < 0 || d->nqual_expr > CG_MAX_QEXPR) return cg_set_error(CG_EINVAL, "nqual_expr %d out of range", d->nqual_expr);
-	if (d->nqual_expr > 0)
+	if (d->nqual_expr > 0 && (rc = validate_postfix("qual_expr", d->qual_expr, d->nqual_expr, d->nquals))) return rc;
+	if (d->nfilter_quals < 0 || d->nfilter_quals > CG_MAX_FILTER_QUALS)
+		return cg_set_error(CG_EINVAL, "nfilter_quals %d out of range", d->nfilter_quals);
+	if ((rc = validate_atoms("filter qual", d->filter_quals, d->nfilter_quals, natts))) return rc;
+	for (int a = 0; a < CG_MAX_AGGS; a++)
 	{
-		/* well-formed postfix: every operator finds two operands, one value is left */
-		int depth = 0;
-		for (int i = 0; i < d->nqual_expr; i++)
-		{
-			int t = d->qual_expr[i];
-			if (t >= 0) { if (t >= d->nquals) return cg_set_error(CG_EINVAL, "qual_expr refers to atom %d of %d", t, d->nquals); depth++; }
-			else if (t == CG_QX_AND || t == CG_QX_OR) { if (depth < 2) return cg_set_error(CG_EINVAL, "qual_expr: operator without operands"); depth--; }
-			else return cg_set_error(CG_EINVAL, "qual_expr: bad token %d", t);
-		}
-		if (depth != 1) return cg_set_error(CG_EINVAL, "qual_expr leaves %d values", depth);
+		const int n = d->nfilter_expr[a];
+		if (n < 0 || n > CG_MAX_QEXPR) return cg_set_error(CG_EINVAL, "nfilter_expr[%d] = %d out of range", a, n);
+		if (n > 0 && a >= d->naggs) return cg_set_error(CG_EINVAL, "filter of aggregate %d of %d", a, d->naggs);
+		if (n > 0 && (rc = validate_postfix("filter_expr", d->filter_expr[a], n, d->nfilter_quals))) return rc;
 	}
 	for (int g = 0; g < d->ngroup_cols; g++)
 	{
@@ -113,6 +133,9 @@ static int validate_desc(const CgScanDesc *d, const CgColumnDesc *columns, int n
  * Counting the NULL inputs instead of the non-NULL ones keeps NULL-free data (the common
  * case) at one atomic per aggregate and row, while "no non-NULL input => SQL NULL" and
  * count(x) stay exact: non-NULL inputs = rows in group - NULL inputs.
+ * An aggregate with a FILTER counts in that word every row that gave no input (NULL input or
+ * filter not TRUE); a filtered count(*) gets one such ADD word (count = rows - it).  Every
+ * word stays additive or min/max, so combines and merges need not know about filters.
  */
 static int layout_partial(CgPartial *p, const CgColumnDesc *columns)
 {
@@ -134,10 +157,12 @@ static int layout_partial(CgPartial *p, const CgColumnDesc *columns)
 		 * range", numeric is exact): unless the caller proved a bound, the kernels check every factor and product */
 		k.ovchk = (int8_t) (!s.is_float && (s.kind == CG_AGG_SUM || s.kind == CG_AGG_MIN || s.kind == CG_AGG_MAX) &&
 							k.tbound == 0 && !(s.nfactors == 1 && s.a[0] == 0 && s.b[0] == 1));
+		k.filt = (int8_t) (d.nfilter_expr[a] > 0);
 		switch (s.kind)
 		{
 			case CG_AGG_COUNT_STAR:
 				k.word0 = 0;
+				if (k.filt) { k.nullword = (int8_t) nw; p->wordop[nw++] = CG_WORD_ADD; }
 				break;
 			case CG_AGG_COUNT:
 				k.word0 = (int8_t) nw; k.nullword = (int8_t) nw; p->wordop[nw++] = CG_WORD_ADD;
@@ -338,7 +363,7 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 	if (partial->desc.naggs != desc->naggs || partial->desc.ngroup_cols != desc->ngroup_cols)
 		return cg_set_error(CG_EINVAL, "partial aggregate was created for a different query shape");
 	for (int a = 0; a < desc->naggs; a++)
-		if (memcmp(&partial->desc.aggs[a], &desc->aggs[a], sizeof(CgAggSpec)) != 0)
+		if (memcmp(&partial->desc.aggs[a], &desc->aggs[a], sizeof(CgAggSpec)) != 0 || partial->aggs[a].filt != (desc->nfilter_expr[a] > 0))
 			return cg_set_error(CG_EINVAL, "partial aggregate was created for a different aggregate list");
 
 	memset(plan, 0, sizeof *plan);
@@ -365,6 +390,22 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 		dst = pc__;                                                                                 \
 	} while (0)
 
+	/* integer atoms in range form: pass iff ((x >= lo && x <= hi) != neg); float atoms keep op + constant (a float4
+	 * column's values are promoted to float8, the constant already is float8 bits) */
+	auto atom_range = [](const CgQual &q, int64_t *lo_out, int64_t *hi_out, uint8_t *neg_out) {
+		int64_t k = q.konst, lo = INT64_MIN, hi = INT64_MAX;
+		bool neg = false;
+		switch (q.op)
+		{
+			case CG_OP_LT: if (k == INT64_MIN) { lo = 1; hi = 0; } else hi = k - 1; break;
+			case CG_OP_LE: hi = k; break;
+			case CG_OP_EQ: lo = hi = k; break;
+			case CG_OP_GE: lo = k; break;
+			case CG_OP_GT: if (k == INT64_MAX) { lo = 1; hi = 0; } else lo = k + 1; break;
+			default: lo = hi = k; neg = true; break;
+		}
+		*lo_out = lo; *hi_out = hi; *neg_out = neg;
+	};
 	plan->nquals = desc->nquals;
 	for (int q = 0; q < desc->nquals; q++)
 	{
@@ -372,24 +413,7 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 		plan->qcol[q] = (uint8_t) pc;
 		plan->qop[q] = (uint8_t) desc->quals[q].op;
 		plan->qk[q] = desc->quals[q].konst;
-		{
-			int64_t k = desc->quals[q].konst, lo = INT64_MIN, hi = INT64_MAX;
-			bool neg = false;
-			switch (desc->quals[q].op)
-			{
-				case CG_OP_LT: if (k == INT64_MIN) { lo = 1; hi = 0; } else hi = k - 1; break;
-				case CG_OP_LE: hi = k; break;
-				case CG_OP_EQ: lo = hi = k; break;
-				case CG_OP_GE: lo = k; break;
-				case CG_OP_GT: if (k == INT64_MAX) { lo = 1; hi = 0; } else lo = k + 1; break;
-				default: lo = hi = k; neg = true; break;
-			}
-			plan->qlo[q] = lo; plan->qhi[q] = hi; plan->qneg[q] = neg;
-		}
-		if (columns[desc->quals[q].column].type_class == CG_TYPE_FLOAT && columns[desc->quals[q].column].attlen == 4)
-		{
-			/* float4 column values are promoted to float8; so is the constant (already float8 bits) */
-		}
+		atom_range(desc->quals[q], &plan->qlo[q], &plan->qhi[q], &plan->qneg[q]);
 	}
 	plan->slices = 1; plan->slice_rows = 1u << 30; plan->max_cg_rows = 0;
 	plan->nqexpr = desc->nqual_expr;
@@ -408,6 +432,24 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 		{
 			int pc; USE_OR_FAIL(pc, desc->aggs[a].column[f]);
 			plan->aggs[a].pcol[f] = (int8_t) pc;
+		}
+	}
+	if (cg_desc_has_filters(desc))
+	{
+		/* a column read only by a FILTER is a plan column like any other (projection, column limit) */
+		plan->nfquals = desc->nfilter_quals;
+		for (int q = 0; q < desc->nfilter_quals; q++)
+		{
+			int pc; USE_OR_FAIL(pc, desc->filter_quals[q].column);
+			plan->fcol[q] = (uint8_t) pc;
+			plan->fop[q] = (uint8_t) desc->filter_quals[q].op;
+			plan->fk[q] = desc->filter_quals[q].konst;
+			atom_range(desc->filter_quals[q], &plan->flo[q], &plan->fhi[q], &plan->fneg[q]);
+		}
+		for (int a = 0; a < desc->naggs; a++)
+		{
+			plan->nfexpr[a] = desc->nfilter_expr[a];
+			for (int i = 0; i < desc->nfilter_expr[a]; i++) plan->fexpr[a][i] = desc->filter_expr[a][i];
 		}
 	}
 	plan->ncols = ncols;
@@ -445,7 +487,7 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
  */
 bool cg_build_fast_plan(const CgScanDesc *desc, const KPlan &plan, bool all8, FPlan *fast)
 {
-	if (!all8 || plan.ngroup > 1 || plan.nqexpr != 0) return false;
+	if (!all8 || plan.ngroup > 1 || plan.nqexpr != 0 || plan.nfquals != 0) return false;
 	for (int c = 0; c < plan.ncols; c++) if (plan.isfloat[c]) return false;
 	memset(fast, 0, sizeof *fast);
 	bool used[CG_KMAX_COLS] = {false};

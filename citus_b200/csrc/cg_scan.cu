@@ -120,6 +120,9 @@ __device__ __forceinline__ void process_row(const KPlan &P, const int64_t (&v)[N
 	else
 		acc.rows++;
 
+	/* aggregate FILTERs: a rejected row is no input of its aggregate, counted like a NULL input */
+	const uint32_t rejected = eval_filters<NCC>(P, v, nullmask);
+
 	/* K4: transition functions */
 #pragma unroll
 	for (int a = 0; a < NAC; a++)
@@ -127,8 +130,16 @@ __device__ __forceinline__ void process_row(const KPlan &P, const int64_t (&v)[N
 		if (a < P.naggs)
 		{
 			const KAgg &g = P.aggs[a];
-			if (g.kind == CG_AGG_COUNT_STAR) continue;
-			bool isnull = false;
+			bool isnull = (rejected >> a) & 1u;
+			if (g.kind == CG_AGG_COUNT_STAR)
+			{
+				if (isnull)
+				{
+					if (MODE == CG_MODE_GLOBAL) acc.w[a][2]++;
+					else atomicAdd((unsigned long long *) entry + g.nullword, 1ull);
+				}
+				continue;
+			}
 			int64_t it = 1;
 			double ft = 1.0;
 #pragma unroll
@@ -325,7 +336,7 @@ cg_scan_kernel(const __grid_constant__ KPlan P)
 #pragma unroll
 		for (int a = 0; a < NAC; a++)
 		{
-			if (a < P.naggs && P.aggs[a].kind != CG_AGG_COUNT_STAR)
+			if (a < P.naggs && (P.aggs[a].kind != CG_AGG_COUNT_STAR || P.aggs[a].filt))
 			{
 				const KAgg &g = P.aggs[a];
 				uint64_t nulls = warp_reduce_word(acc.w[a][2], CG_WORD_ADD);
@@ -334,7 +345,7 @@ cg_scan_kernel(const __grid_constant__ KPlan P)
 				if ((tid & 31) == 0)
 				{
 					if (nulls) atomicAdd((unsigned long long *) P.table + g.nullword, (unsigned long long) nulls);
-					if (g.kind != CG_AGG_COUNT)
+					if (g.kind != CG_AGG_COUNT && g.kind != CG_AGG_COUNT_STAR)
 					{
 						if (x0 != word_identity(P.wordop[g.word0])) word_apply_global(P.table + g.word0, P.wordop[g.word0], x0);
 						if (g.kind == CG_AGG_SUM && !g.is_float && g.nlimbs == 2 && x1)

@@ -72,7 +72,8 @@ __device__ __forceinline__ bool eval_quals(const KPlan &P, const int64_t (&v)[NC
 template <int NCC>
 __device__ __forceinline__ void eval_terms(const KPlan &P, const int64_t (&v)[NCC], uint32_t nullmask, RowTerms<NCC> &t)
 {
-	t.nullbits = 0;
+	/* a row an aggregate's FILTER rejects is no input of it, like a NULL input */
+	t.nullbits = eval_filters<NCC>(P, v, nullmask);
 #pragma unroll
 	for (int a = 0; a < CG_MAX_AGGS; a++)
 	{
@@ -81,7 +82,7 @@ __device__ __forceinline__ void eval_terms(const KPlan &P, const int64_t (&v)[NC
 		{
 			const KAgg &g = P.aggs[a];
 			if (g.kind == CG_AGG_COUNT_STAR) continue;
-			bool isnull = false;
+			bool isnull = (t.nullbits >> a) & 1u;
 			int64_t it = 1;
 			double ft = 1.0;
 #pragma unroll
@@ -133,9 +134,8 @@ __device__ __forceinline__ void small_accumulate(const KPlan &P, uint64_t *mine,
 			if (a < P.naggs)
 			{
 				const KAgg &g = P.aggs[a];
-				if (g.kind == CG_AGG_COUNT_STAR) continue;
 				if ((t.nullbits >> a) & 1u) { atomicAdd((unsigned long long *) ge + g.nullword, 1ull); continue; }
-				if (g.kind == CG_AGG_COUNT) continue;
+				if (g.kind == CG_AGG_COUNT_STAR || g.kind == CG_AGG_COUNT) continue;
 				word_apply_global(ge + g.word0, P.wordop[g.word0], t.w0[a]);
 				if (g.kind == CG_AGG_SUM && !g.is_float && g.nlimbs == 2)
 					atomicAdd((unsigned long long *) ge + g.word0 + 1, (unsigned long long) t.w1[a]);
@@ -149,13 +149,14 @@ __device__ __forceinline__ void small_accumulate(const KPlan &P, uint64_t *mine,
 		if (a < P.naggs)
 		{
 			const KAgg &g = P.aggs[a];
-			if (g.kind == CG_AGG_COUNT_STAR) continue;
 			if ((t.nullbits >> a) & 1u)
 			{
-				atomicAdd((unsigned long long *) P.table + (uint64_t) slot * (uint64_t) P.stride + g.nullword, 1ull);
+				/* a filtered aggregate's no-input counter has a cell (rejected rows are common) */
+				if (g.filt) e[P.hot_of_word[g.nullword] * CGS_THREADS] += 1ull;
+				else atomicAdd((unsigned long long *) P.table + (uint64_t) slot * (uint64_t) P.stride + g.nullword, 1ull);
 				continue;
 			}
-			if (g.kind == CG_AGG_COUNT) continue;
+			if (g.kind == CG_AGG_COUNT_STAR || g.kind == CG_AGG_COUNT) continue;
 			uint64_t *w = e + P.hot_of_word[g.word0] * CGS_THREADS;
 			if (g.kind == CG_AGG_SUM && !g.is_float)
 			{
@@ -306,7 +307,8 @@ static int launch_small_variant(CgContext *ctx, const KPlan &plan, size_t smem, 
 	return CG_OK;
 }
 
-/* the words that get per-lane cells: word 0 and every aggregate's value words */
+/* the words that get per-lane cells: word 0, every aggregate's value words and the no-input counters of filtered
+ * aggregates */
 static int hot_words(const KPlan &plan, int8_t *hot)
 {
 	bool is_hot[CG_KMAX_WORDS] = {false};
@@ -314,6 +316,7 @@ static int hot_words(const KPlan &plan, int8_t *hot)
 	for (int a = 0; a < plan.naggs; a++)
 	{
 		const KAgg &g = plan.aggs[a];
+		if (g.filt) is_hot[g.nullword] = true;
 		if (g.kind == CG_AGG_COUNT_STAR || g.kind == CG_AGG_COUNT) continue;
 		is_hot[g.word0] = true;
 		if (g.kind == CG_AGG_SUM && !g.is_float && g.nlimbs == 2) is_hot[g.word0 + 1] = true;

@@ -44,7 +44,8 @@ extern "C" int cg_partial_merge_values(CgPartial *p, int64_t nrows, const int64_
 		bool exact = false;
 		for (int a = 0; a < na && !exact; a++)
 		{
-			if (p->aggs[a].kind == CG_AGG_COUNT_STAR) { rows = count[i * na + a]; exact = true; }
+			/* a filtered count(*) is one more candidate, not the group's row count */
+			if (p->aggs[a].kind == CG_AGG_COUNT_STAR && !p->aggs[a].filt) { rows = count[i * na + a]; exact = true; }
 			else if (count[i * na + a] > rows) rows = count[i * na + a];
 		}
 		if (rows < 0) return cg_set_error(CG_EINVAL, "negative count in partial row %lld", (long long) i);
@@ -53,10 +54,10 @@ extern "C" int cg_partial_merge_values(CgPartial *p, int64_t nrows, const int64_
 		{
 			const KAgg &k = p->aggs[a];
 			const int64_t c = count[i * na + a];
-			if (k.kind == CG_AGG_COUNT_STAR) continue;
+			if (k.kind == CG_AGG_COUNT_STAR && !k.filt) continue;
 			if (c < 0 || c > rows) return cg_set_error(CG_EINVAL, "count of aggregate %d exceeds the group's rows in partial row %lld", a, (long long) i);
 			w[k.nullword] = (uint64_t) (rows - c);
-			if (k.kind == CG_AGG_COUNT || c == 0) continue;
+			if (k.kind == CG_AGG_COUNT_STAR || k.kind == CG_AGG_COUNT || c == 0) continue;
 			if (k.kind == CG_AGG_SUM)
 			{
 				if (k.is_float)

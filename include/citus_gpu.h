@@ -208,6 +208,7 @@ typedef struct CgAggSpec
 #define CG_MAX_QEXPR 16
 #define CG_QX_AND (-1)
 #define CG_QX_OR (-2)
+#define CG_MAX_FILTER_QUALS 8
 
 typedef struct CgScanDesc
 {
@@ -226,6 +227,20 @@ typedef struct CgScanDesc
 	int32_t nqual_expr;
 	int8_t qual_expr[CG_MAX_QEXPR];
 	int32_t reserved;
+	/* Aggregate FILTER (WHERE ...) clauses ([PG] Aggref.aggfilter; the worker aggregate keeps the filter,
+	 * multi_logical_optimizer.c:3279-3280, 3479).  The atoms filter_quals[0..nfilter_quals) are a pool of their own:
+	 * they never take part in WHERE or in chunk-group skipping (SelectedChunkMask sees the scan's quals only), and
+	 * cg_relation_bounds ignores them.  Aggregate a's filter is the postfix tree filter_expr[a][0..nfilter_expr[a]) over
+	 * that pool, in the qual_expr token language; nfilter_expr[a] = 0 = no filter, so a zero-filled tail is a query
+	 * without filters.  A row that passes WHERE joins its group whatever the filters say; it is an input of aggregate
+	 * a only when a's tree is TRUE under three-valued logic (an atom on a NULL column is not TRUE), and a rejected
+	 * row's argument is not evaluated: it raises neither the int64 overflow nor the term_abs_bound error.  So a group
+	 * without accepted rows has count(*) / count(x) = 0 and sum / min / max = NULL (count 0).  A column read only by a
+	 * filter is staged and counts toward the query's column limit. */
+	int32_t nfilter_quals;
+	CgQual filter_quals[CG_MAX_FILTER_QUALS];
+	int32_t nfilter_expr[CG_MAX_AGGS];
+	int8_t filter_expr[CG_MAX_AGGS][CG_MAX_QEXPR];
 } CgScanDesc;
 
 /* EXPLAIN ANALYZE counters (columnar_customscan.c:1966-1999 and ExecScan instrumentation) */

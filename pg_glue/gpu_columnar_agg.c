@@ -200,9 +200,11 @@ translate_atom(OpExpr *op, TupleDesc tupdesc, CgQual *qual)
 	return true;
 }
 
-/* WHERE tree -> atoms + postfix tokens (CgScanDesc.qual_expr); false when a node is not AND / OR / atom or the tree is too big */
+/* boolean tree -> atoms appended to atoms[0 .. *natoms) (at most max_atoms) + postfix tokens appended to tokens[0 .. *ntokens)
+ * (at most CG_MAX_QEXPR): the WHERE list (quals / qual_expr) and aggregate FILTERs (filter_quals / filter_expr[a]).  false
+ * when a node is not AND / OR / atom or the tree is too big */
 static bool
-translate_where(Node *node, TupleDesc tupdesc, CgScanDesc *desc)
+translate_where(Node *node, TupleDesc tupdesc, CgQual *atoms, int32_t *natoms, int max_atoms, int8_t *tokens, int32_t *ntokens)
 {
 	if (IsA(node, BoolExpr))
 	{
@@ -213,22 +215,22 @@ translate_where(Node *node, TupleDesc tupdesc, CgScanDesc *desc)
 		int n = 0;
 		foreach(lc, b->args)
 		{
-			if (!translate_where((Node *) lfirst(lc), tupdesc, desc))
+			if (!translate_where((Node *) lfirst(lc), tupdesc, atoms, natoms, max_atoms, tokens, ntokens))
 				return false;
 			if (n++ > 0)
 			{
-				if (desc->nqual_expr >= CG_MAX_QEXPR)
+				if (*ntokens >= CG_MAX_QEXPR)
 					return false;
-				desc->qual_expr[desc->nqual_expr++] = b->boolop == AND_EXPR ? CG_QX_AND : CG_QX_OR;
+				tokens[(*ntokens)++] = b->boolop == AND_EXPR ? CG_QX_AND : CG_QX_OR;
 			}
 		}
 		return n > 0;
 	}
-	if (!IsA(node, OpExpr) || desc->nquals >= CG_MAX_QUALS || desc->nqual_expr >= CG_MAX_QEXPR)
+	if (!IsA(node, OpExpr) || *natoms >= max_atoms || *ntokens >= CG_MAX_QEXPR)
 		return false;
-	if (!translate_atom((OpExpr *) node, tupdesc, &desc->quals[desc->nquals]))
+	if (!translate_atom((OpExpr *) node, tupdesc, &atoms[*natoms]))
 		return false;
-	desc->qual_expr[desc->nqual_expr++] = (int8_t) desc->nquals++;
+	tokens[(*ntokens)++] = (int8_t) (*natoms)++;
 	return true;
 }
 
@@ -236,11 +238,19 @@ translate_where(Node *node, TupleDesc tupdesc, CgScanDesc *desc)
 static bool
 translate_aggref(Aggref *agg, TupleDesc tupdesc, CgScanDesc *desc, GpuOutColumn *out)
 {
-	if (agg->aggdistinct != NIL || agg->aggorder != NIL || agg->aggfilter != NULL || agg->aggkind != 'n' || desc->naggs >= CG_MAX_AGGS)
+	if (agg->aggdistinct != NIL || agg->aggorder != NIL || agg->aggkind != 'n' || desc->naggs >= CG_MAX_AGGS)
 		return false;
 	const char *name = get_func_name(agg->aggfnoid);
 	CgAggSpec *spec = &desc->aggs[desc->naggs];
 	memset(spec, 0, sizeof *spec);
+	/* FILTER (WHERE ...): the worker aggregate keeps it (multi_logical_optimizer.c:3279-3280, 3479), so it is evaluated
+	 * here, into the filter atom pool; a filter the atom language cannot express keeps the reference's executor.  (avg's
+	 * sum and count parts are one aggregate here: its non-NULL count rides along with the sum, under the same filter.) */
+	desc->nfilter_expr[desc->naggs] = 0;
+	if (agg->aggfilter != NULL &&
+		!translate_where((Node *) agg->aggfilter, tupdesc, desc->filter_quals, &desc->nfilter_quals, CG_MAX_FILTER_QUALS,
+						 desc->filter_expr[desc->naggs], &desc->nfilter_expr[desc->naggs]))
+		return false;
 	out->index = desc->naggs;
 	out->scale = 0;
 	if (agg->aggstar && strcmp(name, "count") == 0)
@@ -310,7 +320,8 @@ translate_query(PlannerInfo *root, RelOptInfo *input_rel, GpuAggPlan *plan)
 	foreach(lc, input_rel->baserestrictinfo)
 	{
 		RestrictInfo *ri = (RestrictInfo *) lfirst(lc);
-		if (!(ok = translate_where((Node *) ri->clause, tupdesc, &plan->desc)))
+		if (!(ok = translate_where((Node *) ri->clause, tupdesc, plan->desc.quals, &plan->desc.nquals, CG_MAX_QUALS, plan->desc.qual_expr,
+								   &plan->desc.nqual_expr)))
 			break;
 		if (nclauses++ > 0)
 		{
