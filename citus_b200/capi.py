@@ -20,7 +20,9 @@ CG_COMM_SUM, CG_COMM_MIN, CG_COMM_MAX = 0, 1, 2
 CG_TYPE_INT, CG_TYPE_FLOAT = 0, 1
 CG_OP = {"<": 0, "<=": 1, "=": 2, ">=": 3, ">": 4, "<>": 5}
 CG_AGG_COUNT_STAR, CG_AGG_COUNT, CG_AGG_SUM, CG_AGG_MIN, CG_AGG_MAX = range(5)
+CG_AGG_BIT_AND, CG_AGG_BIT_OR, CG_AGG_BOOL_AND, CG_AGG_BOOL_OR = range(5, 9)
 CG_WORD_ADD, CG_WORD_MIN, CG_WORD_MAX, CG_WORD_FADD, CG_WORD_FMIN, CG_WORD_FMAX = range(6)
+CG_WORD_AND, CG_WORD_OR = 6, 7
 CG_GEN_UNIFORM, CG_GEN_SEQUENCE = 0, 1
 CG_MAX_QUALS, CG_MAX_AGGS, CG_MAX_GROUP_COLS = 8, 8, 2
 CG_MAX_QEXPR, CG_QX_AND, CG_QX_OR = 16, -1, -2
@@ -76,7 +78,8 @@ class CgScanDesc(C.Structure):
                 ("aggs", CgAggSpec * CG_MAX_AGGS), ("expected_groups", C.c_int64),
                 ("nqual_expr", C.c_int32), ("qual_expr", C.c_int8 * CG_MAX_QEXPR), ("reserved", C.c_int32),
                 ("nfilter_quals", C.c_int32), ("filter_quals", CgQual * CG_MAX_FILTER_QUALS),
-                ("nfilter_expr", C.c_int32 * CG_MAX_AGGS), ("filter_expr", (C.c_int8 * CG_MAX_QEXPR) * CG_MAX_AGGS)]
+                ("nfilter_expr", C.c_int32 * CG_MAX_AGGS), ("filter_expr", (C.c_int8 * CG_MAX_QEXPR) * CG_MAX_AGGS),
+                ("narg_expr", C.c_int32 * CG_MAX_AGGS), ("arg_expr", (C.c_int8 * CG_MAX_QEXPR) * CG_MAX_AGGS)]
 
 
 class CgScanStats(C.Structure):

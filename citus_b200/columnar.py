@@ -198,6 +198,7 @@ class Agg:
     is_float: bool = False
     term_abs_bound: int = 0
     filter: object = None        # FILTER (WHERE ...): a WHERE-style tree of (column, op, constant) atoms, None = none
+    arg: object = None           # bool_and / bool_or: the predicate argument, a tree in the same form as `filter`
 
 
 def count_star(filter=None):
@@ -218,6 +219,24 @@ def min_(col, is_float=False, filter=None):
 
 def max_(col, is_float=False, filter=None):
     return Agg(CG_AGG_MAX, [(col, 0, 1)], is_float, filter=filter)
+
+
+def bit_and(col, filter=None):
+    """bit_and(col) over an int2 / int4 / int8 column: the value comes back sign-extended in minmax"""
+    return Agg(capi.CG_AGG_BIT_AND, [(col, 0, 1)], filter=filter)
+
+
+def bit_or(col, filter=None):
+    return Agg(capi.CG_AGG_BIT_OR, [(col, 0, 1)], filter=filter)
+
+
+def bool_and(tree, filter=None):
+    """bool_and(p) (and every(p)) of a predicate tree in the WHERE form: minmax 0 / 1, count = rows whose p is known"""
+    return Agg(capi.CG_AGG_BOOL_AND, filter=filter, arg=tree)
+
+
+def bool_or(tree, filter=None):
+    return Agg(capi.CG_AGG_BOOL_OR, filter=filter, arg=tree)
 
 
 def flatten_where(where):
@@ -279,16 +298,18 @@ def make_desc(quals=(), group_cols=(), aggs=(), qual_pushdown=True, expected_gro
     d.nquals = len(quals)
     for i, atom in enumerate(quals):
         _set_atom(d.quals[i], atom, float_cols)
-    pool = []
+    pool = []                    # FILTERs and bool_and / bool_or arguments share one atom pool
     for i, a in enumerate(aggs):
-        if a.filter is None:
-            continue
-        ftok = _filter_tokens(a.filter, pool)
-        if len(pool) > capi.CG_MAX_FILTER_QUALS or len(ftok) > capi.CG_MAX_QEXPR:
-            raise capi.CitusGpuError(capi.CG_EUNSUPPORTED, "FILTER trees too large")
-        d.nfilter_expr[i] = len(ftok)
-        for j, t in enumerate(ftok):
-            d.filter_expr[i][j] = t
+        for tree, n, expr, what in ((a.filter, d.nfilter_expr, d.filter_expr, "FILTER"),
+                                    (getattr(a, "arg", None), d.narg_expr, d.arg_expr, "bool_and / bool_or argument")):
+            if tree is None:
+                continue
+            tok = _filter_tokens(tree, pool)
+            if len(pool) > capi.CG_MAX_FILTER_QUALS or len(tok) > capi.CG_MAX_QEXPR:
+                raise capi.CitusGpuError(capi.CG_EUNSUPPORTED, f"{what} trees too large")
+            n[i] = len(tok)
+            for j, t in enumerate(tok):
+                expr[i][j] = t
     d.nfilter_quals = len(pool)
     for i, atom in enumerate(pool):
         _set_atom(d.filter_quals[i], atom, float_cols)

@@ -147,9 +147,10 @@ __device__ __forceinline__ bool qual_true(int64_t v, int op, int64_t k, bool isf
  */
 template <int NCC>
 __device__ __forceinline__ uint32_t eval_atoms(const KPlan &P, const int64_t (&v)[NCC], uint32_t nullmask, int n, const uint8_t *col,
-											   const uint8_t *op, const int64_t *k, const int64_t *lo, const int64_t *hi, const uint8_t *neg)
+											   const uint8_t *op, const int64_t *k, const int64_t *lo, const int64_t *hi, const uint8_t *neg,
+											   uint32_t *falsity = nullptr)
 {
-	uint32_t truth = 0;
+	uint32_t truth = 0, fals = 0;
 #pragma unroll 1
 	for (int q = 0; q < n; q++)
 	{
@@ -158,12 +159,15 @@ __device__ __forceinline__ uint32_t eval_atoms(const KPlan &P, const int64_t (&v
 		int64_t x = pick<NCC>(v, c);
 		bool t = P.isfloat[c] ? qual_true(x, op[q], k[q], true) : (((x >= lo[q]) && (x <= hi[q])) != (bool) neg[q]);
 		truth |= (uint32_t) (t && !isnull) << q;
+		fals |= (uint32_t) (!t && !isnull) << q;
 	}
+	if (falsity) *falsity = fals;
 	return truth;
 }
 
-/* a postfix tree over "is TRUE" bits of atoms */
-__device__ __forceinline__ bool eval_postfix(uint32_t truth, int n, const int8_t *expr)
+/* a postfix tree over "is TRUE" bits of atoms.  The second rail of three-valued logic: with `dual` and the "is FALSE"
+ * bits, the same tree with AND and OR swapped is "the tree is FALSE" (De Morgan); neither = UNKNOWN */
+__device__ __forceinline__ bool eval_postfix(uint32_t truth, int n, const int8_t *expr, bool dual = false)
 {
 	uint32_t st = 0;
 #pragma unroll 1
@@ -174,7 +178,7 @@ __device__ __forceinline__ bool eval_postfix(uint32_t truth, int n, const int8_t
 		else
 		{
 			uint32_t b = st & 1u, a = (st >> 1) & 1u;
-			st = ((st >> 2) << 1) | (t == CG_QX_AND ? (a & b) : (a | b));
+			st = ((st >> 2) << 1) | (((t == CG_QX_AND) != dual) ? (a & b) : (a | b));
 		}
 	}
 	return st & 1u;
@@ -189,16 +193,29 @@ __device__ __forceinline__ bool eval_where(const KPlan &P, const int64_t (&v)[NC
 }
 
 /* aggregate FILTERs of a row that passed WHERE, same three-valued logic: bit a set = aggregate a has a filter and
- * it is not TRUE, so the row is no input of a */
+ * it is not TRUE, or (bool_and / bool_or) its predicate argument is UNKNOWN, so the row is no input of a.  Bit a of
+ * *argtrue = the predicate argument of aggregate a is TRUE. */
 template <int NCC>
-__device__ __forceinline__ uint32_t eval_filters(const KPlan &P, const int64_t (&v)[NCC], uint32_t nullmask)
+__device__ __forceinline__ uint32_t eval_filters(const KPlan &P, const int64_t (&v)[NCC], uint32_t nullmask, uint32_t *argtrue = nullptr)
 {
+	if (argtrue) *argtrue = 0u;
 	if (P.nfquals == 0) return 0u;
-	uint32_t truth = eval_atoms<NCC>(P, v, nullmask, P.nfquals, P.fcol, P.fop, P.fk, P.flo, P.fhi, P.fneg);
-	uint32_t rejected = 0;
+	uint32_t fals = 0;
+	uint32_t truth = eval_atoms<NCC>(P, v, nullmask, P.nfquals, P.fcol, P.fop, P.fk, P.flo, P.fhi, P.fneg, &fals);
+	uint32_t rejected = 0, at = 0;
 #pragma unroll 1
 	for (int a = 0; a < P.naggs; a++)
+	{
 		if (P.nfexpr[a] > 0 && !eval_postfix(truth, P.nfexpr[a], P.fexpr[a])) rejected |= 1u << a;
+		if (P.nargexpr[a] > 0)
+		{
+			const bool t = eval_postfix(truth, P.nargexpr[a], P.argexpr[a]);
+			const bool f = eval_postfix(fals, P.nargexpr[a], P.argexpr[a], true);
+			if (!t && !f) rejected |= 1u << a;
+			at |= (uint32_t) t << a;
+		}
+	}
+	if (argtrue) *argtrue = at;
 	return rejected;
 }
 
@@ -267,17 +284,21 @@ __device__ __forceinline__ void word_apply_global(uint64_t *p, int op, uint64_t 
 		case CG_WORD_MAX: atomicMax((long long *) p, (long long) val); break;
 		case CG_WORD_FADD: atomicAdd((double *) p, __longlong_as_double((long long) val)); break;
 		case CG_WORD_FMIN: atomicMin((unsigned long long *) p, (unsigned long long) val); break;
+		case CG_WORD_AND: atomicAnd((unsigned long long *) p, (unsigned long long) val); break;
+		case CG_WORD_OR: atomicOr((unsigned long long *) p, (unsigned long long) val); break;
 		default: atomicMax((unsigned long long *) p, (unsigned long long) val); break;
 	}
 }
 
-__device__ __forceinline__ uint64_t word_identity(int op)
+__host__ __device__ __forceinline__ uint64_t word_identity(int op)
 {
 	switch (op)
 	{
 		case CG_WORD_MIN: return (uint64_t) INT64_MAX;
 		case CG_WORD_MAX: return (uint64_t) INT64_MIN;
 		case CG_WORD_FMIN: return ~0ull;
+		case CG_WORD_AND: return ~0ull;
+		case CG_WORD_OR: return 0ull;
 		default: return 0ull;     /* ADD, FADD (+0.0), FMAX */
 	}
 }
@@ -291,6 +312,8 @@ __device__ __forceinline__ uint64_t word_combine(int op, uint64_t a, uint64_t b)
 		case CG_WORD_MAX: return (uint64_t) max((long long) a, (long long) b);
 		case CG_WORD_FADD: return (uint64_t) __double_as_longlong(__longlong_as_double((long long) a) + __longlong_as_double((long long) b));
 		case CG_WORD_FMIN: return a < b ? a : b;
+		case CG_WORD_AND: return a & b;
+		case CG_WORD_OR: return a | b;
 		default: return a > b ? a : b;
 	}
 }

@@ -1281,7 +1281,7 @@ extern "C" int cg_scan_relation(const CgRelation *rel, const CgScanDesc *desc, C
 	for (int a = 0; a < desc->naggs; a++)
 		for (int f = 0; f < desc->aggs[a].nfactors && f < 3; f++)
 			if (desc->aggs[a].column[f] >= 0 && desc->aggs[a].column[f] < rel->natts) need(desc->aggs[a].column[f]);
-	if (cg_desc_has_filters(desc))
+	if (cg_desc_uses_pool(desc))
 		for (int q = 0; q < desc->nfilter_quals && q < CG_MAX_FILTER_QUALS; q++)
 			if (desc->filter_quals[q].column >= 0 && desc->filter_quals[q].column < rel->natts) need(desc->filter_quals[q].column);
 	if (staged.empty()) need(0);   /* count(*) only: the reference still reads the first column's skip nodes; we read its chunk row counts */
@@ -1745,6 +1745,17 @@ extern "C" int cg_partial_fetch(CgPartial *p, int64_t capacity, int64_t *keys, u
 						else s = (__int128) (unsigned __int128) w[k.word0] + ((__int128) (int64_t) w[k.word0 + 1] << 32);
 						hi = (int64_t) (s >> 64); lo = (uint64_t) s;
 					}
+					break;
+				case CG_AGG_BIT_AND:
+				case CG_AGG_BIT_OR:
+					cnt = rows - (int64_t) w[k.nullword];
+					mm = (int64_t) w[k.word0];
+					break;
+				case CG_AGG_BOOL_AND:
+				case CG_AGG_BOOL_OR:
+					/* the truth value is bit 0 (an input TRUE contributes ~0) */
+					cnt = rows - (int64_t) w[k.nullword];
+					mm = (int64_t) (w[k.word0] & 1ull);
 					break;
 				default:
 					cnt = rows - (int64_t) w[k.nullword];

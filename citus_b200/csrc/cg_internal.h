@@ -168,7 +168,8 @@ struct KAgg
 						 * overflow (CG_ERRFLAG_TERM_OVERFLOW) */
 	int8_t filt;        /* the aggregate has a FILTER: nullword counts the rows that gave no input (NULL input or
 						 * filter not TRUE); count(*) then gets a nullword of its own (count = rows - it) */
-	int8_t pad;
+	int8_t barg;        /* bool_and / bool_or: the argument is the predicate tree argexpr[a] over the filter pool;
+						 * nullword counts the rows that gave no input (argument UNKNOWN, or FILTER not TRUE) */
 	int64_t a[3];
 	int64_t b[3];
 	int64_t bound;      /* nlimbs == 1: every |term| must be <= bound */
@@ -245,6 +246,11 @@ struct KPlan
 	uint8_t fneg[CG_MAX_FILTER_QUALS];
 	int32_t nfexpr[CG_MAX_AGGS];
 	int8_t fexpr[CG_MAX_AGGS][CG_MAX_QEXPR];
+	/* bool_and / bool_or: per aggregate its predicate argument, a postfix tree over the same atoms (0 tokens = none).
+	 * These two fields stay last: the generated kernels of plans without predicate arguments restate the struct up to
+	 * fexpr only (cg_jit.cpp) */
+	int32_t nargexpr[CG_MAX_AGGS];
+	int8_t argexpr[CG_MAX_AGGS][CG_MAX_QEXPR];
 };
 
 static inline bool cg_desc_has_filters(const CgScanDesc *d)
@@ -253,6 +259,17 @@ static inline bool cg_desc_has_filters(const CgScanDesc *d)
 		if (d->nfilter_expr[a] > 0) return true;
 	return false;
 }
+
+/* the filter atom pool is read by some FILTER or some bool_and / bool_or argument */
+static inline bool cg_desc_uses_pool(const CgScanDesc *d)
+{
+	for (int a = 0; a < d->naggs && a < CG_MAX_AGGS; a++)
+		if (d->nfilter_expr[a] > 0 || d->narg_expr[a] > 0) return true;
+	return false;
+}
+
+static inline bool cg_kind_is_bool(int kind) { return kind == CG_AGG_BOOL_AND || kind == CG_AGG_BOOL_OR; }
+static inline bool cg_kind_is_bit(int kind) { return kind == CG_AGG_BIT_AND || kind == CG_AGG_BIT_OR; }
 
 /* plan of the specialised kernel (cg_scan_fast.cu): column roles in fixed order
  * [range quals..., group key, summed columns...] */

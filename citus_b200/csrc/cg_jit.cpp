@@ -225,9 +225,10 @@ static void choose_shape(const KPlan &plan, uint32_t nullable, JitShape *sh)
 			else
 				nhot += 1;
 		}
-		/* rejected rows are common, not rare like NULL inputs: a filtered aggregate's no-input counter gets a cell too */
+		/* rejected rows are common, not rare like NULL inputs: a filtered aggregate's no-input counter gets a cell too, and
+		 * so does the counter of a bool_and / bool_or, whose UNKNOWN rows are as common as its atoms' NULLs */
 		for (int a = 0; a < plan.naggs; a++)
-			if (plan.nfexpr[a] > 0) sh->ncell[a] = nhot++;
+			if (plan.nfexpr[a] > 0 || plan.aggs[a].barg) sh->ncell[a] = nhot++;
 		size_t bytes = (size_t) plan.capacity * nhot * sizeof(uint64_t) * JIT_THREADS;
 		if (plan.capacity <= 4096 && bytes <= 200 * 1024)
 		{
@@ -262,6 +263,8 @@ static const char *op_identity(int op)
 		case CG_WORD_MIN: return "0x7fffffffffffffffull";
 		case CG_WORD_MAX: return "0x8000000000000000ull";
 		case CG_WORD_FMIN: return "0xffffffffffffffffull";
+		case CG_WORD_AND: return "0xffffffffffffffffull";
+		case CG_WORD_OR: return "0ull";
 		default: return "0ull";
 	}
 }
@@ -276,6 +279,8 @@ static std::string op_combine(int op, const std::string &acc, const std::string 
 		case CG_WORD_MAX: return "(uint64_t) smax64((int64_t) " + acc + ", (int64_t) " + v + ")";
 		case CG_WORD_FADD: return "(uint64_t) __double_as_longlong(__longlong_as_double((int64_t) " + acc + ") + __longlong_as_double((int64_t) " + v + "))";
 		case CG_WORD_FMIN: return "umin64(" + acc + ", " + v + ")";
+		case CG_WORD_AND: return "(" + acc + " & " + v + ")";
+		case CG_WORD_OR: return "(" + acc + " | " + v + ")";
 		default: return "umax64(" + acc + ", " + v + ")";
 	}
 }
@@ -290,19 +295,34 @@ static std::string op_apply_global(int op, const std::string &p, const std::stri
 		case CG_WORD_MAX: return "atomicMax((long long *) (" + p + "), (long long) (" + v + "));";
 		case CG_WORD_FADD: return "atomicAdd((double *) (" + p + "), __longlong_as_double((long long) (" + v + ")));";
 		case CG_WORD_FMIN: return "atomicMin((unsigned long long *) (" + p + "), (unsigned long long) (" + v + "));";
+		case CG_WORD_AND: return "atomicAnd((unsigned long long *) (" + p + "), (unsigned long long) (" + v + "));";
+		case CG_WORD_OR: return "atomicOr((unsigned long long *) (" + p + "), (unsigned long long) (" + v + "));";
 		default: return "atomicMax((unsigned long long *) (" + p + "), (unsigned long long) (" + v + "));";
 	}
 }
 
 
-static void gen_prelude(std::string &s)
+static bool plan_has_args(const KPlan &plan)
 {
+	for (int a = 0; a < plan.naggs; a++)
+		if (plan.nargexpr[a] > 0) return true;
+	return false;
+}
+
+/* The host's structs restated for NVRTC.  A plan without bool_and / bool_or arguments restates KPlan up to fexpr and
+ * KAgg's barg byte as padding: its kernel reads nothing behind them (the arguments' trees are written out as code), so
+ * the plan parameter it declares is a prefix of the one the host passes, and its source is the one such plans had
+ * before the arguments existed -- the same kernel cache key, the same compiled code. */
+static void gen_prelude(std::string &s, const KPlan &plan)
+{
+	const bool args = plan_has_args(plan);
 	s +=
 		"typedef unsigned long long uint64_t; typedef long long int64_t; typedef unsigned int uint32_t; typedef int int32_t;\n"
 		"typedef unsigned short uint16_t; typedef short int16_t; typedef unsigned char uint8_t; typedef signed char int8_t;\n"
-		"struct DevChunkCol { uint64_t values_off; uint64_t exists_off; uint64_t rank_off; uint32_t value_count; uint32_t row_count; };\n"
-		"struct KAgg { int8_t kind; int8_t nfactors; int8_t is_float; int8_t nlimbs; int8_t pcol[3]; int8_t word0; int8_t nullword; int8_t ovchk; int8_t filt; int8_t pad;\n"
-		"  int64_t a[3]; int64_t b[3]; int64_t bound; int64_t tbound; };\n";
+		"struct DevChunkCol { uint64_t values_off; uint64_t exists_off; uint64_t rank_off; uint32_t value_count; uint32_t row_count; };\n";
+	s += args ? "struct KAgg { int8_t kind; int8_t nfactors; int8_t is_float; int8_t nlimbs; int8_t pcol[3]; int8_t word0; int8_t nullword; int8_t ovchk; int8_t filt; int8_t barg;\n"
+			  : "struct KAgg { int8_t kind; int8_t nfactors; int8_t is_float; int8_t nlimbs; int8_t pcol[3]; int8_t word0; int8_t nullword; int8_t ovchk; int8_t filt; int8_t pad;\n";
+	s += "  int64_t a[3]; int64_t b[3]; int64_t bound; int64_t tbound; };\n";
 	addf(s,
 		 "struct KPlan { const uint8_t *arena; const DevChunkCol *chunkcols; const uint32_t *selected; uint32_t nselected; int32_t nstaged;\n"
 		 "  int32_t ncols; uint8_t slot[%d]; uint8_t len[%d]; uint8_t isfloat[%d];\n"
@@ -313,14 +333,17 @@ static void gen_prelude(std::string &s)
 		 "  int8_t hot_of_word[%d]; int32_t nhot; uint64_t *packed; int32_t pack_shift; int32_t pack_word;\n"
 		 "  int32_t nqexpr; int8_t qexpr[%d]; int32_t slices; uint32_t slice_rows; uint32_t max_cg_rows;\n"
 		 "  int32_t nfquals; uint8_t fcol[%d]; uint8_t fop[%d]; int64_t fk[%d]; int64_t flo[%d]; int64_t fhi[%d]; uint8_t fneg[%d];\n"
-		 "  int32_t nfexpr[%d]; int8_t fexpr[%d][%d]; };\n",
+		 "  int32_t nfexpr[%d]; int8_t fexpr[%d][%d];%s",
 		 CG_KMAX_COLS, CG_KMAX_COLS, CG_KMAX_COLS, CG_MAX_QUALS, CG_MAX_QUALS, CG_MAX_QUALS, CG_MAX_QUALS, CG_MAX_QUALS, CG_MAX_QUALS,
 		 CG_MAX_GROUP_COLS, CG_MAX_AGGS, CG_KMAX_WORDS, CG_KMAX_WORDS, CG_MAX_QEXPR, CG_MAX_FILTER_QUALS, CG_MAX_FILTER_QUALS,
-		 CG_MAX_FILTER_QUALS, CG_MAX_FILTER_QUALS, CG_MAX_FILTER_QUALS, CG_MAX_FILTER_QUALS, CG_MAX_AGGS, CG_MAX_AGGS, CG_MAX_QEXPR);
-	/* the text above must describe the host's structs exactly */
+		 CG_MAX_FILTER_QUALS, CG_MAX_FILTER_QUALS, CG_MAX_FILTER_QUALS, CG_MAX_FILTER_QUALS, CG_MAX_AGGS, CG_MAX_AGGS, CG_MAX_QEXPR,
+		 args ? "\n" : " };\n");
+	if (args) addf(s, "  int32_t nargexpr[%d]; int8_t argexpr[%d][%d]; };\n", CG_MAX_AGGS, CG_MAX_AGGS, CG_MAX_QEXPR);
+	/* the text above must describe the host's structs exactly (without arguments: the prefix up to fexpr) */
+	const size_t prefix = (offsetof(KPlan, nargexpr) + alignof(KPlan) - 1) / alignof(KPlan) * alignof(KPlan);
 	addf(s, "static_assert(sizeof(DevChunkCol) == %zu, \"DevChunkCol\");\n", sizeof(DevChunkCol));
 	addf(s, "static_assert(sizeof(KAgg) == %zu, \"KAgg\");\n", sizeof(KAgg));
-	addf(s, "static_assert(sizeof(KPlan) == %zu, \"KPlan\");\n", sizeof(KPlan));
+	addf(s, "static_assert(sizeof(KPlan) == %zu, \"KPlan\");\n", args ? sizeof(KPlan) : prefix);
 	/* (NVRTC has no offsetof; same field order + same total size is the check) */
 	s +=
 		"#define EMPTY_KEY ((int64_t) 0x8000000000000000ull)\n"
@@ -472,17 +495,19 @@ static std::string agg_null_expr(const KAgg &g, const JitShape &sh)
 	return e;
 }
 
-/* "aggregate a gives no input on this row" (NULL input, or its FILTER is not TRUE: f<a>), or "" when it always does */
+/* "aggregate a gives no input on this row" (NULL input, bool_and / bool_or argument UNKNOWN -- neither TRUE: at<a> nor
+ * FALSE: af<a> --, or its FILTER is not TRUE: f<a>), or "" when it always does */
 static std::string agg_noinput_expr(const KPlan &plan, int a, const JitShape &sh)
 {
 	const KAgg &g = plan.aggs[a];
 	std::string e = g.kind == CG_AGG_COUNT_STAR ? std::string() : agg_null_expr(g, sh);
+	if (plan.nargexpr[a] > 0) e += (e.empty() ? "" : " || ") + ("(!at" + std::to_string(a) + " && !af" + std::to_string(a) + ")");
 	if (plan.nfexpr[a] > 0) e += (e.empty() ? "!f" : " || !f") + std::to_string(a);
 	return e;
 }
 
-/* a postfix tree over the atoms <prefix><q> */
-static std::string tree_expr(int n, const int8_t *expr, const char *prefix)
+/* a postfix tree over the atoms <prefix><q>; dual: with AND and OR swapped (over "is FALSE" atoms: "the tree is FALSE") */
+static std::string tree_expr(int n, const int8_t *expr, const char *prefix, bool dual = false)
 {
 	std::vector<std::string> st;
 	for (int i = 0; i < n; i++)
@@ -493,7 +518,7 @@ static std::string tree_expr(int n, const int8_t *expr, const char *prefix)
 		{
 			std::string b = st.back(); st.pop_back();
 			std::string a = st.back(); st.pop_back();
-			st.push_back("(" + a + (t == CG_QX_AND ? " && " : " || ") + b + ")");
+			st.push_back("(" + a + (((t == CG_QX_AND) != dual) ? " && " : " || ") + b + ")");
 		}
 	}
 	return st.back();
@@ -557,6 +582,12 @@ static void gen_table_updates(std::string &s, const KPlan &plan, const JitShape 
 		char p[32];
 		snprintf(p, sizeof p, "e + %d", g.word0);
 		std::string guard = an[a].empty() ? "" : ("if (!an" + std::to_string(a) + ") ");
+		const int op = plan.wordop[g.word0];
+		if (op == CG_WORD_AND || op == CG_WORD_OR)
+		{
+			/* no reduction for the identity (bit_or of 0, bool_or FALSE, bool_and TRUE), as min / max skip theirs */
+			guard = "if (" + (an[a].empty() ? std::string() : "!an" + std::to_string(a) + " && ") + w0[a] + " != " + op_identity(op) + ") ";
+		}
 		if (agg_two_limbs(g))
 			addf(s, "%s%s{ %s red_add(e + %d, (uint64_t) (it%d >> 32)); }\n", C, guard.c_str(),
 				 op_apply_global(plan.wordop[g.word0], p, w0[a]).c_str(), g.word0 + 1, a);
@@ -583,6 +614,21 @@ static void gen_row(std::string &s, const KPlan &plan, const JitShape &sh, int u
 		addf(s, "%sconst bool u%d = %s;\n", T, q, atom_expr(plan, sh, plan.fcol[q], plan.fop[q], plan.fneg[q], "f", q).c_str());
 	for (int a = 0; a < plan.naggs; a++)
 		if (plan.nfexpr[a] > 0) addf(s, "%sconst bool f%d = %s;\n", T, a, tree_expr(plan.nfexpr[a], plan.fexpr[a], "u").c_str());
+	/* bool_and / bool_or arguments, three-valued on two rails: uf<q> = atom q is FALSE (not NULL, not TRUE); at<a> = the
+	 * argument is TRUE, af<a> = it is FALSE (the same tree with AND / OR swapped over the uf<q>); neither = UNKNOWN */
+	if (plan_has_args(plan))
+	{
+		for (int q = 0; q < plan.nfquals; q++)
+		{
+			const int c = plan.fcol[q];
+			if (col_nullable(sh, c)) addf(s, "%sconst bool uf%d = !z%d && !u%d;\n", T, q, c, q);
+			else addf(s, "%sconst bool uf%d = !u%d;\n", T, q, q);
+		}
+		for (int a = 0; a < plan.naggs; a++)
+			if (plan.nargexpr[a] > 0)
+				addf(s, "%sconst bool at%d = %s;\n%sconst bool af%d = %s;\n", T, a, tree_expr(plan.nargexpr[a], plan.argexpr[a], "u").c_str(), T, a,
+					 tree_expr(plan.nargexpr[a], plan.argexpr[a], "uf", true).c_str());
+	}
 	addf(s, "%sconst bool pass = %s;\n", T, where_expr(plan).c_str());
 	addf(s, "%sif (!pass) removed++;\n%selse {\n", T, T);
 	const char *B = "\t\t\t\t\t\t\t";
@@ -652,6 +698,12 @@ static void gen_row(std::string &s, const KPlan &plan, const JitShape &sh, int u
 		an[a] = agg_noinput_expr(plan, a, sh);
 		if (!an[a].empty()) addf(s, "%sconst bool an%d = %s;\n", C, a, an[a].c_str());
 		if (!agg_has_value(g)) continue;
+		if (g.barg)
+		{
+			/* bool_and / bool_or: TRUE = all ones (the identity of AND), FALSE = 0 (that of OR) */
+			w0v[a] = "(at" + std::to_string(a) + " ? 0xffffffffffffffffull : 0ull)";
+			continue;
+		}
 		std::string e = term_expr(g, a);
 		if (g.is_float) addf(s, "%sconst double ft%d = %s;\n", C, a, e.c_str());
 		else
@@ -764,7 +816,7 @@ static std::string gen_source(const KPlan &plan, const JitShape &sh)
 {
 	std::string s;
 	s.reserve(32768);
-	gen_prelude(s);
+	gen_prelude(s, plan);
 	if (sh.min_blocks > 0)
 		addf(s, "extern \"C\" __global__ void __launch_bounds__(%d, %d) cg_jit_scan(const __grid_constant__ KPlan P)\n{\n", JIT_THREADS, sh.min_blocks);
 	else
@@ -893,8 +945,16 @@ static std::string gen_source(const KPlan &plan, const JitShape &sh)
 				addf(s, "\t{ uint64_t n = wsum(g_n%d); if ((tid & 31) == 0 && n) red_add(P.table + %d, n); }\n", a, g.nullword);
 			if (!agg_has_value(g)) continue;
 			int op = plan.wordop[g.word0];
-			addf(s, "\t{ uint64_t x = g_a%d_0;\n\t  for (int o = 16; o > 0; o >>= 1) { uint64_t y = __shfl_xor_sync(0xffffffffu, x, o); x = %s; }\n", a,
-				 op_combine(op, "x", "y").c_str());
+			if (op == CG_WORD_AND || op == CG_WORD_OR)
+			{
+				/* one redux.sync per 32-bit half instead of five shuffle rounds */
+				const char *rd = op == CG_WORD_AND ? "__reduce_and_sync" : "__reduce_or_sync";
+				addf(s, "\t{ uint64_t x = g_a%d_0;\n\t  x = ((uint64_t) %s(0xffffffffu, (uint32_t) (x >> 32)) << 32) | (uint64_t) %s(0xffffffffu, (uint32_t) x);\n",
+					 a, rd, rd);
+			}
+			else
+				addf(s, "\t{ uint64_t x = g_a%d_0;\n\t  for (int o = 16; o > 0; o >>= 1) { uint64_t y = __shfl_xor_sync(0xffffffffu, x, o); x = %s; }\n", a,
+					 op_combine(op, "x", "y").c_str());
 			char p[48];
 			snprintf(p, sizeof p, "P.table + %d", g.word0);
 			addf(s, "\t  if ((tid & 31) == 0 && x != %s) { %s }\n", op_identity(op), op_apply_global(op, p, "x").c_str());

@@ -93,6 +93,12 @@ static int validate_desc(const CgScanDesc *d, const CgColumnDesc *columns, int n
 		if (n < 0 || n > CG_MAX_QEXPR) return cg_set_error(CG_EINVAL, "nfilter_expr[%d] = %d out of range", a, n);
 		if (n > 0 && a >= d->naggs) return cg_set_error(CG_EINVAL, "filter of aggregate %d of %d", a, d->naggs);
 		if (n > 0 && (rc = validate_postfix("filter_expr", d->filter_expr[a], n, d->nfilter_quals))) return rc;
+		/* predicate arguments: only bool_and / bool_or have one, and they must (checked with the aggregates below) */
+		const int m = d->narg_expr[a];
+		if (m == 0) continue;
+		if (a >= d->naggs || !cg_kind_is_bool(d->aggs[a].kind)) return cg_set_error(CG_EINVAL, "predicate argument on aggregate %d, which takes none", a);
+		if (m < 0 || m > CG_MAX_QEXPR) return cg_set_error(CG_EINVAL, "narg_expr[%d] = %d out of range", a, m);
+		if ((rc = validate_postfix("arg_expr", d->arg_expr[a], m, d->nfilter_quals))) return rc;
 	}
 	for (int g = 0; g < d->ngroup_cols; g++)
 	{
@@ -106,8 +112,26 @@ static int validate_desc(const CgScanDesc *d, const CgColumnDesc *columns, int n
 	for (int a = 0; a < d->naggs; a++)
 	{
 		const CgAggSpec &s = d->aggs[a];
-		if (s.kind < CG_AGG_COUNT_STAR || s.kind > CG_AGG_MAX) return cg_set_error(CG_EINVAL, "aggregate %d: bad kind", a);
+		if (s.kind < CG_AGG_COUNT_STAR || s.kind > CG_AGG_BOOL_OR) return cg_set_error(CG_EINVAL, "aggregate %d: bad kind", a);
 		if (s.nfactors < 0 || s.nfactors > 3) return cg_set_error(CG_EINVAL, "aggregate %d: nfactors", a);
+		if (s.kind > CG_AGG_MAX && s.term_abs_bound != 0) return cg_set_error(CG_EINVAL, "aggregate %d: term_abs_bound on bit / bool kind", a);
+		if (cg_kind_is_bool(s.kind))
+		{
+			/* the argument is a predicate tree, not factors */
+			if (s.nfactors != 0) return cg_set_error(CG_EINVAL, "aggregate %d: bool_and / bool_or with factors", a);
+			if (d->narg_expr[a] < 1) return cg_set_error(CG_EINVAL, "aggregate %d: bool_and / bool_or without a predicate argument", a);
+			continue;
+		}
+		if (cg_kind_is_bit(s.kind))
+		{
+			/* one bare integer column: bitwise ops on the sign-extended words are exact for every width */
+			if (s.nfactors != 1 || s.a[0] != 0 || s.b[0] != 1 || s.is_float)
+				return cg_set_error(CG_EINVAL, "aggregate %d: bit_and / bit_or take one bare integer column", a);
+			if (s.column[0] < 0 || s.column[0] >= natts) return cg_set_error(CG_EINVAL, "aggregate %d: column out of range", a);
+			if (columns[s.column[0]].type_class != CG_TYPE_INT)
+				return cg_set_error(CG_EINVAL, "aggregate %d: bit_and / bit_or over a column that is not an integer type", a);
+			continue;
+		}
 		if (s.kind != CG_AGG_COUNT_STAR && s.nfactors == 0)
 			return cg_set_error(CG_EINVAL, "aggregate %d needs an argument", a);
 		for (int f = 0; f < s.nfactors; f++)
@@ -130,6 +154,9 @@ static int validate_desc(const CgScanDesc *d, const CgColumnDesc *columns, int n
  *                 two-limb form (low 32 bits unsigned, term >> 32 signed), + NULL-input count
  *   sum(float8)   1 FADD word + NULL-input count
  *   min/max       1 MIN/MAX (FMIN/FMAX on the order-preserving float encoding) + NULL-input count
+ *   bit_and/or    1 AND/OR word (identity ~0 / 0) over the sign-extended values + NULL-input count
+ *   bool_and/or   1 AND/OR word whose bit 0 is the result (a TRUE input contributes ~0, a FALSE one 0, so TRUE is the
+ *                 identity of bool_and and FALSE that of bool_or) + a count of the rows that gave no input (UNKNOWN)
  * Counting the NULL inputs instead of the non-NULL ones keeps NULL-free data (the common
  * case) at one atomic per aggregate and row, while "no non-NULL input => SQL NULL" and
  * count(x) stay exact: non-NULL inputs = rows in group - NULL inputs.
@@ -158,8 +185,17 @@ static int layout_partial(CgPartial *p, const CgColumnDesc *columns)
 		k.ovchk = (int8_t) (!s.is_float && (s.kind == CG_AGG_SUM || s.kind == CG_AGG_MIN || s.kind == CG_AGG_MAX) &&
 							k.tbound == 0 && !(s.nfactors == 1 && s.a[0] == 0 && s.b[0] == 1));
 		k.filt = (int8_t) (d.nfilter_expr[a] > 0);
+		k.barg = (int8_t) cg_kind_is_bool(s.kind);
 		switch (s.kind)
 		{
+			case CG_AGG_BIT_AND:
+			case CG_AGG_BIT_OR:
+			case CG_AGG_BOOL_AND:
+			case CG_AGG_BOOL_OR:
+				k.word0 = (int8_t) nw;
+				p->wordop[nw++] = (s.kind == CG_AGG_BIT_AND || s.kind == CG_AGG_BOOL_AND) ? CG_WORD_AND : CG_WORD_OR;
+				k.nullword = (int8_t) nw; p->wordop[nw++] = CG_WORD_ADD;
+				break;
 			case CG_AGG_COUNT_STAR:
 				k.word0 = 0;
 				if (k.filt) { k.nullword = (int8_t) nw; p->wordop[nw++] = CG_WORD_ADD; }
@@ -363,7 +399,9 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 	if (partial->desc.naggs != desc->naggs || partial->desc.ngroup_cols != desc->ngroup_cols)
 		return cg_set_error(CG_EINVAL, "partial aggregate was created for a different query shape");
 	for (int a = 0; a < desc->naggs; a++)
-		if (memcmp(&partial->desc.aggs[a], &desc->aggs[a], sizeof(CgAggSpec)) != 0 || partial->aggs[a].filt != (desc->nfilter_expr[a] > 0))
+		if (memcmp(&partial->desc.aggs[a], &desc->aggs[a], sizeof(CgAggSpec)) != 0 || partial->aggs[a].filt != (desc->nfilter_expr[a] > 0) ||
+			partial->desc.narg_expr[a] != desc->narg_expr[a] ||
+			memcmp(partial->desc.arg_expr[a], desc->arg_expr[a], (size_t) desc->narg_expr[a]) != 0)
 			return cg_set_error(CG_EINVAL, "partial aggregate was created for a different aggregate list");
 
 	memset(plan, 0, sizeof *plan);
@@ -434,9 +472,10 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 			plan->aggs[a].pcol[f] = (int8_t) pc;
 		}
 	}
-	if (cg_desc_has_filters(desc))
+	if (cg_desc_uses_pool(desc))
 	{
-		/* a column read only by a FILTER is a plan column like any other (projection, column limit) */
+		/* a column read only by a FILTER or a predicate argument is a plan column like any other (projection, column
+		 * limit) */
 		plan->nfquals = desc->nfilter_quals;
 		for (int q = 0; q < desc->nfilter_quals; q++)
 		{
@@ -450,6 +489,8 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 		{
 			plan->nfexpr[a] = desc->nfilter_expr[a];
 			for (int i = 0; i < desc->nfilter_expr[a]; i++) plan->fexpr[a][i] = desc->filter_expr[a][i];
+			plan->nargexpr[a] = desc->narg_expr[a];
+			for (int i = 0; i < desc->narg_expr[a]; i++) plan->argexpr[a][i] = desc->arg_expr[a][i];
 		}
 	}
 	plan->ncols = ncols;

@@ -120,8 +120,10 @@ __device__ __forceinline__ void process_row(const KPlan &P, const int64_t (&v)[N
 	else
 		acc.rows++;
 
-	/* aggregate FILTERs: a rejected row is no input of its aggregate, counted like a NULL input */
-	const uint32_t rejected = eval_filters<NCC>(P, v, nullmask);
+	/* aggregate FILTERs: a rejected row is no input of its aggregate, counted like a NULL input; so is a row whose
+	 * bool_and / bool_or argument is UNKNOWN */
+	uint32_t argtrue;
+	const uint32_t rejected = eval_filters<NCC>(P, v, nullmask, &argtrue);
 
 	/* K4: transition functions */
 #pragma unroll
@@ -173,7 +175,9 @@ __device__ __forceinline__ void process_row(const KPlan &P, const int64_t (&v)[N
 				}
 				else { w0 = (uint64_t) (uint32_t) it; w1 = (uint64_t) (it >> 32); }
 			}
-			else /* MIN / MAX */
+			else if (g.barg) /* BOOL_AND / BOOL_OR: TRUE = all ones */
+				w0 = ((argtrue >> a) & 1u) ? ~0ull : 0ull;
+			else /* MIN / MAX, BIT_AND / BIT_OR (the sign-extended column value) */
 				w0 = g.is_float ? f8_ordered(__double_as_longlong(ft)) : (uint64_t) it;
 			const bool two = (g.kind == CG_AGG_SUM && !g.is_float && g.nlimbs == 2);
 			if (MODE == CG_MODE_GLOBAL)

@@ -72,8 +72,10 @@ __device__ __forceinline__ bool eval_quals(const KPlan &P, const int64_t (&v)[NC
 template <int NCC>
 __device__ __forceinline__ void eval_terms(const KPlan &P, const int64_t (&v)[NCC], uint32_t nullmask, RowTerms<NCC> &t)
 {
-	/* a row an aggregate's FILTER rejects is no input of it, like a NULL input */
-	t.nullbits = eval_filters<NCC>(P, v, nullmask);
+	/* a row an aggregate's FILTER rejects is no input of it, like a NULL input; so is a row whose bool_and / bool_or
+	 * argument is UNKNOWN */
+	uint32_t argtrue;
+	t.nullbits = eval_filters<NCC>(P, v, nullmask, &argtrue);
 #pragma unroll
 	for (int a = 0; a < CG_MAX_AGGS; a++)
 	{
@@ -106,6 +108,8 @@ __device__ __forceinline__ void eval_terms(const KPlan &P, const int64_t (&v)[NC
 				}
 				else { t.w0[a] = (uint64_t) (uint32_t) it; t.w1[a] = (uint64_t) (it >> 32); }
 			}
+			else if (g.barg)
+				t.w0[a] = ((argtrue >> a) & 1u) ? ~0ull : 0ull;
 			else
 				t.w0[a] = g.is_float ? f8_ordered(__double_as_longlong(ft)) : (uint64_t) it;
 		}
@@ -152,7 +156,7 @@ __device__ __forceinline__ void small_accumulate(const KPlan &P, uint64_t *mine,
 			if ((t.nullbits >> a) & 1u)
 			{
 				/* a filtered aggregate's no-input counter has a cell (rejected rows are common) */
-				if (g.filt) e[P.hot_of_word[g.nullword] * CGS_THREADS] += 1ull;
+				if (g.filt || g.barg) e[P.hot_of_word[g.nullword] * CGS_THREADS] += 1ull;
 				else atomicAdd((unsigned long long *) P.table + (uint64_t) slot * (uint64_t) P.stride + g.nullword, 1ull);
 				continue;
 			}
@@ -316,7 +320,7 @@ static int hot_words(const KPlan &plan, int8_t *hot)
 	for (int a = 0; a < plan.naggs; a++)
 	{
 		const KAgg &g = plan.aggs[a];
-		if (g.filt) is_hot[g.nullword] = true;
+		if (g.filt || g.barg) is_hot[g.nullword] = true;
 		if (g.kind == CG_AGG_COUNT_STAR || g.kind == CG_AGG_COUNT) continue;
 		is_hot[g.word0] = true;
 		if (g.kind == CG_AGG_SUM && !g.is_float && g.nlimbs == 2) is_hot[g.word0 + 1] = true;

@@ -35,9 +35,7 @@ extern "C" int cg_partial_merge_values(CgPartial *p, int64_t nrows, const int64_
 		hk[i] = keys ? keys[i] : 0;
 		hn[i] = key_nulls ? key_nulls[i] : 0;
 		uint64_t *w = &hw[(size_t) i * nw];
-		for (int x = 0; x < nw; x++) w[x] = p->wordop[x] == CG_WORD_MIN ? (uint64_t) INT64_MAX :
-											p->wordop[x] == CG_WORD_MAX ? (uint64_t) INT64_MIN :
-											p->wordop[x] == CG_WORD_FMIN ? ~0ull : 0ull;
+		for (int x = 0; x < nw; x++) w[x] = word_identity(p->wordop[x]);
 		/* rows in the group: count(*) when the query has one, else the largest non-NULL input count (at least 1, so
 		 * that a group whose aggregates all saw only NULLs still exists); NULL-input counters are rows - count */
 		int64_t rows = 1;
@@ -86,8 +84,16 @@ extern "C" int cg_partial_merge_values(CgPartial *p, int64_t nrows, const int64_
 					}
 				}
 			}
+			else if (cg_kind_is_bool(k.kind))
+			{
+				if (!minmax) return cg_set_error(CG_EINVAL, "NULL minmax array");
+				if (minmax[i * na + a] != 0 && minmax[i * na + a] != 1)
+					return cg_set_error(CG_EINVAL, "bool_and / bool_or value %lld in partial row %lld", (long long) minmax[i * na + a], (long long) i);
+				w[k.word0] = minmax[i * na + a] ? ~0ull : 0ull;
+			}
 			else
 			{
+				/* min / max, and bit_and / bit_or (sign-extended values) */
 				if (!minmax) return cg_set_error(CG_EINVAL, "NULL minmax array");
 				uint64_t u = (uint64_t) minmax[i * na + a];
 				if (k.is_float) u = f8_ordered((int64_t) u);     /* order-preserving encoding of the words */

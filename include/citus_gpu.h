@@ -179,10 +179,15 @@ typedef struct CgQual
 	int64_t konst;    /* integer, or float8 bits for float columns */
 } CgQual;
 
-enum { CG_AGG_COUNT_STAR = 0, CG_AGG_COUNT = 1, CG_AGG_SUM = 2, CG_AGG_MIN = 3, CG_AGG_MAX = 4 };
+enum { CG_AGG_COUNT_STAR = 0, CG_AGG_COUNT = 1, CG_AGG_SUM = 2, CG_AGG_MIN = 3, CG_AGG_MAX = 4,
+	   CG_AGG_BIT_AND = 5, CG_AGG_BIT_OR = 6, CG_AGG_BOOL_AND = 7, CG_AGG_BOOL_OR = 8 };
 
 /* aggregate argument = product over factors of (a + b * column); covers sum(x),
- * sum(x*y), sum(x*(1-d)), sum(x*(1-d)*(1+t)) on scaled-integer decimals (TPC-H Q1/Q6) */
+ * sum(x*y), sum(x*(1-d)), sum(x*(1-d)*(1+t)) on scaled-integer decimals (TPC-H Q1/Q6).
+ * bit_and / bit_or (CG_AGG_BIT_*): the argument is one bare integer column (nfactors 1, a 0, b 1, is_float 0); the
+ * result is in the column's type, the words hold it sign-extended to 64 bits.  bool_and / bool_or / every
+ * (CG_AGG_BOOL_*): nfactors 0, the argument is the predicate tree arg_expr[a] of CgScanDesc.  None of the four takes
+ * a term_abs_bound. */
 typedef struct CgAggSpec
 {
 	int32_t kind;        /* CG_AGG_* */
@@ -236,11 +241,24 @@ typedef struct CgScanDesc
 	 * a only when a's tree is TRUE under three-valued logic (an atom on a NULL column is not TRUE), and a rejected
 	 * row's argument is not evaluated: it raises neither the int64 overflow nor the term_abs_bound error.  So a group
 	 * without accepted rows has count(*) / count(x) = 0 and sum / min / max = NULL (count 0).  A column read only by a
-	 * filter is staged and counts toward the query's column limit. */
+	 * filter is staged and counts toward the query's column limit.
+	 * The pool is shared with the predicate arguments of bool_and / bool_or below: at most CG_MAX_FILTER_QUALS atoms
+	 * for all FILTERs and arguments of a query together, and an atom they have in common is stored once. */
 	int32_t nfilter_quals;
 	CgQual filter_quals[CG_MAX_FILTER_QUALS];
 	int32_t nfilter_expr[CG_MAX_AGGS];
 	int8_t filter_expr[CG_MAX_AGGS][CG_MAX_QEXPR];
+	/* Predicate argument of bool_and / bool_or / every (CG_AGG_BOOL_*): aggregate a's argument p is the postfix tree
+	 * arg_expr[a][0..narg_expr[a]) over the filter_quals pool, 1..CG_MAX_QEXPR tokens; narg_expr[a] = 0 for every other
+	 * kind, so a zero-filled tail is a query without predicate arguments.  p is evaluated under three-valued logic: an
+	 * atom on a NULL column is UNKNOWN (a float atom is never UNKNOWN otherwise: NaN compares in btree order), AND is
+	 * FALSE if an arm is FALSE, OR is TRUE if an arm is TRUE.  A row whose p is UNKNOWN is no input (like a NULL
+	 * argument), and so is a row the aggregate's FILTER rejects (its p is not consulted).  bool_and = every input is
+	 * TRUE, bool_or = some input is TRUE; with no input the result is NULL.  cg_partial_fetch returns the value in
+	 * minmax (0 / 1) and the number of inputs in count (0 = NULL); chunk-group skipping and cg_relation_bounds ignore
+	 * the argument atoms, as they ignore the filter atoms. */
+	int32_t narg_expr[CG_MAX_AGGS];
+	int8_t arg_expr[CG_MAX_AGGS][CG_MAX_QEXPR];
 } CgScanDesc;
 
 /* EXPLAIN ANALYZE counters (columnar_customscan.c:1966-1999 and ExecScan instrumentation) */
@@ -320,7 +338,8 @@ int cg_scan_relation(const CgRelation *rel, const CgScanDesc *desc, CgPartial *i
  *   sum_hi/sum_lo  128-bit integer sum (two's complement), or float8 sum in fsum
  *   count          count(*) / count(x) value, or for sum/min/max the number of non-NULL
  *                  inputs (0 => the SQL result is NULL)
- *   minmax         min or max (integer, or float8 bits)
+ *   minmax         min or max (integer, or float8 bits); bit_and / bit_or (sign-extended); bool_and / bool_or (0 / 1)
+ *   count          of bit_* / bool_*: the number of inputs (0 => NULL)
  * Any output pointer may be NULL. */
 int cg_partial_ngroups(CgPartial *p, int64_t *ngroups);
 int cg_partial_fetch(CgPartial *p, int64_t capacity, int64_t *keys, uint8_t *key_nulls,
@@ -347,7 +366,10 @@ int cg_agg_column(int32_t attlen, int32_t is_float, const void *values, const ui
  * or by ncclReduce on the dense layout. */
 int cg_partial_layout(const CgPartial *p, int32_t *nwords, int32_t *word_ops /* [nwords] CG_WORD_* */,
 					  int32_t *is_dense, int64_t *capacity);
-enum { CG_WORD_ADD = 0, CG_WORD_MIN = 1, CG_WORD_MAX = 2, CG_WORD_FADD = 3, CG_WORD_FMIN = 4, CG_WORD_FMAX = 5 };
+/* CG_WORD_AND / CG_WORD_OR: bitwise, identities ~0 and 0 (bit_and / bit_or values; bool_and / bool_or keep the truth
+ * value in bit 0, an input TRUE contributes ~0 and FALSE 0) */
+enum { CG_WORD_ADD = 0, CG_WORD_MIN = 1, CG_WORD_MAX = 2, CG_WORD_FADD = 3, CG_WORD_FMIN = 4, CG_WORD_FMAX = 5,
+	   CG_WORD_AND = 6, CG_WORD_OR = 7 };
 
 /* Compact occupied groups into device arrays owned by the caller (e.g. torch tensors):
  * d_keys[capacity], d_key_nulls[capacity] (may be NULL), d_words[capacity*nwords];

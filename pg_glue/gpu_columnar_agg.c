@@ -125,6 +125,7 @@ type_is_supported(Oid type, int *attlen, int *type_class)
 		case INT8OID: case TIMESTAMPOID: case TIMESTAMPTZOID: *attlen = 8; *type_class = CG_TYPE_INT; return true;
 		case INT4OID: case DATEOID: *attlen = 4; *type_class = CG_TYPE_INT; return true;
 		case INT2OID: *attlen = 2; *type_class = CG_TYPE_INT; return true;
+		case BOOLOID: *attlen = 1; *type_class = CG_TYPE_INT; return true;        /* one byte, 0 / 1 */
 		case FLOAT8OID: *attlen = 8; *type_class = CG_TYPE_FLOAT; return true;
 		case FLOAT4OID: *attlen = 4; *type_class = CG_TYPE_FLOAT; return true;
 		default: return false;
@@ -196,13 +197,28 @@ translate_atom(OpExpr *op, TupleDesc tupdesc, CgQual *qual)
 	}
 	else
 		qual->konst = attlen == 8 ? DatumGetInt64(konst->constvalue) :
-					  attlen == 4 ? (int64) DatumGetInt32(konst->constvalue) : (int64) DatumGetInt16(konst->constvalue);
+					  attlen == 4 ? (int64) DatumGetInt32(konst->constvalue) :
+					  attlen == 2 ? (int64) DatumGetInt16(konst->constvalue) : (int64) DatumGetBool(konst->constvalue);
+	return true;
+}
+
+/* a bare bool column `flag` as the atom "flag = 1", and NOT flag as "flag = 0" (a NULL flag stays UNKNOWN either way) */
+static bool
+translate_bool_var(Node *node, bool negated, TupleDesc tupdesc, CgQual *qual)
+{
+	Var *var = strip_to_var(node);
+	if (var == NULL || var->vartype != BOOLOID || var->varattno <= 0 || var->varattno > tupdesc->natts)
+		return false;
+	qual->column = var->varattno - 1;
+	qual->op = CG_OP_EQ;
+	qual->konst = negated ? 0 : 1;
 	return true;
 }
 
 /* boolean tree -> atoms appended to atoms[0 .. *natoms) (at most max_atoms) + postfix tokens appended to tokens[0 .. *ntokens)
- * (at most CG_MAX_QEXPR): the WHERE list (quals / qual_expr) and aggregate FILTERs (filter_quals / filter_expr[a]).  false
- * when a node is not AND / OR / atom or the tree is too big */
+ * (at most CG_MAX_QEXPR): the WHERE list (quals / qual_expr), aggregate FILTERs (filter_quals / filter_expr[a]) and the
+ * predicate arguments of bool_and / bool_or / every (filter_quals / arg_expr[a]).  An atom is "Var op Const", a bare bool
+ * Var, or NOT over a bare bool Var.  false when a node is anything else or the tree is too big */
 static bool
 translate_where(Node *node, TupleDesc tupdesc, CgQual *atoms, int32_t *natoms, int max_atoms, int8_t *tokens, int32_t *ntokens)
 {
@@ -210,7 +226,14 @@ translate_where(Node *node, TupleDesc tupdesc, CgQual *atoms, int32_t *natoms, i
 	{
 		BoolExpr *b = (BoolExpr *) node;
 		if (b->boolop == NOT_EXPR)
-			return false;
+		{
+			/* only NOT over a bare bool column: its negation is the atom "flag = 0" */
+			if (list_length(b->args) != 1 || *natoms >= max_atoms || *ntokens >= CG_MAX_QEXPR ||
+				!translate_bool_var((Node *) linitial(b->args), true, tupdesc, &atoms[*natoms]))
+				return false;
+			tokens[(*ntokens)++] = (int8_t) (*natoms)++;
+			return true;
+		}
 		ListCell *lc;
 		int n = 0;
 		foreach(lc, b->args)
@@ -226,9 +249,9 @@ translate_where(Node *node, TupleDesc tupdesc, CgQual *atoms, int32_t *natoms, i
 		}
 		return n > 0;
 	}
-	if (!IsA(node, OpExpr) || *natoms >= max_atoms || *ntokens >= CG_MAX_QEXPR)
+	if (*natoms >= max_atoms || *ntokens >= CG_MAX_QEXPR)
 		return false;
-	if (!translate_atom((OpExpr *) node, tupdesc, &atoms[*natoms]))
+	if (IsA(node, OpExpr) ? !translate_atom((OpExpr *) node, tupdesc, &atoms[*natoms]) : !translate_bool_var(node, false, tupdesc, &atoms[*natoms]))
 		return false;
 	tokens[(*ntokens)++] = (int8_t) (*natoms)++;
 	return true;
@@ -262,7 +285,21 @@ translate_aggref(Aggref *agg, TupleDesc tupdesc, CgScanDesc *desc, GpuOutColumn 
 	}
 	if (list_length(agg->args) != 1)
 		return false;
-	Var *var = strip_to_var((Node *) ((TargetEntry *) linitial(agg->args))->expr);
+	Node *arg = (Node *) ((TargetEntry *) linitial(agg->args))->expr;
+	if (strcmp(name, "bool_and") == 0 || strcmp(name, "bool_or") == 0 || strcmp(name, "every") == 0)
+	{
+		/* the argument is a predicate (a bool column or any tree translate_where accepts), written into the atom pool it
+		 * shares with the FILTERs; three-valued: an UNKNOWN row is no input, no input at all is NULL (count 0) */
+		spec->kind = strcmp(name, "bool_or") == 0 ? CG_AGG_BOOL_OR : CG_AGG_BOOL_AND;
+		desc->narg_expr[desc->naggs] = 0;
+		if (!translate_where(arg, tupdesc, desc->filter_quals, &desc->nfilter_quals, CG_MAX_FILTER_QUALS, desc->arg_expr[desc->naggs],
+							 &desc->narg_expr[desc->naggs]))
+			return false;
+		out->kind = GPU_OUT_MINMAX; out->type = BOOLOID;
+		desc->naggs++;
+		return true;
+	}
+	Var *var = strip_to_var(arg);
 	int attlen, type_class;
 	if (var == NULL || var->varattno <= 0 || var->varattno > tupdesc->natts || !type_is_supported(var->vartype, &attlen, &type_class))
 		return false;
@@ -286,9 +323,18 @@ translate_aggref(Aggref *agg, TupleDesc tupdesc, CgScanDesc *desc, GpuOutColumn 
 		else return false;
 		if (var->vartype == FLOAT4OID) return false;          /* [PG] sum(float4) accumulates in float4: not what the kernels do */
 	}
-	else if (strcmp(name, "min") == 0 || strcmp(name, "max") == 0)
+	else if (strcmp(name, "min") == 0 || strcmp(name, "max") == 0 || strcmp(name, "any_value") == 0)
 	{
-		spec->kind = name[1] == 'i' ? CG_AGG_MIN : CG_AGG_MAX;
+		/* any_value(x): any non-NULL input -- the minimum is one */
+		spec->kind = name[1] == 'a' ? CG_AGG_MAX : CG_AGG_MIN;
+		out->kind = GPU_OUT_MINMAX; out->type = var->vartype;
+	}
+	else if (strcmp(name, "bit_and") == 0 || strcmp(name, "bit_or") == 0)
+	{
+		/* bare int2 / int4 / int8 column; the result has the argument's type (words hold it sign-extended) */
+		if (var->vartype != INT2OID && var->vartype != INT4OID && var->vartype != INT8OID)
+			return false;
+		spec->kind = name[4] == 'a' ? CG_AGG_BIT_AND : CG_AGG_BIT_OR;
 		out->kind = GPU_OUT_MINMAX; out->type = var->vartype;
 	}
 	else
@@ -458,6 +504,7 @@ datum_to_i64(Datum d, Oid type)
 		case INT8OID: case TIMESTAMPOID: case TIMESTAMPTZOID: return DatumGetInt64(d);
 		case INT4OID: case DATEOID: return (int64) DatumGetInt32(d);
 		case INT2OID: return (int64) DatumGetInt16(d);
+		case BOOLOID: return (int64) DatumGetBool(d);
 		case FLOAT8OID: { double x = DatumGetFloat8(d); int64 v; memcpy(&v, &x, sizeof v); return v; }
 		case FLOAT4OID: { double x = (double) DatumGetFloat4(d); int64 v; memcpy(&v, &x, sizeof v); return v; }
 		default: return 0;
@@ -596,6 +643,7 @@ i64_to_datum(int64 v, Oid type)
 	{
 		case INT4OID: case DATEOID: return Int32GetDatum((int32) v);
 		case INT2OID: return Int16GetDatum((int16) v);
+		case BOOLOID: return BoolGetDatum(v != 0);
 		case FLOAT8OID: { double x; memcpy(&x, &v, sizeof x); return Float8GetDatum(x); }
 		default: return Int64GetDatum(v);
 	}
