@@ -100,6 +100,23 @@ __device__ __forceinline__ void load_pair(const uint8_t *vals, uint32_t r, int l
 	}
 }
 
+/* two consecutive rows (r even, r + 1 may be past `rows`) of column c, which has NULLs: row -> value index through
+ * the exists bitmap and the rank directory (rank[b] = set exists bits before row 64 b; NULL rows occupy no bytes in
+ * the value stream, columnar_reader.c:1550-1555).  A NULL row reads 0 and sets bit c of n0 / n1. */
+__device__ __forceinline__ void load_pair_nullable(const uint8_t *vals, const uint64_t *exists, const uint32_t *rank, uint32_t r,
+												   uint32_t rows, int len, bool isfloat, int c, int64_t &v0, int64_t &v1,
+												   uint32_t &n0, uint32_t &n1)
+{
+	uint64_t w = ldg_stream8(exists + (r >> 6));
+	uint32_t sh = r & 63u;
+	uint32_t before = __ldg(rank + (r >> 6)) + __popcll(w & ((1ull << sh) - 1ull));
+	uint32_t e0 = (uint32_t) (w >> sh) & 1u, e1 = (uint32_t) (w >> (sh + 1)) & 1u;
+	v0 = e0 ? load_scalar(vals + (uint64_t) before * len, len, isfloat) : 0;
+	v1 = (e1 && r + 1 < rows) ? load_scalar(vals + (uint64_t) (before + e0) * len, len, isfloat) : 0;
+	n0 |= (e0 ^ 1u) << c;
+	n1 |= (e1 ^ 1u) << c;
+}
+
 template <int N>
 __device__ __forceinline__ int64_t pick(const int64_t (&v)[N], int idx)
 {
@@ -318,22 +335,133 @@ __device__ __forceinline__ uint64_t word_combine(int op, uint64_t a, uint64_t b)
 	}
 }
 
+__device__ __forceinline__ uint64_t warp_reduce_word(uint64_t x, int op)
+{
+#pragma unroll
+	for (int o = 16; o > 0; o >>= 1)
+	{
+		uint64_t y = __shfl_xor_sync(0xffffffffu, x, o);
+		x = word_combine(op, x, y);
+	}
+	return x;
+}
 
+/* the group key of a row that passed WHERE: one column, or two packed (low / high 32 bits).  false = a NULL in a
+ * two-column key: the row has no group here (CG_ERRFLAG_NULL_MULTIKEY raised) */
+template <int NCC>
+__device__ __forceinline__ bool group_key(const KPlan &P, const int64_t (&v)[NCC], uint32_t nullmask, int64_t &key, bool &key_null)
+{
+	if (P.ngroup == 1)
+	{
+		int c = P.gcol[0];
+		key_null = (nullmask >> c) & 1u;
+		key = pick<NCC>(v, c);
+		return true;
+	}
+	int c0 = P.gcol[0], c1 = P.gcol[1];
+	if (((nullmask >> c0) | (nullmask >> c1)) & 1u)
+	{
+		atomicOr(P.stats + 2, CG_ERRFLAG_NULL_MULTIKEY);
+		return false;
+	}
+	key_null = false;
+	key = (int64_t) ((uint64_t) (uint32_t) pick<NCC>(v, c0) | ((uint64_t) (uint32_t) pick<NCC>(v, c1) << 32));
+	return true;
+}
 
-/* direct index of a group key that arrives packed (two columns: low / high 32 bits);
- * ~0 = outside the declared domain */
+/* direct index of a group key (group_key's packing); the NULL key -> `capacity`; ~0 = outside the declared domain
+ * (CG_ERRFLAG_KEY_RANGE raised) */
 __device__ __forceinline__ uint64_t dense_slot_of_packed(const KPlan &P, int64_t key, bool key_null)
 {
 	if (key_null) return P.capacity;
+	uint64_t s;
 	if (P.ngroup == 2)
 	{
 		uint64_t a = (uint64_t) (int64_t) (int32_t) (uint32_t) key - (uint64_t) P.key_min;
 		uint64_t b = (uint64_t) (int64_t) (int32_t) (uint32_t) ((uint64_t) key >> 32) - (uint64_t) P.key_min1;
-		if (b >= P.range1 || a * P.range1 + b >= P.capacity) return ~0ull;
-		return a * P.range1 + b;
+		s = (b >= P.range1) ? ~0ull : a * P.range1 + b;
 	}
-	uint64_t s = (uint64_t) key - (uint64_t) P.key_min;
-	return s >= P.capacity ? ~0ull : s;
+	else
+		s = (uint64_t) key - (uint64_t) P.key_min;
+	if (s < P.capacity) return s;
+	atomicOr(P.stats + 2, CG_ERRFLAG_KEY_RANGE);
+	return ~0ull;
+}
+
+/*
+ * K4: the transition terms of a row that passed WHERE and has a group.  For each aggregate a < min(naggs, NA), in
+ * order, term(a, g, noinput, w0, w1) is called when the row is no input of a -- an argument is NULL, its FILTER is
+ * not TRUE or its bool_and / bool_or argument is UNKNOWN: a strict transition function skips the row, it is only
+ * counted -- and otherwise when a has a value word: w0 = that word's operand, w1 = the high limb of a two-limb sum
+ * (count(x) is rows - no-input rows).  A term goes to its accumulator before the next one is computed, so that the
+ * 64-register general kernel never holds more than one.
+ */
+template <int NCC, int NA, class Term>
+__device__ __forceinline__ void row_terms(const KPlan &P, const int64_t (&v)[NCC], uint32_t nullmask, Term term)
+{
+	uint32_t argtrue;
+	const uint32_t rejected = eval_filters<NCC>(P, v, nullmask, &argtrue);
+#pragma unroll
+	for (int a = 0; a < NA; a++)
+	{
+		if (a < P.naggs)
+		{
+			const KAgg &g = P.aggs[a];
+			bool isnull = (rejected >> a) & 1u;
+			if (g.kind == CG_AGG_COUNT_STAR)
+			{
+				if (isnull) term(a, g, true, 0ull, 0ull);
+				continue;
+			}
+			int64_t it = 1;
+			double ft = 1.0;
+#pragma unroll
+			for (int f = 0; f < 3; f++)
+				if (f < g.nfactors)
+				{
+					int c = g.pcol[f];
+					isnull = isnull || ((nullmask >> c) & 1u);
+					if (g.is_float) ft *= __longlong_as_double(g.a[f]) + __longlong_as_double(g.b[f]) * __longlong_as_double(pick<NCC>(v, c));
+				}
+			if (!g.is_float) it = int_term<NCC>(g, v, isnull, P.stats);
+			if (isnull) { term(a, g, true, 0ull, 0ull); continue; }
+			if (g.kind == CG_AGG_COUNT) continue;
+			uint64_t w0, w1 = 0;
+			if (g.kind == CG_AGG_SUM)
+			{
+				if (g.is_float) w0 = (uint64_t) __double_as_longlong(ft);
+				else if (g.nlimbs == 1)
+				{
+					if (it > g.bound || it < -g.bound) atomicOr(P.stats + 2, CG_ERRFLAG_SUM_BOUND);
+					w0 = (uint64_t) it;
+				}
+				else { w0 = (uint64_t) (uint32_t) it; w1 = (uint64_t) (it >> 32); }
+			}
+			else if (g.barg) /* BOOL_AND / BOOL_OR: TRUE = all ones */
+				w0 = ((argtrue >> a) & 1u) ? ~0ull : 0ull;
+			else /* MIN / MAX, BIT_AND / BIT_OR (the sign-extended column value) */
+				w0 = g.is_float ? f8_ordered(__double_as_longlong(ft)) : (uint64_t) it;
+			term(a, g, false, w0, w1);
+		}
+	}
+}
+
+/* an exact integer sum kept as two words (low 32 bits, high part) */
+__host__ __device__ __forceinline__ bool two_limbs(const KAgg &g) { return g.kind == CG_AGG_SUM && !g.is_float && g.nlimbs == 2; }
+
+/* one row into an entry of the global group table (word 0 = rows in the group) */
+template <int NCC, int NA>
+__device__ __forceinline__ void global_accumulate(const KPlan &P, uint64_t *entry, const int64_t (&v)[NCC], uint32_t nullmask)
+{
+	atomicAdd((unsigned long long *) entry, 1ull);
+	row_terms<NCC, NA>(P, v, nullmask, [&](int, const KAgg &g, bool noinput, uint64_t w0, uint64_t w1) {
+		if (noinput) atomicAdd((unsigned long long *) entry + g.nullword, 1ull);
+		else
+		{
+			word_apply_global(entry + g.word0, P.wordop[g.word0], w0);
+			if (two_limbs(g)) atomicAdd((unsigned long long *) entry + g.word0 + 1, (unsigned long long) w1);
+		}
+	});
 }
 
 #endif

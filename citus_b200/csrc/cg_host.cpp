@@ -927,18 +927,83 @@ static int after_launch(CgContext *ctx, CgPartial *p, bool used_packed, bool pac
 	return CG_OK;
 }
 
-static int read_stats(CgContext *ctx, CgPartial *p, unsigned long long before[3], CgScanStats *stats)
+/* the ahead-of-time fast kernel takes NULL-free chunk groups of a plan it covers (cg_build_fast_plan), unless the key
+ * domain is small enough for per-lane shared-memory tables or the scan is forced onto the general or the generated
+ * kernel */
+static bool fast_eligible(const CgScanDesc *desc, const KPlan &plan, bool all8, FPlan *fast)
 {
+	return !cg_small_eligible(plan) && !cg_force_general() && cg_jit_level() < 2 && cg_build_fast_plan(desc, plan, all8, fast);
+}
+
+/*
+ * The specialised kernels over plan.selected[0 .. nselected): the fast kernel when `fast` is given, else -- unless
+ * the general kernel is forced -- the generated kernel; nullable = the plan columns that may have NULLs there (0:
+ * its plain form).  *taken = false: neither took the chunk groups (the JIT is off, unavailable or declines).
+ */
+static int scan_specialised(CgContext *ctx, CgPartial *into, const KPlan &plan, const FPlan *fast, uint32_t nullable, uint64_t rows,
+							bool *taken)
+{
+	bool packed = false, ponly = false;
+	*taken = false;
+	if (fast)
+	{
+		FPlan f = *fast;
+		f.selected = plan.selected;
+		f.nselected = plan.nselected;
+		int rc = cg_launch_scan_fast(ctx, f, ctx->compute);
+		if (rc) return rc;
+		*taken = true;
+		packed = f.packed != nullptr;
+		ponly = f.nsums == 1;
+	}
+	else if (!cg_force_general())
+	{
+		int rc = cg_launch_scan_jit(ctx, plan, nullable, ctx->compute, taken, &packed, &ponly);
+		if (rc) return rc;
+	}
+	return *taken ? after_launch(ctx, into, packed, ponly, rows) : CG_OK;
+}
+
+/* the interpretive kernels: the small-domain one when per-lane tables fit shared memory, the general one otherwise */
+static int scan_interpretive(CgContext *ctx, CgPartial *into, const KPlan &plan, bool all8, uint64_t rows)
+{
+	int rc = (cg_small_eligible(plan) && !cg_force_general()) ? cg_launch_scan_small(ctx, plan, all8, ctx->compute)
+															   : cg_launch_scan(ctx, plan, all8, ctx->compute);
+	return rc ? rc : after_launch(ctx, into, false, false, rows);
+}
+
+/* the statistics counters before a scan (its statistics are the difference) */
+static int stats_begin(CgContext *ctx, CgPartial *p, const CgScanStats *stats, unsigned long long before[3])
+{
+	before[0] = before[1] = before[2] = 0;
+	if (!stats) return CG_OK;
+	CG_CUDA(cudaMemcpyAsync(before, p->d_stats, 3 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->compute));
+	CG_CUDA(cudaStreamSynchronize(ctx->compute));
+	return CG_OK;
+}
+
+/* surfaces kernel-raised errors and fills *stats; kernel_ms = ev_a .. ev_b, recorded when chunk groups were scanned */
+static int stats_end(CgContext *ctx, CgPartial *p, const unsigned long long before[3], int64_t filtered, uint64_t scanned,
+					 uint64_t bytes, CgScanStats *stats)
+{
+	if (!stats) return CG_OK;
+	memset(stats, 0, sizeof *stats);
 	unsigned long long after[3];
 	CG_CUDA(cudaMemcpyAsync(after, p->d_stats, sizeof after, cudaMemcpyDeviceToHost, ctx->compute));
 	CG_CUDA(cudaStreamSynchronize(ctx->compute));
 	int rc = check_error_flags(p, after[2]);
 	if (rc) return rc;
-	if (stats)
+	stats->rows_scanned = (int64_t) (after[0] - before[0]);
+	stats->rows_removed_by_filter = (int64_t) (after[1] - before[1]);
+	stats->rows_passed = stats->rows_scanned - stats->rows_removed_by_filter;
+	stats->chunk_groups_filtered = filtered;
+	stats->chunk_groups_scanned = (int64_t) scanned;
+	stats->bytes_scanned = (int64_t) bytes;
+	if (scanned > 0)
 	{
-		stats->rows_scanned = (int64_t) (after[0] - before[0]);
-		stats->rows_removed_by_filter = (int64_t) (after[1] - before[1]);
-		stats->rows_passed = stats->rows_scanned - stats->rows_removed_by_filter;
+		float ms = 0;
+		CG_CUDA(cudaEventElapsedTime(&ms, ctx->ev_a, ctx->ev_b));
+		stats->kernel_ms = ms;
 	}
 	return CG_OK;
 }
@@ -1016,12 +1081,9 @@ extern "C" int cg_scan_shard(const CgShard *sh, const CgScanDesc *desc, CgPartia
 	if (stats)
 		for (uint32_t cg : selected)
 			for (int c = 0; c < plan.ncols; c++) bytes += sh->algorithmic_bytes_per_cg_col(cg, plan.slot[c]);
-	unsigned long long before[3] = {0, 0, 0};
-	if (stats)
-	{
-		CG_CUDA(cudaMemcpyAsync(before, into->d_stats, sizeof before, cudaMemcpyDeviceToHost, ctx->compute));
-		CG_CUDA(cudaStreamSynchronize(ctx->compute));
-	}
+	unsigned long long before[3];
+	rc = stats_begin(ctx, into, stats, before);
+	if (rc) return rc;
 	if (!selected.empty())
 	{
 		plan.arena = sh->d_arena;
@@ -1030,85 +1092,43 @@ extern "C" int cg_scan_shard(const CgShard *sh, const CgScanDesc *desc, CgPartia
 		plan.selected = sh->d_selected;
 		plan.nselected = (uint32_t) selected.size();
 		plan.max_cg_rows = sh->sel_max_cg_rows;
-		FPlan fast;
-		const bool use_small = cg_small_eligible(plan) && !cg_force_general();
-		bool use_fast = !use_small && !cg_force_general() && cg_jit_level() < 2 && cg_build_fast_plan(desc, plan, all8, &fast);
-		/* the chunk groups without NULLs in the plan columns come first in the selection */
-		uint32_t nfast = sh->sel_nfast;
+		FPlan fplan;
+		const FPlan *fast = fast_eligible(desc, plan, all8, &fplan) ? &fplan : nullptr;
 		if (stats) CG_CUDA(cudaEventRecord(ctx->ev_a, ctx->compute));
 		rc = cg_prof_mark(ctx, ctx->compute);
 		if (rc) return rc;
-		if (use_fast && nfast > 0)
+		/* the chunk groups without NULLs in the plan columns come first in the selection; when no specialised kernel
+		 * takes them they join the rest */
+		KPlan rest = plan;
+		uint64_t rest_rows = sh->sel_rows_total;
+		if (sh->sel_nfast > 0)
 		{
-			fast.nselected = nfast;
-			rc = cg_launch_scan_fast(ctx, fast, ctx->compute);
+			KPlan prefix = plan;
+			prefix.nselected = sh->sel_nfast;
+			bool taken = false;
+			rc = scan_specialised(ctx, into, prefix, fast, 0u, sh->sel_rows_fast, &taken);
 			if (rc) return rc;
-			rc = after_launch(ctx, into, fast.packed != nullptr, fast.nsums == 1, sh->sel_rows_fast);
-			if (rc) return rc;
+			if (taken)
+			{
+				rest.selected += sh->sel_nfast;
+				rest.nselected -= sh->sel_nfast;
+				rest_rows -= sh->sel_rows_fast;
+			}
 		}
-		else if (nfast > 0 && !cg_force_general())
+		if (rest.nselected > 0)
 		{
-			/* no ahead-of-time specialisation for this shape: the plan-specialised (NVRTC) kernel */
-			KPlan piece = plan;
-			piece.nselected = nfast;
-			bool launched = false, packed = false, ponly = false;
-			rc = cg_launch_scan_jit(ctx, piece, 0u, ctx->compute, &launched, &packed, &ponly);
+			/* chunk groups with NULLs in a plan column: the generated kernel in its nullable form (exists bitmap + rank
+			 * directory addressing, columnar_reader.c:1506-1572); the interpretive kernels when it does not take them */
+			bool taken = false;
+			rc = scan_specialised(ctx, into, rest, nullptr, sh->sel_nullmask ? sh->sel_nullmask : ~0u, rest_rows, &taken);
+			if (rc == CG_OK && !taken) rc = scan_interpretive(ctx, into, rest, all8, rest_rows);
 			if (rc) return rc;
-			if (launched)
-			{
-				rc = after_launch(ctx, into, packed, ponly, sh->sel_rows_fast);
-				if (rc) return rc;
-			}
-			if (!launched) nfast = 0;
-		}
-		else
-			nfast = 0;
-		if (nfast < plan.nselected)
-		{
-			/* chunk groups with NULLs in a plan column: the plan-specialised kernel in its nullable form
-			 * (exists bitmap + rank directory addressing, columnar_reader.c:1506-1572); the interpretive
-			 * kernels only when the JIT is off or unavailable */
-			plan.selected = sh->d_selected + nfast;
-			plan.nselected -= nfast;
-			bool launched = false, packed = false, ponly = false;
-			if (!cg_force_general())
-			{
-				rc = cg_launch_scan_jit(ctx, plan, sh->sel_nullmask ? sh->sel_nullmask : ~0u, ctx->compute, &launched, &packed, &ponly);
-				if (rc) return rc;
-				if (launched)
-				{
-					rc = after_launch(ctx, into, packed, ponly, sh->sel_rows_total - sh->sel_rows_fast);
-					if (rc) return rc;
-				}
-			}
-			if (!launched)
-			{
-				if (use_small) rc = cg_launch_scan_small(ctx, plan, all8, ctx->compute);
-				else rc = cg_launch_scan(ctx, plan, true, all8, ctx->compute);
-				if (rc) return rc;
-				into->wide_dirty = true;
-			}
 		}
 		rc = cg_prof_mark(ctx, ctx->compute);
 		if (rc) return rc;
 		if (stats) CG_CUDA(cudaEventRecord(ctx->ev_b, ctx->compute));
 	}
-	if (stats)
-	{
-		memset(stats, 0, sizeof *stats);
-		rc = read_stats(ctx, into, before, stats);
-		if (rc) return rc;
-		stats->chunk_groups_filtered = filtered;
-		stats->chunk_groups_scanned = (int64_t) selected.size();
-		stats->bytes_scanned = (int64_t) bytes;
-		if (!selected.empty())
-		{
-			float ms = 0;
-			CG_CUDA(cudaEventElapsedTime(&ms, ctx->ev_a, ctx->ev_b));
-			stats->kernel_ms = ms;
-		}
-	}
-	return CG_OK;
+	return stats_end(ctx, into, before, filtered, selected.size(), bytes, stats);
 }
 
 /* ------------------------------------------------------------------------------ *
@@ -1306,12 +1326,9 @@ extern "C" int cg_scan_relation(const CgRelation *rel, const CgScanDesc *desc, C
 	size_t ns = staged.size();
 	uint64_t ncg = sp.cg_rows.size();
 
-	unsigned long long before[3] = {0, 0, 0};
-	if (stats)
-	{
-		CG_CUDA(cudaMemcpyAsync(before, into->d_stats, sizeof before, cudaMemcpyDeviceToHost, ctx->compute));
-		CG_CUDA(cudaStreamSynchronize(ctx->compute));
-	}
+	unsigned long long before[3];
+	rc = stats_begin(ctx, into, stats, before);
+	if (rc) return rc;
 	uint64_t bytes = 0;
 	for (uint64_t g = 0; g < ncg; g++)
 		for (int c = 0; c < plan.ncols; c++)
@@ -1396,11 +1413,8 @@ extern "C" int cg_scan_relation(const CgRelation *rel, const CgScanDesc *desc, C
 		plan.chunkcols = d_cols;
 		plan.nstaged = (int32_t) ns;
 		for (uint32_t r : sp.cg_rows) plan.max_cg_rows = std::max(plan.max_cg_rows, r);
-		FPlan fast;
-		const bool use_small = cg_small_eligible(plan) && !cg_force_general();
-		const bool use_fast = !use_small && !sp.any_nulls && !cg_force_general() && cg_jit_level() < 2 &&
-							  cg_build_fast_plan(desc, plan, all8, &fast);
-		const bool try_jit = !use_fast && !cg_force_general();
+		FPlan fplan;
+		const FPlan *fast = (!sp.any_nulls && fast_eligible(desc, plan, all8, &fplan)) ? &fplan : nullptr;
 		/* plan columns with NULLs somewhere in the planned chunk groups: the generated kernel takes the exists
 		 * bitmap + rank directory path for those (per chunk, uniformly), dense loads everywhere else */
 		uint32_t nullable = 0;
@@ -1434,42 +1448,13 @@ extern "C" int cg_scan_relation(const CgRelation *rel, const CgScanDesc *desc, C
 			}
 			r = cg_prof_mark(ctx, ctx->compute);
 			if (r) return r;
-			bool jitted = false;
-			if (try_jit)
-			{
-				KPlan blk = plan;
-				blk.selected = d_ids + cg0;
-				blk.nselected = (uint32_t) (cg1 - cg0);
-				bool packed = false, ponly = false;
-				r = cg_launch_scan_jit(ctx, blk, nullable, ctx->compute, &jitted, &packed, &ponly);
-				if (r) return r;
-				if (jitted) { r = after_launch(ctx, into, packed, ponly, block_rows(cg0, cg1)); if (r) return r; }
-			}
-			if (jitted) { }
-			else if (use_small)
-			{
-				KPlan blk = plan;
-				blk.selected = d_ids + cg0;
-				blk.nselected = (uint32_t) (cg1 - cg0);
-				r = cg_launch_scan_small(ctx, blk, all8, ctx->compute);
-				into->wide_dirty = true;
-			}
-			else if (use_fast)
-			{
-				FPlan blk = fast;
-				blk.selected = d_ids + cg0;
-				blk.nselected = (uint32_t) (cg1 - cg0);
-				r = cg_launch_scan_fast(ctx, blk, ctx->compute);
-				if (r == CG_OK) r = after_launch(ctx, into, blk.packed != nullptr, blk.nsums == 1, block_rows(cg0, cg1));
-			}
-			else
-			{
-				KPlan blk = plan;
-				blk.selected = d_ids + cg0;
-				blk.nselected = (uint32_t) (cg1 - cg0);
-				r = cg_launch_scan(ctx, blk, sp.any_nulls, all8, ctx->compute);
-				into->wide_dirty = true;
-			}
+			KPlan blk = plan;
+			blk.selected = d_ids + cg0;
+			blk.nselected = (uint32_t) (cg1 - cg0);
+			const uint64_t rows = block_rows(cg0, cg1);
+			bool taken = false;
+			r = scan_specialised(ctx, into, blk, fast, nullable, rows, &taken);
+			if (r == CG_OK && !taken) r = scan_interpretive(ctx, into, blk, all8, rows);
 			if (r) return r;
 			return cg_prof_mark(ctx, ctx->compute);
 		};
@@ -1555,24 +1540,12 @@ extern "C" int cg_scan_relation(const CgRelation *rel, const CgScanDesc *desc, C
 		CG_CUDA(cudaEventRecord(ctx->dma_done[mslot], ctx->compute));
 		slot_guard.armed = false;
 	}
-	if (stats)
-	{
-		memset(stats, 0, sizeof *stats);
-		rc = read_stats(ctx, into, before, stats);
-		if (rc) return rc;
-		stats->chunk_groups_filtered = filtered;
-		stats->chunk_groups_scanned = (int64_t) ncg;
-		stats->bytes_scanned = (int64_t) bytes;
-		if (ncg > 0)
-		{
-			float ms = 0;
-			CG_CUDA(cudaEventElapsedTime(&ms, ctx->ev_a, ctx->ev_b));
-			stats->kernel_ms = ms;   /* here: first kernel start to last kernel end, H2D overlapped */
-			stats->h2d_bytes = (int64_t) ((used_dma ? dma_bytes + 2 * ncg * ns * sizeof(RealignItem) : sp.wire_bytes) +
-										  sp.cols.size() * sizeof(DevChunkCol) + ncg * sizeof(uint32_t) +
-										  sp.decode.size() * sizeof(DecodeItem));
-		}
-	}
+	/* kernel_ms here: first kernel start to last kernel end, H2D overlapped */
+	rc = stats_end(ctx, into, before, filtered, ncg, bytes, stats);
+	if (rc) return rc;
+	if (stats && ncg > 0)
+		stats->h2d_bytes = (int64_t) ((used_dma ? dma_bytes + 2 * ncg * ns * sizeof(RealignItem) : sp.wire_bytes) +
+									  sp.cols.size() * sizeof(DevChunkCol) + ncg * sizeof(uint32_t) + sp.decode.size() * sizeof(DecodeItem));
 	return CG_OK;
 }
 

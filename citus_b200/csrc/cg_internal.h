@@ -372,7 +372,7 @@ struct CgPartial
 };
 
 /* cg_scan.cu */
-int cg_launch_scan(CgContext *ctx, const KPlan &plan, bool any_nulls, bool all8, cudaStream_t stream);
+int cg_launch_scan(CgContext *ctx, const KPlan &plan, bool all8, cudaStream_t stream);
 /* one chunk buffer to move from the raw (page-payload) device buffer to its aligned arena slot */
 struct RealignItem
 {

@@ -41,12 +41,7 @@ __device__ __forceinline__ uint64_t *find_entry(const KPlan &P, int64_t key, boo
 	if (MODE == CG_MODE_DENSE)
 	{
 		uint64_t slot = dense_slot_of_packed(P, key, key_null);
-		if (slot == ~0ull)
-		{
-			atomicOr(P.stats + 2, CG_ERRFLAG_KEY_RANGE);
-			return nullptr;
-		}
-		return P.table + slot * (uint64_t) P.stride;
+		return slot == ~0ull ? nullptr : P.table + slot * (uint64_t) P.stride;
 	}
 	else
 	{
@@ -84,125 +79,29 @@ __device__ __forceinline__ void process_row(const KPlan &P, const int64_t (&v)[N
 											ThreadAcc<NAC> &acc, uint32_t &removed)
 {
 	/* K3: WHERE tree, three-valued: an atom on a NULL input is not TRUE */
-	const bool pass = eval_where<NCC>(P, v, nullmask);
-	if (!pass)
+	if (!eval_where<NCC>(P, v, nullmask))
 	{
 		removed++;
 		return;
 	}
-
-	uint64_t *entry = nullptr;
 	if (MODE != CG_MODE_GLOBAL)
 	{
 		int64_t key;
 		bool key_null;
-		if (P.ngroup == 1)
-		{
-			int c = P.gcol[0];
-			key_null = (nullmask >> c) & 1u;
-			key = pick<NCC>(v, c);
-		}
+		if (!group_key<NCC>(P, v, nullmask, key, key_null)) return;
+		uint64_t *entry = find_entry<MODE>(P, key, key_null);
+		if (entry != nullptr) global_accumulate<NCC, NAC>(P, entry, v, nullmask);
+		return;
+	}
+	acc.rows++;
+	row_terms<NCC, NAC>(P, v, nullmask, [&](int a, const KAgg &g, bool noinput, uint64_t w0, uint64_t w1) {
+		if (noinput) acc.w[a][2]++;
 		else
 		{
-			int c0 = P.gcol[0], c1 = P.gcol[1];
-			if (((nullmask >> c0) | (nullmask >> c1)) & 1u)
-			{
-				atomicOr(P.stats + 2, CG_ERRFLAG_NULL_MULTIKEY);
-				return;
-			}
-			key_null = false;
-			key = (int64_t) ((uint64_t) (uint32_t) pick<NCC>(v, c0) | ((uint64_t) (uint32_t) pick<NCC>(v, c1) << 32));
+			acc.w[a][0] = word_combine(P.wordop[g.word0], acc.w[a][0], w0);
+			if (two_limbs(g)) acc.w[a][1] += w1;
 		}
-		entry = find_entry<MODE>(P, key, key_null);
-		if (entry == nullptr) return;
-		atomicAdd((unsigned long long *) entry, 1ull);
-	}
-	else
-		acc.rows++;
-
-	/* aggregate FILTERs: a rejected row is no input of its aggregate, counted like a NULL input; so is a row whose
-	 * bool_and / bool_or argument is UNKNOWN */
-	uint32_t argtrue;
-	const uint32_t rejected = eval_filters<NCC>(P, v, nullmask, &argtrue);
-
-	/* K4: transition functions */
-#pragma unroll
-	for (int a = 0; a < NAC; a++)
-	{
-		if (a < P.naggs)
-		{
-			const KAgg &g = P.aggs[a];
-			bool isnull = (rejected >> a) & 1u;
-			if (g.kind == CG_AGG_COUNT_STAR)
-			{
-				if (isnull)
-				{
-					if (MODE == CG_MODE_GLOBAL) acc.w[a][2]++;
-					else atomicAdd((unsigned long long *) entry + g.nullword, 1ull);
-				}
-				continue;
-			}
-			int64_t it = 1;
-			double ft = 1.0;
-#pragma unroll
-			for (int f = 0; f < 3; f++)
-			{
-				if (f < g.nfactors)
-				{
-					int c = g.pcol[f];
-					isnull = isnull || ((nullmask >> c) & 1u);
-					if (g.is_float)
-						ft *= __longlong_as_double(g.a[f]) + __longlong_as_double(g.b[f]) * __longlong_as_double(pick<NCC>(v, c));
-				}
-			}
-			if (!g.is_float) it = int_term<NCC>(g, v, isnull, P.stats);
-			if (isnull)
-			{
-				/* strict transition function: a NULL input is skipped, only counted */
-				if (MODE == CG_MODE_GLOBAL) acc.w[a][2]++;
-				else atomicAdd((unsigned long long *) entry + g.nullword, 1ull);
-				continue;
-			}
-			if (g.kind == CG_AGG_COUNT) continue;   /* count(x) = rows - NULL inputs */
-			uint64_t w0, w1 = 0;
-			if (g.kind == CG_AGG_SUM)
-			{
-				if (g.is_float) w0 = (uint64_t) __double_as_longlong(ft);
-				else if (g.nlimbs == 1)
-				{
-					if (it > g.bound || it < -g.bound) atomicOr(P.stats + 2, CG_ERRFLAG_SUM_BOUND);
-					w0 = (uint64_t) it;
-				}
-				else { w0 = (uint64_t) (uint32_t) it; w1 = (uint64_t) (it >> 32); }
-			}
-			else if (g.barg) /* BOOL_AND / BOOL_OR: TRUE = all ones */
-				w0 = ((argtrue >> a) & 1u) ? ~0ull : 0ull;
-			else /* MIN / MAX, BIT_AND / BIT_OR (the sign-extended column value) */
-				w0 = g.is_float ? f8_ordered(__double_as_longlong(ft)) : (uint64_t) it;
-			const bool two = (g.kind == CG_AGG_SUM && !g.is_float && g.nlimbs == 2);
-			if (MODE == CG_MODE_GLOBAL)
-			{
-				acc.w[a][0] = word_combine(P.wordop[g.word0], acc.w[a][0], w0);
-				if (two) acc.w[a][1] += w1;
-			}
-			else
-			{
-				word_apply_global(entry + g.word0, P.wordop[g.word0], w0);
-				if (two) atomicAdd((unsigned long long *) entry + g.word0 + 1, (unsigned long long) w1);
-			}
-		}
-	}
-}
-
-__device__ __forceinline__ uint64_t warp_reduce_word(uint64_t x, int op)
-{
-#pragma unroll
-	for (int o = 16; o > 0; o >>= 1)
-	{
-		uint64_t y = __shfl_xor_sync(0xffffffffu, x, o);
-		x = word_combine(op, x, y);
-	}
-	return x;
+	});
 }
 
 /*
@@ -292,8 +191,7 @@ cg_scan_kernel(const __grid_constant__ KPlan P)
 		}
 		else
 		{
-			/* chunk group with NULLs: row -> value index through the rank directory
-			 * (NULL rows occupy no bytes in the value stream, columnar_reader.c:1550-1555) */
+			/* chunk group with NULLs: the NULL-bearing columns through their rank directories */
 			for (uint32_t r = tid * 2; r < rows; r += CG_THREADS * 2)
 			{
 				int64_t v0[NCC], v1[NCC];
@@ -303,20 +201,10 @@ cg_scan_kernel(const __grid_constant__ KPlan P)
 					if (c < P.ncols)
 					{
 						int len = ALL8 ? 8 : P.len[c];
-						bool isf = P.isfloat[c];
 						if ((hasnull >> c) & 1u)
-						{
-							uint64_t w = ldg_stream8(bptr[c] + (r >> 6));
-							uint32_t sh = r & 63u;
-							uint32_t before = __ldg(rptr[c] + (r >> 6)) + __popcll(w & ((1ull << sh) - 1ull));
-							uint32_t e0 = (uint32_t) (w >> sh) & 1u, e1 = (uint32_t) (w >> (sh + 1)) & 1u;
-							v0[c] = e0 ? load_scalar(vptr[c] + (uint64_t) before * len, len, isf) : 0;
-							v1[c] = (e1 && r + 1 < rows) ? load_scalar(vptr[c] + (uint64_t) (before + e0) * len, len, isf) : 0;
-							n0 |= (e0 ^ 1u) << c;
-							n1 |= (e1 ^ 1u) << c;
-						}
+							load_pair_nullable(vptr[c], bptr[c], rptr[c], r, rows, len, P.isfloat[c], c, v0[c], v1[c], n0, n1);
 						else
-							load_pair(vptr[c], r, len, isf, v0[c], v1[c]);
+							load_pair(vptr[c], r, len, P.isfloat[c], v0[c], v1[c]);
 					}
 				process_row<NCC, NAC, MODE>(P, v0, n0, acc, removed);
 				if (r + 1 < rows) process_row<NCC, NAC, MODE>(P, v1, n1, acc, removed);
@@ -352,7 +240,7 @@ cg_scan_kernel(const __grid_constant__ KPlan P)
 					if (g.kind != CG_AGG_COUNT && g.kind != CG_AGG_COUNT_STAR)
 					{
 						if (x0 != word_identity(P.wordop[g.word0])) word_apply_global(P.table + g.word0, P.wordop[g.word0], x0);
-						if (g.kind == CG_AGG_SUM && !g.is_float && g.nlimbs == 2 && x1)
+						if (two_limbs(g) && x1)
 							atomicAdd((unsigned long long *) P.table + g.word0 + 1, (unsigned long long) x1);
 					}
 				}
@@ -398,9 +286,8 @@ static int launch_mode(CgContext *ctx, const KPlan &plan, bool all8, cudaStream_
 	}
 }
 
-int cg_launch_scan(CgContext *ctx, const KPlan &plan, bool any_nulls, bool all8, cudaStream_t stream)
+int cg_launch_scan(CgContext *ctx, const KPlan &plan, bool all8, cudaStream_t stream)
 {
-	(void) any_nulls;
 	if (plan.ncols <= 2) return launch_mode<2>(ctx, plan, all8, stream);
 	if (plan.ncols <= 4) return launch_mode<4>(ctx, plan, all8, stream);
 	return launch_mode<CG_KMAX_COLS>(ctx, plan, all8, stream);
@@ -849,7 +736,7 @@ __global__ void cg_merge_kernel(const __grid_constant__ KPlan P, const int64_t *
 	 * (bits 32..63) moves to the high word, so the table's low word grows by < 2^32 per merged row */
 	uint32_t lo_words = 0;
 	for (int a = 0; a < P.naggs; a++)
-		if (P.aggs[a].kind == CG_AGG_SUM && !P.aggs[a].is_float && P.aggs[a].nlimbs == 2) lo_words |= 1u << P.aggs[a].word0;
+		if (two_limbs(P.aggs[a])) lo_words |= 1u << P.aggs[a].word0;
 	for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < nrows; i += (int64_t) gridDim.x * blockDim.x)
 	{
 		uint64_t *entry;
