@@ -1144,9 +1144,11 @@ extern "C" int cg_partition_copy_serialize(const int32_t *d_index, int64_t n, in
 	CgAsyncBuf len_buf, block_buf, tot_buf;
 	CG_CUDA(len_buf.alloc(sizeof(uint32_t) * (size_t) std::max<int64_t>(n, 1), ctx->compute));
 	CG_CUDA(block_buf.alloc(sizeof(unsigned long long) * (size_t) std::max<int64_t>(nblocks, 1) * P, ctx->compute));
-	CG_CUDA(tot_buf.alloc(sizeof(unsigned long long) * (4 * (size_t) P + 4), ctx->compute));
+	/* [P] totals, [P] row starts, [P] file begins, [P] file ends (8 bytes each), then present[P] (one byte each) */
+	const size_t tot_bytes = sizeof(unsigned long long) * 4 * (size_t) P + (size_t) P;
+	CG_CUDA(tot_buf.alloc(tot_bytes, ctx->compute));
 	unsigned long long *d_tot = tot_buf.as<unsigned long long>();
-	CG_CUDA(cudaMemsetAsync(d_tot, 0, sizeof(unsigned long long) * (4 * (size_t) P + 4), ctx->compute));
+	CG_CUDA(cudaMemsetAsync(d_tot, 0, tot_bytes, ctx->compute));
 	CopyWriteParams A;
 	memset(&A, 0, sizeof A);
 	A.index = d_index; A.n = n; A.P = P; A.ncols = ncols; A.binary = binary ? 1 : 0;

@@ -476,7 +476,9 @@ int cg_comm_combine(CgPartial *p, int32_t root, int32_t local_status);
  * all-to-all at once -- rows leave shared memory as runs straight into the owner's receive buffer.  NCCL path:
  * scatter into destination-major order and one grouped ncclSend/ncclRecv of all columns on a second stream, so
  * that the next table's routing and scatter overlap this table's exchange.  Results live in the slot (0..3)
- * until its next use. */
+ * until its next use.  A NULL key (d_key_nulls[i] != 0) routes its row to partition 0, but the received table carries
+ * only the value columns, so the receiver cannot tell that row's key slot from a real key: a join over the received
+ * rows would match it on whatever value the slot holds. */
 int cg_comm_repartition_exchange(int32_t slot, const int64_t *const *d_cols, const uint8_t *d_key_nulls, int64_t n,
 								 int32_t ncols, int32_t key_len, int32_t P, const int32_t *mins, const int32_t *maxs,
 								 int64_t *recv_rows);
