@@ -565,8 +565,10 @@ cg_lz4_lane_kernel(uint8_t *arena, const DecodeItem *items, uint32_t nitems, uns
 
 static int g_lz4_lanes = -1;
 static int g_lz4_lane_warps = 64;         /* > 0: as few streams per warp as fit into that many warps per SM, each lane on its own; 0: 32 streams per warp in step (probe) */
+static int g_zstd_coop = -1;              /* 1: zstd_frame_coop (default), 0: zs_decode_frame on one lane; < 0: CG_ZSTD_COOP, else 1 */
 void cg_decompress_set_lz4_lane_warps(int n) { g_lz4_lane_warps = n < 0 ? 0 : n > 64 ? 64 : n; }
 void cg_decompress_set_lz4_lanes(int on) { g_lz4_lanes = on < 0 ? -1 : (on > 1 ? 2 : on); }      /* < 0: back to the default */
+void cg_decompress_set_zstd_coop(int on) { g_zstd_coop = on < 0 ? -1 : (on ? 1 : 0); }         /* < 0: back to the default */
 
 /* h_items: the host copy of the same items (which kernels are needed) */
 int cg_launch_decompress(CgContext *ctx, uint8_t *arena, const DecodeItem *items, const DecodeItem *h_items, uint64_t nitems,
@@ -635,9 +637,8 @@ int cg_launch_decompress(CgContext *ctx, uint8_t *arena, const DecodeItem *items
 			ctx->zstd_scratch_bytes = need;
 		}
 		unsigned blocks = (unsigned) std::min<uint64_t>(nitems, max_blocks);
-		static int coop = -1;
-		if (coop < 0) { const char *e = getenv("CG_ZSTD_COOP"); coop = e ? atoi(e) : 1; }
-		cg_zstd_kernel<<<blocks, 32, 0, stream>>>(arena, items, (uint32_t) nitems, ctx->zstd_scratch, err, flag, coop);
+		if (g_zstd_coop < 0) { const char *e = getenv("CG_ZSTD_COOP"); g_zstd_coop = (e && atoi(e) == 0) ? 0 : 1; }
+		cg_zstd_kernel<<<blocks, 32, 0, stream>>>(arena, items, (uint32_t) nitems, ctx->zstd_scratch, err, flag, g_zstd_coop);
 		CG_CUDA(cudaGetLastError()); g_cg_launches++;
 	}
 	return CG_OK;

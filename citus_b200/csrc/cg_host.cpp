@@ -852,7 +852,8 @@ static bool cg_force_general(void)
 /* run-time switches (the same ones the CG_* environment variables set at first use): which kernel family
  * scans -- "jit" 0 = ahead-of-time kernels only, 1 = plan-specialised where no ahead-of-time specialisation
  * applies (default), 2 = always; "force_general" 1 = the interpretive kernels for everything; "lz4_lanes" 1 / 0 = LZ4 value
- * streams are decoded a lane per stream / eight lanes per stream, 2 or < 0 = by launch size (default); "peer_window" 0 = the
+ * streams are decoded a lane per stream / eight lanes per stream, 2 or < 0 = by launch size (default); "zstd_coop" 0 = Zstandard
+ * frames are decoded by one lane, 1 or < 0 = by the whole warp (default); "peer_window" 0 = the
  * combine and the repartition exchange stay on NCCL instead of the IPC-mapped peer window (set it on every rank) */
 extern "C" int cg_set_option(const char *name, int64_t value)
 {
@@ -862,6 +863,7 @@ extern "C" int cg_set_option(const char *name, int64_t value)
 	if (strcmp(name, "realign_tma") == 0) { cg_realign_set_tma((int) value); return CG_OK; }
 	if (strcmp(name, "lz4_lanes") == 0) { cg_decompress_set_lz4_lanes((int) value); return CG_OK; }
 	if (strcmp(name, "lz4_lane_warps") == 0) { cg_decompress_set_lz4_lane_warps((int) value); return CG_OK; }
+	if (strcmp(name, "zstd_coop") == 0) { cg_decompress_set_zstd_coop((int) value); return CG_OK; }
 	if (strcmp(name, "peer_window") == 0) { cg_comm_set_peer_window((int) value); return CG_OK; }     /* the same value on every rank */
 	return cg_set_error(CG_EINVAL, "unknown option %s", name);
 }

@@ -397,6 +397,7 @@ struct DecodeItem
 };
 void cg_decompress_set_lz4_lanes(int on);
 void cg_decompress_set_lz4_lane_warps(int n);
+void cg_decompress_set_zstd_coop(int on);
 int cg_launch_decompress(CgContext *ctx, uint8_t *arena, const DecodeItem *items, const DecodeItem *h_items, uint64_t nitems,
 						 unsigned long long *err, unsigned long long flag, cudaStream_t stream);
 

@@ -66,6 +66,7 @@ uint64_t cg_jit_compiles(void);
  *   "realign_tma" 0 | 1                         cp.async.bulk or plain-load form of the page realign kernel
  *   "lz4_lanes" 0 | 1 | 2 (< 0 = default = 2)    LZ4 streams: eight lanes per stream | a lane per stream | by launch size
  *   "lz4_lane_warps" n                          (probe) warps per SM the lane-per-stream kernel spreads a launch over
+ *   "zstd_coop" 0 | 1 (< 0 = default = 1)       Zstandard frames: one lane decodes a frame | the warp cooperates on it
  *   "peer_window" 0 | 1                         exchange steps over NCCL | over the IPC-mapped peer window; the same
  *                                               value on every rank
  * An unknown name is CG_EINVAL. */

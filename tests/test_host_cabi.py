@@ -266,7 +266,8 @@ def test_jit_generates_valid_sm90a_code_for_every_plan_form(cg):
 def test_run_time_options_are_named(cg):
     """cg_set_option: every documented switch is accepted, anything else is an error (no silent typos)"""
     from citus_b200 import capi
-    for name, value in (("jit", 1), ("force_general", 0), ("realign_tma", 1), ("peer_window", 1), ("lz4_lanes", -1), ("lz4_lane_warps", 64)):
+    for name, value in (("jit", 1), ("force_general", 0), ("realign_tma", 1), ("peer_window", 1), ("lz4_lanes", -1), ("lz4_lane_warps", 64),
+                        ("zstd_coop", 0), ("zstd_coop", -1)):
         cg.set_option(name, value)
     with pytest.raises(capi.CitusGpuError) as e:
         cg.set_option("lz4_lane", 1)
