@@ -24,7 +24,7 @@ CG_AGG_BIT_AND, CG_AGG_BIT_OR, CG_AGG_BOOL_AND, CG_AGG_BOOL_OR = range(5, 9)
 CG_WORD_ADD, CG_WORD_MIN, CG_WORD_MAX, CG_WORD_FADD, CG_WORD_FMIN, CG_WORD_FMAX = range(6)
 CG_WORD_AND, CG_WORD_OR = 6, 7
 CG_GEN_UNIFORM, CG_GEN_SEQUENCE = 0, 1
-CG_MAX_QUALS, CG_MAX_AGGS, CG_MAX_GROUP_COLS = 8, 8, 2
+CG_MAX_QUALS, CG_MAX_AGGS, CG_MAX_GROUP_COLS = 8, 8, 4
 CG_MAX_QEXPR, CG_QX_AND, CG_QX_OR = 16, -1, -2
 CG_MAX_FILTER_QUALS = 8
 
@@ -79,7 +79,9 @@ class CgScanDesc(C.Structure):
                 ("nqual_expr", C.c_int32), ("qual_expr", C.c_int8 * CG_MAX_QEXPR), ("reserved", C.c_int32),
                 ("nfilter_quals", C.c_int32), ("filter_quals", CgQual * CG_MAX_FILTER_QUALS),
                 ("nfilter_expr", C.c_int32 * CG_MAX_AGGS), ("filter_expr", (C.c_int8 * CG_MAX_QEXPR) * CG_MAX_AGGS),
-                ("narg_expr", C.c_int32 * CG_MAX_AGGS), ("arg_expr", (C.c_int8 * CG_MAX_QEXPR) * CG_MAX_AGGS)]
+                ("narg_expr", C.c_int32 * CG_MAX_AGGS), ("arg_expr", (C.c_int8 * CG_MAX_QEXPR) * CG_MAX_AGGS),
+                ("composite_key", C.c_int32), ("key_col_min", C.c_int64 * CG_MAX_GROUP_COLS),
+                ("key_col_max", C.c_int64 * CG_MAX_GROUP_COLS)]
 
 
 class CgScanStats(C.Structure):
@@ -146,6 +148,9 @@ SYMBOLS = [
     ("cg_partition_scatter_ordered", C.c_int, [_P, C.c_int64, C.c_int32, _P, _P, C.c_int32, _P, _P]),
     ("cg_relation_bounds", C.c_int, [C.POINTER(CgRelation), C.POINTER(CgScanDesc), C.POINTER(C.c_int64),
                                      C.POINTER(C.c_int64), _P, C.POINTER(C.c_int64)]),
+    ("cg_relation_key_bounds", C.c_int, [C.POINTER(CgRelation), C.POINTER(CgScanDesc), _P, _P]),
+    ("cg_group_key_decode", C.c_int, [C.POINTER(CgScanDesc), C.c_int64, _P, _P, _P]),
+    ("cg_group_key_encode", C.c_int, [C.POINTER(CgScanDesc), C.c_int64, _P, _P, _P]),
     ("cg_selected_chunk_mask", C.c_int, [C.POINTER(CgRelation), C.c_int32, C.POINTER(CgScanDesc), _P,
                                          C.POINTER(C.c_int64)]),
     ("cg_numeric_out", C.c_int, [C.c_int64, C.c_uint64, C.c_int32, C.c_char_p, C.c_size_t]),

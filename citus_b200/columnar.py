@@ -287,8 +287,17 @@ def _set_atom(q, atom, float_cols):
     q.konst = int(np.float64(k).view(np.int64)) if col in float_cols else int(k)
 
 
-def make_desc(quals=(), group_cols=(), aggs=(), qual_pushdown=True, expected_groups=0, float_cols=()):
+def make_desc(quals=(), group_cols=(), aggs=(), qual_pushdown=True, expected_groups=0, float_cols=(), composite=False,
+              key_bounds=None):
+    """composite=True: the GROUP BY key is the exact mixed-radix code over group_cols (1..4 columns, NULLs included);
+    key_bounds = [(min, max)] per group column (relation_key_bounds; min > max = the column is always NULL)"""
     d = CgScanDesc()
+    if composite:
+        d.composite_key = 1
+        if key_bounds is None or len(key_bounds) != len(group_cols):
+            raise ValueError("a composite key needs one (min, max) per group column")
+        for i, (lo, hi) in enumerate(key_bounds):
+            d.key_col_min[i], d.key_col_max[i] = lo, hi
     quals, tokens = flatten_where(quals)
     if len(quals) > capi.CG_MAX_QUALS or len(tokens) > capi.CG_MAX_QEXPR:
         raise capi.CitusGpuError(capi.CG_EUNSUPPORTED, "WHERE tree too large")
@@ -341,6 +350,38 @@ def relation_bounds(rel: Relation, desc: CgScanDesc):
     bounds = (C.c_int64 * capi.CG_MAX_AGGS)()
     check(lib().cg_relation_bounds(C.byref(rel.view), C.byref(desc), C.byref(kmin), C.byref(kmax), bounds, C.byref(rows)))
     return kmin.value, kmax.value, [bounds[i] for i in range(desc.naggs)], rows.value
+
+
+def relation_key_bounds(rel: Relation, desc: CgScanDesc):
+    """[(min, max)] of every group column over the chunk groups that survive skipping (min > max: no value)"""
+    k = desc.ngroup_cols
+    lo, hi = (C.c_int64 * capi.CG_MAX_GROUP_COLS)(), (C.c_int64 * capi.CG_MAX_GROUP_COLS)()
+    check(lib().cg_relation_key_bounds(C.byref(rel.view), C.byref(desc), lo, hi))
+    return [(lo[i], hi[i]) for i in range(k)]
+
+
+def group_key_decode(desc: CgScanDesc, codes):
+    """composite codes -> list of key tuples (None = NULL)"""
+    codes = np.ascontiguousarray(codes, np.int64)
+    n, k = codes.shape[0], desc.ngroup_cols
+    values, nulls = np.zeros(n * k, np.int64), np.zeros(n * k, np.uint8)
+    check(lib().cg_group_key_decode(C.byref(desc), n, codes.ctypes.data, values.ctypes.data, nulls.ctypes.data))
+    return [tuple(None if nulls[i * k + c] else int(values[i * k + c]) for c in range(k)) for i in range(n)]
+
+
+def group_key_encode(desc: CgScanDesc, keys):
+    """key tuples (None = NULL) -> composite codes (int64 array)"""
+    n, k = len(keys), desc.ngroup_cols
+    values, nulls = np.zeros(n * k, np.int64), np.zeros(n * k, np.uint8)
+    for i, key in enumerate(keys):
+        for c, v in enumerate(key):
+            if v is None:
+                nulls[i * k + c] = 1
+            else:
+                values[i * k + c] = v
+    codes = np.zeros(n, np.int64)
+    check(lib().cg_group_key_encode(C.byref(desc), n, values.ctypes.data, nulls.ctypes.data, codes.ctypes.data))
+    return codes
 
 
 class Shard:
@@ -455,8 +496,10 @@ class GpuColumnarAgg:
                     minmax=mm[:n * na].reshape(n, na), fsum=fs[:n * na].reshape(n, na))
 
     def groups(self):
-        """same shape as oracle.Result.groups(): key (None = NULL group) -> per-aggregate dicts"""
+        """same shape as oracle.Result.groups(): key (None = NULL group) -> per-aggregate dicts.  A composite partial's
+        keys are tuples with None for NULL (the shape tests/reference.py produces)"""
         f = self.fetch()
+        keys = group_key_decode(self.desc, f["keys"]) if self.desc.composite_key else None
         out = {}
         for i in range(f["n"]):
             per = []
@@ -464,8 +507,23 @@ class GpuColumnarAgg:
                 s = (int(f["sum_hi"][i, a]) << 64) + int(f["sum_lo"][i, a])
                 per.append(dict(sum=s, count=int(f["count"][i, a]), minmax=int(f["minmax"][i, a]),
                                 fsum=float(f["fsum"][i, a])))
-            out[None if f["key_nulls"][i] else int(f["keys"][i])] = per
+            if keys is not None:
+                out[keys[i]] = per
+            else:
+                out[None if f["key_nulls"][i] else int(f["keys"][i])] = per
         return out
+
+    def merge_values(self, keys, key_nulls, sum_hi, sum_lo, count, minmax, fsum):
+        """cg_partial_merge_values over host rows laid out like fetch()'s.  For a composite partial, keys may be a list of
+        key tuples (None = NULL): they are encoded to codes and key_nulls is ignored"""
+        if self.desc.composite_key and len(keys) and isinstance(keys[0], tuple):
+            keys, key_nulls = group_key_encode(self.desc, keys), None
+        keys = np.ascontiguousarray(keys, np.int64)
+        arrs = [None if x is None else np.ascontiguousarray(x, t) for x, t in
+                ((key_nulls, np.uint8), (sum_hi, np.int64), (sum_lo, np.uint64), (count, np.int64), (minmax, np.int64),
+                 (fsum, np.float64))]
+        check(lib().cg_partial_merge_values(self.h, keys.shape[0], keys.ctypes.data,
+                                            *[None if x is None else x.ctypes.data for x in arrs]))
 
     # -- combine (device arrays are torch tensors or any object with data_ptr()) ---------
     def export_device(self, d_keys_ptr, d_nulls_ptr, d_words_ptr, capacity):

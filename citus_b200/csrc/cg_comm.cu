@@ -545,25 +545,29 @@ extern "C" int cg_comm_combine(CgPartial *p, int32_t root, int32_t local_status)
 		int st = local_status;
 		if (st == 0) st = cg_partial_ngroups(p, &nrows);
 		const size_t row_bytes = sizeof(int64_t) + sizeof(uint64_t) * (size_t) p->nwords + 8;   /* key + words + NULL flag (padded) */
-		int rc = comm_ensure_small((size_t) 2 * g_comm.nranks + 2);
+		/* per rank: status, rows, and the key codec (composite codes of different bounds must not be merged) */
+		int rc = comm_ensure_small((size_t) 3 * g_comm.nranks + 3);
 		if (rc) return rc;
-		g_comm.h_small[0] = st; g_comm.h_small[1] = nrows;
-		CG_CUDA(cudaMemcpyAsync(g_comm.d_small, g_comm.h_small, 2 * sizeof(int64_t), cudaMemcpyHostToDevice, g_comm.side));
-		CG_NCCL(g_nccl.AllGather(g_comm.d_small, g_comm.d_small + 2, 2, ncclInt64, g_comm.comm, g_comm.side));
-		CG_CUDA(cudaMemcpyAsync(g_comm.h_small + 2, g_comm.d_small + 2, 2 * sizeof(int64_t) * g_comm.nranks, cudaMemcpyDeviceToHost, g_comm.side));
+		g_comm.h_small[0] = st; g_comm.h_small[1] = nrows; g_comm.h_small[2] = (int64_t) cg_key_codec_id(&p->desc);
+		CG_CUDA(cudaMemcpyAsync(g_comm.d_small, g_comm.h_small, 3 * sizeof(int64_t), cudaMemcpyHostToDevice, g_comm.side));
+		CG_NCCL(g_nccl.AllGather(g_comm.d_small, g_comm.d_small + 3, 3, ncclInt64, g_comm.comm, g_comm.side));
+		CG_CUDA(cudaMemcpyAsync(g_comm.h_small + 3, g_comm.d_small + 3, 3 * sizeof(int64_t) * g_comm.nranks, cudaMemcpyDeviceToHost, g_comm.side));
 		CG_CUDA(cudaStreamSynchronize(g_comm.side));
 		std::vector<int64_t> rows(g_comm.nranks);
 		int failed = -1, failed_code = 0;
+		bool same_codec = true;
 		for (int r = 0; r < g_comm.nranks; r++)
 		{
-			rows[r] = g_comm.h_small[2 + 2 * r + 1];
-			if (g_comm.h_small[2 + 2 * r] != 0 && failed < 0) { failed = r; failed_code = (int) g_comm.h_small[2 + 2 * r]; }
+			rows[r] = g_comm.h_small[3 + 3 * r + 1];
+			if (g_comm.h_small[3 + 3 * r] != 0 && failed < 0) { failed = r; failed_code = (int) g_comm.h_small[3 + 3 * r]; }
+			if (g_comm.h_small[3 + 3 * r + 2] != g_comm.h_small[2]) same_codec = false;
 		}
 		if (failed >= 0)
 		{
 			if (failed == g_comm.rank) return failed_code;      /* own message is already set */
 			return cg_set_error(failed_code, "rank %d failed before the combine (code %d)", failed, failed_code);
 		}
+		if (!same_codec) return cg_set_error(CG_EINVAL, "the partials of the ranks do not share one layout (group key codec)");
 		/* layout of one rank's rows in the gather buffer: keys | words | nulls, each 16-byte aligned */
 		auto seg = [&](int64_t n, size_t *off_words, size_t *off_nulls) {
 			size_t k = ((size_t) n * sizeof(int64_t) + 15) & ~(size_t) 15;
@@ -626,7 +630,7 @@ extern "C" int cg_comm_combine(CgPartial *p, int32_t root, int32_t local_status)
 	int rc = comm_check_status();
 	if (rc) return rc;
 	int64_t agree[5] = {local_status, p->wide_dirty ? 1 : 0, p->packed_dirty ? 1 : 0,
-						(int64_t) (p->entries * 1000003ull + (uint64_t) p->stride * 31ull + (uint64_t) p->pack_shift),
+						(int64_t) (p->entries * 1000003ull + (uint64_t) p->stride * 31ull + (uint64_t) p->pack_shift + cg_key_codec_id(&p->desc)),
 						(g_comm.win_ok && g_comm.use_peer) ? 0 : 1};
 	int64_t lay_min = agree[3];
 	rc = comm_agree(agree, 5, ncclMax);

@@ -346,11 +346,36 @@ __device__ __forceinline__ uint64_t warp_reduce_word(uint64_t x, int op)
 	return x;
 }
 
-/* the group key of a row that passed WHERE: one column, or two packed (low / high 32 bits).  false = a NULL in a
- * two-column key: the row has no group here (CG_ERRFLAG_NULL_MULTIKEY raised) */
+/* the group key of a row that passed WHERE: the composite code, one column, or two packed (low / high 32 bits).  false =
+ * the row has no group here: a NULL in a packed two-column key (CG_ERRFLAG_NULL_MULTIKEY raised), or a composite key
+ * value outside its column's bounds (CG_ERRFLAG_KEY_RANGE raised) */
 template <int NCC>
 __device__ __forceinline__ bool group_key(const KPlan &P, const int64_t (&v)[NCC], uint32_t nullmask, int64_t &key, bool &key_null)
 {
+	if (P.composite)
+	{
+		uint64_t code = 0;
+		bool ok = true;
+#pragma unroll
+		for (int g = 0; g < CG_MAX_GROUP_COLS; g++)
+			if (g < P.ngroup)
+			{
+				const int c = P.gcol[g];
+				const uint64_t d = (uint64_t) pick<NCC>(v, c) - (uint64_t) P.kmin[g];
+				const bool isnull = (nullmask >> c) & 1u;
+				ok = ok && (isnull || d < P.kradix[g] - 1u);
+				const uint64_t digit = isnull ? 0u : d + 1u;
+				code = g ? code * P.kradix[g] + digit : digit;
+			}
+		if (!ok)
+		{
+			atomicOr(P.stats + 2, CG_ERRFLAG_KEY_RANGE);
+			return false;
+		}
+		key_null = false;
+		key = (int64_t) code;
+		return true;
+	}
 	if (P.ngroup == 1)
 	{
 		int c = P.gcol[0];
@@ -369,13 +394,13 @@ __device__ __forceinline__ bool group_key(const KPlan &P, const int64_t (&v)[NCC
 	return true;
 }
 
-/* direct index of a group key (group_key's packing); the NULL key -> `capacity`; ~0 = outside the declared domain
- * (CG_ERRFLAG_KEY_RANGE raised) */
+/* direct index of a group key (group_key's packing; a composite code is a one-column key with key_min 0); the NULL key
+ * -> `capacity`; ~0 = outside the declared domain (CG_ERRFLAG_KEY_RANGE raised) */
 __device__ __forceinline__ uint64_t dense_slot_of_packed(const KPlan &P, int64_t key, bool key_null)
 {
 	if (key_null) return P.capacity;
 	uint64_t s;
-	if (P.ngroup == 2)
+	if (P.ngroup == 2 && !P.composite)
 	{
 		uint64_t a = (uint64_t) (int64_t) (int32_t) (uint32_t) key - (uint64_t) P.key_min;
 		uint64_t b = (uint64_t) (int64_t) (int32_t) (uint32_t) ((uint64_t) key >> 32) - (uint64_t) P.key_min1;

@@ -371,14 +371,14 @@ extern "C" int cg_selected_chunk_mask(const CgRelation *rel, int32_t stripe_inde
 	return rc;
 }
 
-/* interval arithmetic over the skip lists of the chunk groups that survive skipping */
-extern "C" int cg_relation_bounds(const CgRelation *rel, const CgScanDesc *desc, int64_t *key_min, int64_t *key_max,
-								  int64_t *term_abs_bound, int64_t *rows)
+/* per-column min / max over the skip lists of the chunk groups that survive skipping (cmin > cmax: no value); unknown[c]
+ * = a surviving chunk of c has values but no min / max, or c is a float column */
+static int64_t column_bounds(const CgRelation *rel, const CgScanDesc *desc, std::vector<int64_t> &cmin, std::vector<int64_t> &cmax,
+							 std::vector<uint8_t> &unknown)
 {
-	int rc = validate_relation(rel);
-	if (rc) return rc;
-	std::vector<int64_t> cmin(rel->natts, INT64_MAX), cmax(rel->natts, INT64_MIN);
-	std::vector<uint8_t> unknown(rel->natts, 0);
+	cmin.assign(rel->natts, INT64_MAX);
+	cmax.assign(rel->natts, INT64_MIN);
+	unknown.assign(rel->natts, 0);
 	int64_t nrows = 0;
 	std::vector<uint8_t> mask;
 	for (int si = 0; si < rel->nstripes; si++)
@@ -406,6 +406,18 @@ extern "C" int cg_relation_bounds(const CgRelation *rel, const CgScanDesc *desc,
 			}
 		}
 	}
+	return nrows;
+}
+
+/* interval arithmetic over the skip lists of the chunk groups that survive skipping */
+extern "C" int cg_relation_bounds(const CgRelation *rel, const CgScanDesc *desc, int64_t *key_min, int64_t *key_max,
+								  int64_t *term_abs_bound, int64_t *rows)
+{
+	int rc = validate_relation(rel);
+	if (rc) return rc;
+	std::vector<int64_t> cmin, cmax;
+	std::vector<uint8_t> unknown;
+	const int64_t nrows = column_bounds(rel, desc, cmin, cmax, unknown);
 	if (rows) *rows = nrows;
 	if (key_min && key_max)
 	{
@@ -447,6 +459,27 @@ extern "C" int cg_relation_bounds(const CgRelation *rel, const CgScanDesc *desc,
 			}
 			if (ok) term_abs_bound[a] = bound == 0 ? 1 : (int64_t) bound;
 		}
+	return CG_OK;
+}
+
+extern "C" int cg_relation_key_bounds(const CgRelation *rel, const CgScanDesc *desc, int64_t *col_min, int64_t *col_max)
+{
+	int rc = validate_relation(rel);
+	if (rc) return rc;
+	if (!desc || !col_min || !col_max) return cg_set_error(CG_EINVAL, "NULL argument");
+	if (desc->ngroup_cols < 1 || desc->ngroup_cols > CG_MAX_GROUP_COLS) return cg_set_error(CG_EINVAL, "ngroup_cols %d out of range", desc->ngroup_cols);
+	for (int g = 0; g < desc->ngroup_cols; g++)
+		if (desc->group_cols[g] < 0 || desc->group_cols[g] >= rel->natts) return cg_set_error(CG_EINVAL, "group column %d out of range", desc->group_cols[g]);
+	std::vector<int64_t> cmin, cmax;
+	std::vector<uint8_t> unknown;
+	column_bounds(rel, desc, cmin, cmax, unknown);
+	for (int g = 0; g < desc->ngroup_cols; g++)
+	{
+		const int c = desc->group_cols[g];
+		if (unknown[c]) return cg_set_error(CG_EUNSUPPORTED, "group column %d has a chunk with values but no min / max (or is a float column)", c);
+		col_min[g] = cmin[c];       /* INT64_MAX > INT64_MIN when the column has no value */
+		col_max[g] = cmax[c];
+	}
 	return CG_OK;
 }
 
@@ -876,7 +909,8 @@ static int check_error_flags(CgPartial *p, unsigned long long flags)
 	if (flags & CG_ERRFLAG_NULL_MULTIKEY)
 		return cg_set_error(CG_EUNSUPPORTED, "NULL in a two-column group key");
 	if (flags & CG_ERRFLAG_KEY_RANGE)
-		return cg_set_error(CG_EINVAL, "group key outside [key_min, key_max] given to cg_partial_create");
+		return cg_set_error(CG_EINVAL, "group key outside [key_min, key_max] or the composite key bounds given to cg_partial_create, "
+										"or a NULL key flag merged into a composite partial");
 	if (flags & CG_ERRFLAG_SUM_BOUND)
 		return cg_set_error(CG_EINVAL, "sum argument exceeds term_abs_bound");
 	if (flags & CG_ERRFLAG_DECOMPRESS)
@@ -1597,7 +1631,9 @@ static int pending_errors(CgContext *ctx, CgPartial *p)
 static int export_rows(CgContext *ctx, CgPartial *p, uint64_t capacity, int64_t *d_keys, uint8_t *d_nulls, uint64_t *d_words, int64_t *nrows)
 {
 	unsigned long long st[5], counts[2] = {0, 0};
-	const bool direct = p->d_packed && p->packed_dirty && !p->wide_dirty && p->mode == CG_MODE_DENSE && p->desc.ngroup_cols == 1;
+	/* the packed export's key of entry e is key_min + e: one-column keys and composite codes */
+	const bool direct = p->d_packed && p->packed_dirty && !p->wide_dirty && p->mode == CG_MODE_DENSE &&
+						(p->desc.ngroup_cols == 1 || p->desc.composite_key);
 	int rc;
 	if (direct)
 	{

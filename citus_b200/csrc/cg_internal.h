@@ -247,10 +247,17 @@ struct KPlan
 	int32_t nfexpr[CG_MAX_AGGS];
 	int8_t fexpr[CG_MAX_AGGS][CG_MAX_QEXPR];
 	/* bool_and / bool_or: per aggregate its predicate argument, a postfix tree over the same atoms (0 tokens = none).
-	 * These two fields stay last: the generated kernels of plans without predicate arguments restate the struct up to
-	 * fexpr only (cg_jit.cpp) */
+	 * These two fields and the composite key's stay behind fexpr: the generated kernels of plans with neither restate the
+	 * struct up to fexpr only (cg_jit.cpp) */
 	int32_t nargexpr[CG_MAX_AGGS];
 	int8_t argexpr[CG_MAX_AGGS][CG_MAX_QEXPR];
+	/* composite key (CgScanDesc.composite_key): the key is the mixed-radix code over gcol[0..ngroup) (cg_plan.cpp), then
+	 * a one-column key with key_min 0 and no NULL group.  Column g's digit is 0 for NULL, v - kmin[g] + 1 otherwise, and
+	 * a value with v - kmin[g] >= kradix[g] - 1 is out of range.  Last, so that the generated kernels of other plans
+	 * restate the struct without them (cg_jit.cpp) */
+	int32_t composite;
+	int64_t kmin[CG_MAX_GROUP_COLS];
+	uint64_t kradix[CG_MAX_GROUP_COLS];
 };
 
 static inline bool cg_desc_has_filters(const CgScanDesc *d)
@@ -481,6 +488,11 @@ int cg_partition_route_scatter_async(const int64_t *d_keys, const uint8_t *d_nul
 void cg_comm_set_peer_window(int on);
 
 /* cg_plan.cpp */
+/* the composite key codec (the only place that knows the code): radix[g] of every key column and the domain D; CG_EINVAL
+ * for a descriptor that is not composite or has a bad column count, CG_EUNSUPPORTED when D > 2^63 */
+int cg_key_codec(const CgScanDesc *desc, uint64_t *radix, unsigned __int128 *domain);
+/* identity of the key codec, folded into what ranks agree on before they combine (0 for the other key forms) */
+uint64_t cg_key_codec_id(const CgScanDesc *desc);
 int cg_partial_shape(CgPartial *p, const CgScanDesc *desc, const CgColumnDesc *columns, int32_t natts,
 					 int64_t key_min, int64_t key_max, int64_t max_rows);
 bool cg_build_fast_plan(const CgScanDesc *desc, const KPlan &plan, bool all8, FPlan *fast);

@@ -313,9 +313,18 @@ static bool plan_has_args(const KPlan &plan)
  * KAgg's barg byte as padding: its kernel reads nothing behind them (the arguments' trees are written out as code), so
  * the plan parameter it declares is a prefix of the one the host passes, and its source is the one such plans had
  * before the arguments existed -- the same kernel cache key, the same compiled code. */
+/* gcol is restated with the two entries it had before composite keys: the generated code names its key columns v<c> and
+ * never reads gcol, and naggs follows at the same offset either way (the padding after gcol absorbs the difference), so
+ * the source of every existing plan shape stays as it was */
+#define KPLAN_GCOL_RESTATED 2
+static_assert(offsetof(KPlan, naggs) == offsetof(KPlan, gcol) + 4 && (offsetof(KPlan, gcol) + KPLAN_GCOL_RESTATED + 3) / 4 * 4 == offsetof(KPlan, naggs),
+			  "a two-entry gcol must give KPlan's layout");
+
 static void gen_prelude(std::string &s, const KPlan &plan)
 {
 	const bool args = plan_has_args(plan);
+	/* plans with a composite key restate the whole struct; the others stop at fexpr or argexpr as before */
+	const bool tail = args || plan.composite;
 	s +=
 		"typedef unsigned long long uint64_t; typedef long long int64_t; typedef unsigned int uint32_t; typedef int int32_t;\n"
 		"typedef unsigned short uint16_t; typedef short int16_t; typedef unsigned char uint8_t; typedef signed char int8_t;\n"
@@ -335,15 +344,18 @@ static void gen_prelude(std::string &s, const KPlan &plan)
 		 "  int32_t nfquals; uint8_t fcol[%d]; uint8_t fop[%d]; int64_t fk[%d]; int64_t flo[%d]; int64_t fhi[%d]; uint8_t fneg[%d];\n"
 		 "  int32_t nfexpr[%d]; int8_t fexpr[%d][%d];%s",
 		 CG_KMAX_COLS, CG_KMAX_COLS, CG_KMAX_COLS, CG_MAX_QUALS, CG_MAX_QUALS, CG_MAX_QUALS, CG_MAX_QUALS, CG_MAX_QUALS, CG_MAX_QUALS,
-		 CG_MAX_GROUP_COLS, CG_MAX_AGGS, CG_KMAX_WORDS, CG_KMAX_WORDS, CG_MAX_QEXPR, CG_MAX_FILTER_QUALS, CG_MAX_FILTER_QUALS,
+		 KPLAN_GCOL_RESTATED, CG_MAX_AGGS, CG_KMAX_WORDS, CG_KMAX_WORDS, CG_MAX_QEXPR, CG_MAX_FILTER_QUALS, CG_MAX_FILTER_QUALS,
 		 CG_MAX_FILTER_QUALS, CG_MAX_FILTER_QUALS, CG_MAX_FILTER_QUALS, CG_MAX_FILTER_QUALS, CG_MAX_AGGS, CG_MAX_AGGS, CG_MAX_QEXPR,
-		 args ? "\n" : " };\n");
-	if (args) addf(s, "  int32_t nargexpr[%d]; int8_t argexpr[%d][%d]; };\n", CG_MAX_AGGS, CG_MAX_AGGS, CG_MAX_QEXPR);
-	/* the text above must describe the host's structs exactly (without arguments: the prefix up to fexpr) */
+		 tail ? "\n" : " };\n");
+	if (tail) addf(s, "  int32_t nargexpr[%d]; int8_t argexpr[%d][%d];%s", CG_MAX_AGGS, CG_MAX_AGGS, CG_MAX_QEXPR, plan.composite ? "\n" : " };\n");
+	if (plan.composite) addf(s, "  int32_t composite; int64_t kmin[%d]; uint64_t kradix[%d]; };\n", CG_MAX_GROUP_COLS, CG_MAX_GROUP_COLS);
+	/* the text above must describe the host's structs exactly (without arguments: the prefix up to fexpr; with arguments
+	 * only: the prefix up to argexpr) */
 	const size_t prefix = (offsetof(KPlan, nargexpr) + alignof(KPlan) - 1) / alignof(KPlan) * alignof(KPlan);
+	const size_t prefix_args = (offsetof(KPlan, composite) + alignof(KPlan) - 1) / alignof(KPlan) * alignof(KPlan);
 	addf(s, "static_assert(sizeof(DevChunkCol) == %zu, \"DevChunkCol\");\n", sizeof(DevChunkCol));
 	addf(s, "static_assert(sizeof(KAgg) == %zu, \"KAgg\");\n", sizeof(KAgg));
-	addf(s, "static_assert(sizeof(KPlan) == %zu, \"KPlan\");\n", args ? sizeof(KPlan) : prefix);
+	addf(s, "static_assert(sizeof(KPlan) == %zu, \"KPlan\");\n", plan.composite ? sizeof(KPlan) : args ? prefix_args : prefix);
 	/* (NVRTC has no offsetof; same field order + same total size is the check) */
 	s +=
 		"#define EMPTY_KEY ((int64_t) 0x8000000000000000ull)\n"
@@ -634,7 +646,32 @@ static void gen_row(std::string &s, const KPlan &plan, const JitShape &sh, int u
 	const char *B = "\t\t\t\t\t\t\t";
 	/* group slot; a NULL key is its own group (the entry behind the addressable ones) */
 	std::string zkey;
-	if (plan.mode != CG_MODE_GLOBAL)
+	if (plan.composite)
+	{
+		/* the composite code (cg_plan.cpp): a NULL is digit 0, so there is no NULL group; kok = every value within its
+		 * column's bounds */
+		std::string code, ok;
+		for (int g = 0; g < plan.ngroup; g++)
+		{
+			const int c = plan.gcol[g];
+			addf(s, "%sconst uint64_t kd%d = (uint64_t) v%d - (uint64_t) P.kmin[%d];\n", B, g, c, g);
+			char digit[64], in[96];
+			if (col_nullable(sh, c))
+			{
+				snprintf(digit, sizeof digit, "(z%d ? 0ull : kd%d + 1ull)", c, g);
+				snprintf(in, sizeof in, "(z%d || kd%d < P.kradix[%d] - 1ull)", c, g, g);
+			}
+			else
+			{
+				snprintf(digit, sizeof digit, "(kd%d + 1ull)", g);
+				snprintf(in, sizeof in, "kd%d < P.kradix[%d] - 1ull", g, g);
+			}
+			code = g ? "(" + code + ") * P.kradix[" + std::to_string(g) + "] + " + digit : std::string(digit);
+			ok += (g ? " && " : "") + std::string(in);
+		}
+		addf(s, "%sconst bool kok = %s;\n%sconst uint64_t kcode = %s;\n", B, ok.c_str(), B, code.c_str());
+	}
+	else if (plan.mode != CG_MODE_GLOBAL)
 	{
 		if (plan.ngroup == 1) { if (col_nullable(sh, plan.gcol[0])) zkey = "z" + std::to_string(plan.gcol[0]); }
 		else
@@ -643,7 +680,20 @@ static void gen_row(std::string &s, const KPlan &plan, const JitShape &sh, int u
 			if (col_nullable(sh, plan.gcol[1])) zkey += (zkey.empty() ? "z" : " || z") + std::to_string(plan.gcol[1]);
 		}
 	}
-	if (plan.mode == CG_MODE_DENSE)
+	if (plan.mode == CG_MODE_DENSE && plan.composite)
+		addf(s, "%suint64_t slot = kcode;\n%sbool ok = kok;\n%sif (!ok) raise_flag(P.stats, %lluull);\n", B, B, B,
+			 (unsigned long long) CG_ERRFLAG_KEY_RANGE);
+	else if (plan.mode == CG_MODE_HASH && plan.composite)
+		/* a code is never EMPTY_KEY (it is >= 0) */
+		addf(s,
+			 "%sconst int64_t key = (int64_t) kcode;\n%suint64_t slot;\n"
+			 "%sif (!kok) { raise_flag(P.stats, %lluull); slot = ~0ull; }\n"
+			 "%selse { uint64_t h = ((uint64_t) key * 0x9E3779B97F4A7C15ull) >> P.hash_shift;\n"
+			 "%s  long long cur = (long long) __ldcg((unsigned long long *) (P.hkeys + h));\n"
+			 "%s  slot = (cur == key) ? h : hash_slot_slow(P, key, h); }\n"
+			 "%sbool ok = slot != ~0ull;\n",
+			 B, B, B, (unsigned long long) CG_ERRFLAG_KEY_RANGE, B, B, B, B);
+	else if (plan.mode == CG_MODE_DENSE)
 	{
 		if (plan.ngroup == 1)
 		{

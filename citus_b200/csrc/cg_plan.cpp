@@ -60,7 +60,9 @@ static int validate_desc(const CgScanDesc *d, const CgColumnDesc *columns, int n
 {
 	if (d->nquals < 0 || d->nquals > CG_MAX_QUALS) return cg_set_error(CG_EINVAL, "nquals %d out of range", d->nquals);
 	if (d->naggs < 0 || d->naggs > CG_MAX_AGGS) return cg_set_error(CG_EINVAL, "naggs %d out of range", d->naggs);
-	if (d->ngroup_cols < 0 || d->ngroup_cols > CG_MAX_GROUP_COLS)
+	if (d->composite_key != 0 && d->composite_key != 1) return cg_set_error(CG_EINVAL, "composite_key %d", d->composite_key);
+	/* the packed key form holds at most two columns */
+	if (d->ngroup_cols < (d->composite_key ? 1 : 0) || d->ngroup_cols > (d->composite_key ? CG_MAX_GROUP_COLS : 2))
 		return cg_set_error(CG_EINVAL, "ngroup_cols %d out of range", d->ngroup_cols);
 	for (int c = 0; c < natts; c++)
 	{
@@ -106,7 +108,7 @@ static int validate_desc(const CgScanDesc *d, const CgColumnDesc *columns, int n
 		if (c < 0 || c >= natts) return cg_set_error(CG_EINVAL, "group column %d out of range", c);
 		if (columns[c].type_class == CG_TYPE_FLOAT)
 			return cg_set_error(CG_EUNSUPPORTED, "GROUP BY on a float column");
-		if (d->ngroup_cols == 2 && cg_decoded_len(columns[c]) > 4)
+		if (!d->composite_key && d->ngroup_cols == 2 && cg_decoded_len(columns[c]) > 4)
 			return cg_set_error(CG_EUNSUPPORTED, "two-column GROUP BY needs columns of at most 4 bytes");
 	}
 	for (int a = 0; a < d->naggs; a++)
@@ -141,6 +143,95 @@ static int validate_desc(const CgScanDesc *d, const CgColumnDesc *columns, int n
 			bool colf = columns[s.column[f]].type_class == CG_TYPE_FLOAT;
 			if (s.kind != CG_AGG_COUNT && colf != (s.is_float != 0))
 				return cg_set_error(CG_EINVAL, "aggregate %d: integer/float mismatch with column %d", a, s.column[f]);
+		}
+	}
+	return CG_OK;
+}
+
+/*
+ * The composite group key codec (CgScanDesc.composite_key; include/citus_gpu.h states the code).  This block is the only
+ * code that knows it: the kernels receive kmin / kradix per column and compute the digits the same way, everything behind
+ * them sees a one-column key over [0, D).  A column of bounds [lo, hi] has hi - lo + 1 values plus NULL (digit 0); an
+ * all-NULL column (lo > hi) has NULL only.  D is computed in 128 bits: K radixes of up to 2^64 + 1 each.
+ */
+int cg_key_codec(const CgScanDesc *d, uint64_t *radix, unsigned __int128 *domain)
+{
+	if (!d->composite_key) return cg_set_error(CG_EINVAL, "the descriptor has no composite key");
+	const int K = d->ngroup_cols;
+	if (K < 1 || K > CG_MAX_GROUP_COLS) return cg_set_error(CG_EINVAL, "composite key over %d columns", K);
+	const unsigned __int128 limit = (unsigned __int128) 1 << 63;
+	unsigned __int128 D = 1;
+	for (int g = 0; g < K; g++)
+	{
+		const int64_t lo = d->key_col_min[g], hi = d->key_col_max[g];
+		const unsigned __int128 r = lo > hi ? 1 : (unsigned __int128) ((__int128) hi - (__int128) lo) + 2;
+		D *= r;                       /* D <= 2^63 before, r <= 2^64 + 1: no 128-bit overflow */
+		if (D > limit) return cg_set_error(CG_EUNSUPPORTED, "composite key domain exceeds 2^63 (column %d: [%lld, %lld])", g, (long long) lo, (long long) hi);
+		radix[g] = (uint64_t) r;
+	}
+	*domain = D;
+	return CG_OK;
+}
+
+uint64_t cg_key_codec_id(const CgScanDesc *d)
+{
+	if (!d->composite_key) return 0;
+	/* FNV-1a over the column count and the bounds */
+	uint64_t h = 0xcbf29ce484222325ull;
+	auto mix = [&](uint64_t x) { for (int i = 0; i < 8; i++) { h ^= (x >> (8 * i)) & 0xff; h *= 0x100000001b3ull; } };
+	mix((uint64_t) d->ngroup_cols);
+	for (int g = 0; g < d->ngroup_cols && g < CG_MAX_GROUP_COLS; g++) { mix((uint64_t) d->key_col_min[g]); mix((uint64_t) d->key_col_max[g]); }
+	return h | 1;                     /* never 0, the value of the other key forms */
+}
+
+extern "C" int cg_group_key_encode(const CgScanDesc *desc, int64_t n, const int64_t *values, const uint8_t *nulls, int64_t *codes)
+{
+	if (!desc || n < 0 || (n > 0 && (!values || !codes))) return cg_set_error(CG_EINVAL, "NULL argument");
+	uint64_t radix[CG_MAX_GROUP_COLS];
+	unsigned __int128 D;
+	int rc = cg_key_codec(desc, radix, &D);
+	if (rc) return rc;
+	const int K = desc->ngroup_cols;
+	for (int64_t i = 0; i < n; i++)
+	{
+		uint64_t code = 0;
+		for (int g = 0; g < K; g++)
+		{
+			uint64_t digit = 0;
+			if (!(nulls && nulls[i * K + g]))
+			{
+				const int64_t v = values[i * K + g];
+				if (v < desc->key_col_min[g] || v > desc->key_col_max[g])
+					return cg_set_error(CG_EINVAL, "row %lld: key column %d value %lld outside [%lld, %lld]", (long long) i, g, (long long) v,
+										(long long) desc->key_col_min[g], (long long) desc->key_col_max[g]);
+				digit = (uint64_t) v - (uint64_t) desc->key_col_min[g] + 1;
+			}
+			code = code * radix[g] + digit;     /* < D <= 2^63 */
+		}
+		codes[i] = (int64_t) code;
+	}
+	return CG_OK;
+}
+
+extern "C" int cg_group_key_decode(const CgScanDesc *desc, int64_t n, const int64_t *codes, int64_t *values, uint8_t *nulls)
+{
+	if (!desc || n < 0 || (n > 0 && (!codes || !values || !nulls))) return cg_set_error(CG_EINVAL, "NULL argument");
+	uint64_t radix[CG_MAX_GROUP_COLS];
+	unsigned __int128 D;
+	int rc = cg_key_codec(desc, radix, &D);
+	if (rc) return rc;
+	const int K = desc->ngroup_cols;
+	for (int64_t i = 0; i < n; i++)
+	{
+		if (codes[i] < 0 || (unsigned __int128) codes[i] >= D)
+			return cg_set_error(CG_EINVAL, "row %lld: code %lld outside the key domain", (long long) i, (long long) codes[i]);
+		uint64_t c = (uint64_t) codes[i];
+		for (int g = K - 1; g >= 0; g--)
+		{
+			const uint64_t digit = c % radix[g];
+			c /= radix[g];
+			nulls[i * K + g] = digit == 0;
+			values[i * K + g] = digit == 0 ? 0 : (int64_t) ((uint64_t) desc->key_col_min[g] + digit - 1);
 		}
 	}
 	return CG_OK;
@@ -240,6 +331,15 @@ int cg_partial_shape(CgPartial *p, const CgScanDesc *desc, const CgColumnDesc *c
 {
 	int rc = validate_desc(desc, columns, natts);
 	if (rc) return rc;
+	if (desc->composite_key)
+	{
+		/* a one-column key over the codes [0, D): key_min / key_max are not used */
+		uint64_t radix[CG_MAX_GROUP_COLS];
+		unsigned __int128 D;
+		if ((rc = cg_key_codec(desc, radix, &D))) return rc;
+		key_min = 0;
+		key_max = (int64_t) (D - 1);
+	}
 	p->desc = *desc;
 	p->columns.assign(columns, columns + natts);
 	p->key_min = key_min;
@@ -254,7 +354,7 @@ int cg_partial_shape(CgPartial *p, const CgScanDesc *desc, const CgColumnDesc *c
 		p->mode = CG_MODE_GLOBAL;
 		p->capacity = 1; p->entries = 1; p->stride = p->nwords;
 	}
-	else if (desc->ngroup_cols == 2 &&
+	else if (desc->ngroup_cols == 2 && !desc->composite_key &&
 			 (int32_t) (uint32_t) key_min <= (int32_t) (uint32_t) key_max &&
 			 (int32_t) ((uint64_t) key_min >> 32) <= (int32_t) ((uint64_t) key_max >> 32) &&
 			 ((uint64_t) ((int64_t) (int32_t) (uint32_t) key_max - (int32_t) (uint32_t) key_min) + 1) *
@@ -273,7 +373,7 @@ int cg_partial_shape(CgPartial *p, const CgScanDesc *desc, const CgColumnDesc *c
 		int s = 1; while (s < p->nwords) s <<= 1;
 		p->stride = s;
 	}
-	else if (desc->ngroup_cols == 1 && key_min <= key_max && ((uint64_t) key_max - (uint64_t) key_min) < kDenseLimit)
+	else if ((desc->ngroup_cols == 1 || desc->composite_key) && key_min <= key_max && ((uint64_t) key_max - (uint64_t) key_min) < kDenseLimit)
 	{
 		p->mode = CG_MODE_DENSE;
 		p->capacity = ((uint64_t) key_max - (uint64_t) key_min) + 1;
@@ -403,6 +503,14 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 			partial->desc.narg_expr[a] != desc->narg_expr[a] ||
 			memcmp(partial->desc.arg_expr[a], desc->arg_expr[a], (size_t) desc->narg_expr[a]) != 0)
 			return cg_set_error(CG_EINVAL, "partial aggregate was created for a different aggregate list");
+	/* a composite partial's codes mean something only under its own key columns and bounds */
+	if (partial->desc.composite_key != desc->composite_key)
+		return cg_set_error(CG_EINVAL, "partial aggregate was created for a different group key form");
+	if (desc->composite_key)
+		for (int g = 0; g < desc->ngroup_cols; g++)
+			if (partial->desc.group_cols[g] != desc->group_cols[g] || partial->desc.key_col_min[g] != desc->key_col_min[g] ||
+				partial->desc.key_col_max[g] != desc->key_col_max[g])
+				return cg_set_error(CG_EINVAL, "partial aggregate was created for other composite key columns or bounds (column %d)", g);
 
 	memset(plan, 0, sizeof *plan);
 	int pcol_of_att[256];
@@ -461,6 +569,13 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 	{
 		int pc; USE_OR_FAIL(pc, desc->group_cols[g]);
 		plan->gcol[g] = (uint8_t) pc;
+	}
+	if (desc->composite_key)
+	{
+		unsigned __int128 D;
+		if ((rc = cg_key_codec(desc, plan->kradix, &D))) return rc;
+		plan->composite = 1;
+		for (int g = 0; g < desc->ngroup_cols; g++) plan->kmin[g] = desc->key_col_min[g];
 	}
 	plan->naggs = desc->naggs;
 	for (int a = 0; a < desc->naggs; a++)
@@ -521,14 +636,14 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 /*
  * Specialised-kernel eligibility: 8-byte integer columns only; the WHERE list reduces to at
  * most two column ranges (btree conjuncts on one column intersect; a lone <> is a negated
- * point range); at most one group column; aggregates are count(*) and up to three
+ * point range); at most one group column, not a composite key; aggregates are count(*) and up to three
  * sum(column); every column plays exactly one role.  Anything else runs on the general
  * kernel.  NULLs are handled outside: the fast kernel only sees chunk groups whose plan
  * columns have none.
  */
 bool cg_build_fast_plan(const CgScanDesc *desc, const KPlan &plan, bool all8, FPlan *fast)
 {
-	if (!all8 || plan.ngroup > 1 || plan.nqexpr != 0 || plan.nfquals != 0) return false;
+	if (!all8 || plan.ngroup > 1 || plan.composite || plan.nqexpr != 0 || plan.nfquals != 0) return false;
 	for (int c = 0; c < plan.ncols; c++) if (plan.isfloat[c]) return false;
 	memset(fast, 0, sizeof *fast);
 	bool used[CG_KMAX_COLS] = {false};

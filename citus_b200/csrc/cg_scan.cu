@@ -555,7 +555,8 @@ static TableView view_of(const CgPartial *p)
 	TableView v;
 	v.hkeys = p->d_hkeys; v.table = p->d_table; v.capacity = p->capacity; v.entries = p->entries; v.stride = p->stride;
 	v.nwords = p->nwords; v.mode = p->mode; v.key_min = p->key_min;
-	v.key_min1 = p->key_min1; v.range1 = p->range1; v.ngroup = p->desc.ngroup_cols;
+	/* a composite partial is a one-column table over the codes: the key of direct-indexed entry e is e */
+	v.key_min1 = p->key_min1; v.range1 = p->range1; v.ngroup = p->desc.composite_key ? 1 : p->desc.ngroup_cols;
 	for (int i = 0; i < CG_KMAX_WORDS; i++) v.wordop[i] = p->wordop[i];
 	return v;
 }
@@ -744,6 +745,12 @@ __global__ void cg_merge_kernel(const __grid_constant__ KPlan P, const int64_t *
 		else
 		{
 			bool kn = nulls ? nulls[i] != 0 : false;
+			if (kn && P.composite)
+			{
+				/* a composite code encodes its NULLs: a NULL key flag is a malformed row, never a group */
+				atomicOr(P.stats + 2, CG_ERRFLAG_KEY_RANGE);
+				continue;
+			}
 			entry = (P.mode == CG_MODE_DENSE) ? find_entry<CG_MODE_DENSE>(P, keys[i], kn)
 											  : find_entry<CG_MODE_HASH>(P, keys[i], kn);
 			if (entry == nullptr) continue;
@@ -767,7 +774,7 @@ int cg_launch_merge(CgPartial *p, const int64_t *d_keys, const uint8_t *d_nulls,
 	memset(&plan, 0, sizeof plan);
 	plan.mode = p->mode; plan.nwords = p->nwords; plan.stride = p->stride; plan.table = p->d_table; plan.hkeys = p->d_hkeys;
 	plan.capacity = p->capacity; plan.key_min = p->key_min; plan.stats = p->d_stats;
-	plan.key_min1 = p->key_min1; plan.range1 = p->range1; plan.ngroup = p->desc.ngroup_cols;
+	plan.key_min1 = p->key_min1; plan.range1 = p->range1; plan.ngroup = p->desc.ngroup_cols; plan.composite = p->desc.composite_key;
 	plan.hash_shift = 64;
 	for (uint64_t c = p->capacity; c > 1; c >>= 1) plan.hash_shift--;
 	for (int i = 0; i < CG_KMAX_WORDS; i++) plan.wordop[i] = p->wordop[i];

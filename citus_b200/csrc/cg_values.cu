@@ -34,6 +34,8 @@ extern "C" int cg_partial_merge_values(CgPartial *p, int64_t nrows, const int64_
 	{
 		hk[i] = keys ? keys[i] : 0;
 		hn[i] = key_nulls ? key_nulls[i] : 0;
+		if (hn[i] && p->desc.composite_key)
+			return cg_set_error(CG_EINVAL, "partial row %lld: NULL key flag on a composite partial (its codes encode NULLs)", (long long) i);
 		uint64_t *w = &hw[(size_t) i * nw];
 		for (int x = 0; x < nw; x++) w[x] = word_identity(p->wordop[x]);
 		/* rows in the group: count(*) when the query has one, else the largest non-NULL input count (at least 1, so

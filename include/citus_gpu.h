@@ -207,7 +207,7 @@ typedef struct CgAggSpec
 
 #define CG_MAX_QUALS 8
 #define CG_MAX_AGGS 8
-#define CG_MAX_GROUP_COLS 2
+#define CG_MAX_GROUP_COLS 4
 /* WHERE as a boolean tree over the atoms quals[0..nquals): postfix tokens, >= 0 = atom index,
  * CG_QX_AND / CG_QX_OR combine the two entries on top of the stack (PostgreSQL's BoolExpr; NOT is
  * folded into the operators).  nqual_expr = 0 means the plain AND of all atoms. */
@@ -260,6 +260,26 @@ typedef struct CgScanDesc
 	 * the argument atoms, as they ignore the filter atoms. */
 	int32_t narg_expr[CG_MAX_AGGS];
 	int8_t arg_expr[CG_MAX_AGGS][CG_MAX_QEXPR];
+	/* Composite GROUP BY key.  composite_key = 0: the key forms above -- one column, or two columns of at most 4 bytes
+	 * packed into one int64 (low 32 bits: the first), where a NULL in either column fails the scan with CG_EUNSUPPORTED;
+	 * ngroup_cols > 2 is CG_EINVAL.  composite_key = 1: ngroup_cols = K in 1..CG_MAX_GROUP_COLS columns of any integer-like
+	 * type (int1 / int2 / int4 / int8, bool, char(1), numeric(p, s); float is CG_EUNSUPPORTED), NULLs included, with every
+	 * row's key value of column c in [key_col_min[c], key_col_max[c]] (cg_relation_key_bounds; key_col_min > key_col_max
+	 * = the column is NULL in every row).  The key is one exact int64 code, a mixed-radix number:
+	 *     d_c = 0 if column c is NULL, else v_c - key_col_min[c] + 1;   R_c = key_col_max[c] - key_col_min[c] + 2 (1 if all NULL)
+	 *     code = ((d_0 * R_1 + d_1) * R_2 + d_2) * R_3 + d_3,   in [0, D), D = R_0 * ... * R_{K-1}
+	 * Codes sort the way the key tuples sort, NULL lowest in each column.  cg_partial_create refuses D > 2^63 with
+	 * CG_EUNSUPPORTED and ignores its key_min / key_max; the partial is then a one-column partial over the code, with no
+	 * NULL group: direct-indexed when D <= 2^26, else a hash table.  A row whose key value lies outside its column's
+	 * bounds joins no group and fails the scan with CG_EINVAL, in every table kind.  cg_partial_fetch,
+	 * cg_partial_export_device, cg_partial_merge_rows and cg_partial_merge_values carry codes in their key arrays;
+	 * key_nulls is always 0 on export, and a row merged with a non-zero key_nulls entry is refused with CG_EINVAL
+	 * (merge_values: at once; merge_rows: by the calls that read the partial).  cg_group_key_decode / cg_group_key_encode
+	 * convert.  A scan's descriptor must have the
+	 * partial's key columns and bounds (CG_EINVAL otherwise); a zero-filled tail is composite_key = 0. */
+	int32_t composite_key;
+	int64_t key_col_min[CG_MAX_GROUP_COLS];
+	int64_t key_col_max[CG_MAX_GROUP_COLS];
 } CgScanDesc;
 
 /* EXPLAIN ANALYZE counters (columnar_customscan.c:1966-1999 and ExecScan instrumentation) */
@@ -511,6 +531,16 @@ int cg_join_rows(const int64_t *d_build_keys, const uint8_t *d_build_nulls, cons
  * e.g. a chunk without min/max).  Feed them to cg_partial_create / CgAggSpec.term_abs_bound. */
 int cg_relation_bounds(const CgRelation *rel, const CgScanDesc *desc, int64_t *key_min, int64_t *key_max,
 					   int64_t *term_abs_bound /* [naggs] */, int64_t *rows);
+/* The same per group column, for a composite key (CgScanDesc.composite_key): col_min[g] / col_max[g] = bounds of column
+ * group_cols[g] over the chunk groups that survive skipping; a column without any non-NULL value there gets
+ * col_min > col_max.  A surviving chunk that has values but no min / max (or a float column) is CG_EUNSUPPORTED. */
+int cg_relation_key_bounds(const CgRelation *rel, const CgScanDesc *desc, int64_t *col_min /* [ngroup_cols] */,
+						   int64_t *col_max /* [ngroup_cols] */);
+/* Composite key codes <-> key tuples under desc's codec (composite_key = 1, ngroup_cols = K, key_col_min / key_col_max):
+ * values[i * K + c] / nulls[i * K + c] are column c of row i (a NULL's value is 0).  Pure host functions.  A code outside
+ * [0, D) or a value outside its column's bounds is CG_EINVAL; D > 2^63 is CG_EUNSUPPORTED. */
+int cg_group_key_decode(const CgScanDesc *desc, int64_t n, const int64_t *codes, int64_t *values, uint8_t *nulls);
+int cg_group_key_encode(const CgScanDesc *desc, int64_t n, const int64_t *values, const uint8_t *nulls, int64_t *codes);
 
 /* ---------------------------------------------------------------------------------- *
  *  Host-side helpers that belong to the path.

@@ -18,7 +18,9 @@
  *   errors           the library returns codes, never longjmps; every non-zero code becomes ereport(ERROR) here
  *
  * A query shape the library does not cover (CG_EUNSUPPORTED at plan time) simply gets no GpuColumnarAgg path: the
- * reference's own Agg <- ColumnarScan plan runs.  Built against the real headers with `make -C pg_glue`; type-checked in
+ * reference's own Agg <- ColumnarScan plan runs.  A composite GROUP BY key (three or four columns, a column wider than 4
+ * bytes, or a nullable column in a two-column key) can also be refused at execution time, because its code domain
+ * depends on the data: such a node keeps the reference plan as its child and runs it instead, before any scan.  Built against the real headers with `make -C pg_glue`; type-checked in
  * this repository against pg_glue/stub/ (tests/test_pg_glue.py).
  */
 #include "postgres.h"
@@ -26,6 +28,7 @@
 #include "access/table.h"
 #include "catalog/pg_type.h"
 #include "commands/explain.h"
+#include "executor/executor.h"
 #include "executor/tuptable.h"
 #include "fmgr.h"
 #include "nodes/extensible.h"
@@ -84,7 +87,13 @@ typedef struct GpuColumnarAggState
 	int64 *count;
 	int64 *minmax;
 	double *fsum;
+	/* composite key: the decoded key columns of every group, [group][column] */
+	int64 *key_values;
+	uint8 *key_value_nulls;
 	bool done_scan;
+	/* composite key: the reference Agg <- ColumnarScan plan, run when the library refuses the key domain */
+	PlanState *child;
+	bool use_child;
 } GpuColumnarAggState;
 
 static create_upper_paths_hook_type prev_create_upper_paths_hook = NULL;
@@ -375,7 +384,10 @@ translate_query(PlannerInfo *root, RelOptInfo *input_rel, GpuAggPlan *plan)
 			plan->desc.qual_expr[plan->desc.nqual_expr++] = CG_QX_AND;
 		}
 	}
-	/* GROUP BY plain integer columns */
+	/* GROUP BY plain integer columns.  One column, and two NOT NULL columns of at most 4 bytes, keep the one-column and
+	 * packed two-column key forms; anything wider, or a two-column key with a nullable column (whose NULL the packed form
+	 * refuses at run time), takes the composite key, whose bounds run_scan reads from the skip lists */
+	bool composite = false;
 	foreach(lc, q->groupClause)
 	{
 		if (!ok) break;
@@ -383,12 +395,16 @@ translate_query(PlannerInfo *root, RelOptInfo *input_rel, GpuAggPlan *plan)
 		TargetEntry *tle = get_sortgroupref_tle(sgc->tleSortGroupRef, q->targetList);
 		Var *var = strip_to_var((Node *) tle->expr);
 		int attlen, type_class;
-		if (var == NULL || plan->desc.ngroup_cols >= CG_MAX_GROUP_COLS || !type_is_supported(var->vartype, &attlen, &type_class) ||
-			type_class != CG_TYPE_INT)
+		if (var == NULL || var->varattno <= 0 || var->varattno > tupdesc->natts || plan->desc.ngroup_cols >= CG_MAX_GROUP_COLS ||
+			!type_is_supported(var->vartype, &attlen, &type_class) || type_class != CG_TYPE_INT)
 			ok = false;
 		else
+		{
+			composite |= attlen > 4 || !TupleDescAttr(tupdesc, var->varattno - 1)->attnotnull;
 			plan->desc.group_cols[plan->desc.ngroup_cols++] = var->varattno - 1;
+		}
 	}
+	plan->desc.composite_key = plan->desc.ngroup_cols > 2 || (plan->desc.ngroup_cols == 2 && composite);
 	/* target list: group columns and aggregates, in output order */
 	foreach(lc, q->targetList)
 	{
@@ -463,6 +479,24 @@ GpuColumnarAggUpperPaths(PlannerInfo *root, UpperRelationKind stage, RelOptInfo 
 	cpath->path.startup_cost = 0;
 	cpath->path.total_cost = input_rel->rows * 1e-6;
 	cpath->methods = &GpuColumnarAggPathMethods;
+	if (plan->desc.composite_key)
+	{
+		/* the composite key's domain is known only at execution time, where cg_partial_create may refuse it: the cheapest
+		 * reference path becomes the node's child.  It is taken out of the pathlist because add_path frees the paths the
+		 * GPU path displaces. */
+		Path *ref = NULL;
+		ListCell *lc;
+		foreach(lc, output_rel->pathlist)
+		{
+			Path *p = (Path *) lfirst(lc);
+			if (ref == NULL || p->total_cost < ref->total_cost)
+				ref = p;
+		}
+		if (ref == NULL)
+			return;
+		output_rel->pathlist = list_delete_ptr(output_rel->pathlist, ref);
+		cpath->custom_paths = list_make1(ref);
+	}
 	bytea *blob = palloc(VARHDRSZ + sizeof(GpuAggPlan));
 	SET_VARSIZE(blob, VARHDRSZ + sizeof(GpuAggPlan));
 	memcpy(VARDATA(blob), plan, sizeof(GpuAggPlan));
@@ -478,8 +512,9 @@ GpuColumnarAgg_PlanCustomPath(PlannerInfo *root, RelOptInfo *rel, CustomPath *be
 	cscan->scan.scanrelid = 0;                       /* not a scan of one base relation's tuples: it emits aggregate rows */
 	cscan->custom_scan_tlist = tlist;
 	cscan->custom_private = best_path->custom_private;
+	cscan->custom_plans = custom_plans;                /* composite key: the reference plan (GpuColumnarAggUpperPaths) */
 	cscan->methods = &GpuColumnarAggScanMethods;
-	(void) root; (void) rel; (void) clauses; (void) custom_plans;
+	(void) root; (void) rel; (void) clauses;
 	return (Plan *) cscan;
 }
 
@@ -593,7 +628,15 @@ build_relation_image(Relation rel, Snapshot snapshot, CgRelation *out)
 static void
 GpuColumnarAgg_Begin(CustomScanState *node, EState *estate, int eflags)
 {
-	(void) node; (void) estate; (void) eflags;      /* everything happens at the first Exec call: EXPLAIN without ANALYZE must not touch the GPU */
+	/* everything on the GPU happens at the first Exec call: EXPLAIN without ANALYZE must not touch it.  The reference
+	 * child of a composite-key node is initialised here like any subplan (EXPLAIN shows it under the node). */
+	GpuColumnarAggState *state = (GpuColumnarAggState *) node;
+	CustomScan *cscan = (CustomScan *) node->ss.ps.plan;
+	if (cscan->custom_plans != NIL)
+	{
+		state->child = ExecInitNode((Plan *) linitial(cscan->custom_plans), estate, eflags);
+		node->custom_ps = list_make1(state->child);
+	}
 }
 
 static void
@@ -611,8 +654,31 @@ run_scan(GpuColumnarAggState *state)
 	gpu_check(cg_relation_bounds(&image, desc, &key_min, &key_max, bounds, &rows));
 	for (int a = 0; a < desc->naggs; a++)
 		desc->aggs[a].term_abs_bound = bounds[a];
-	gpu_check(cg_partial_create(desc, image.columns, image.natts, key_min, key_max, Max(rows, 1), &state->partial));
-	int rc = cg_scan_relation(&image, desc, state->partial, &state->stats);
+	int rc = CG_OK;
+	if (desc->composite_key)
+	{
+		/* per-column bounds over the chunk groups the scan keeps; a domain the library refuses (D > 2^63, or a column
+		 * without min / max) runs the reference child instead, before anything is scanned */
+		int64 lo[CG_MAX_GROUP_COLS], hi[CG_MAX_GROUP_COLS];
+		rc = cg_relation_key_bounds(&image, desc, lo, hi);
+		for (int g = 0; rc == CG_OK && g < desc->ngroup_cols; g++)
+		{
+			desc->key_col_min[g] = lo[g];
+			desc->key_col_max[g] = hi[g];
+		}
+	}
+	if (rc == CG_OK)
+		rc = cg_partial_create(desc, image.columns, image.natts, key_min, key_max, Max(rows, 1), &state->partial);
+	if (rc == CG_EUNSUPPORTED && state->child != NULL)
+	{
+		table_close(rel, AccessShareLock);
+		state->use_child = true;
+		state->done_scan = true;
+		MemoryContextSwitchTo(old);
+		return;
+	}
+	gpu_check(rc);
+	rc = cg_scan_relation(&image, desc, state->partial, &state->stats);
 	if (rc == CG_ERETRY_UNPACKED)
 	{
 		/* an optimistic packed accumulator overflowed: nothing wrong was produced; rescan with wide accumulators */
@@ -630,6 +696,14 @@ run_scan(GpuColumnarAggState *state)
 	state->fsum = palloc(sizeof(double) * cells);
 	gpu_check(cg_partial_fetch(state->partial, Max(n, 1), state->keys, state->key_nulls, state->sum_hi, state->sum_lo, state->count,
 							   state->minmax, state->fsum, &state->ngroups));
+	if (desc->composite_key)
+	{
+		/* the key arrays hold composite codes: the key columns come from the library's decoder */
+		Size kcells = (Size) Max(state->ngroups, 1) * desc->ngroup_cols;
+		state->key_values = palloc(sizeof(int64) * kcells);
+		state->key_value_nulls = palloc(kcells);
+		gpu_check(cg_group_key_decode(desc, state->ngroups, state->keys, state->key_values, state->key_value_nulls));
+	}
 	table_close(rel, AccessShareLock);
 	state->next = 0;
 	state->done_scan = true;
@@ -655,6 +729,8 @@ GpuColumnarAgg_Exec(CustomScanState *node)
 	GpuColumnarAggState *state = (GpuColumnarAggState *) node;
 	if (!state->done_scan)
 		run_scan(state);
+	if (state->use_child)
+		return ExecProcNode(state->child);             /* the reference plan's rows have the node's target list */
 	TupleTableSlot *slot = node->ss.ps.ps_ResultTupleSlot;
 	ExecClearTuple(slot);
 	if (state->next >= state->ngroups)
@@ -670,6 +746,13 @@ GpuColumnarAgg_Exec(CustomScanState *node)
 		{
 			case GPU_OUT_KEY:
 			{
+				if (state->plan.desc.composite_key)
+				{
+					const Size kc = (Size) g * state->plan.desc.ngroup_cols + out->index;
+					slot->tts_isnull[i] = state->key_value_nulls[kc] != 0;
+					slot->tts_values[i] = i64_to_datum(state->key_values[kc], out->type);
+					break;
+				}
 				/* two group columns travel packed: low 32 bits the first, high 32 bits the second */
 				int64 k = state->keys[g];
 				if (state->plan.desc.ngroup_cols == 2)
@@ -713,12 +796,17 @@ GpuColumnarAgg_End(CustomScanState *node)
 	if (state->partial)
 		cg_partial_free(state->partial);
 	state->partial = NULL;
+	if (state->child)
+		ExecEndNode(state->child);
+	state->child = NULL;
 }
 
 static void
 GpuColumnarAgg_ReScan(CustomScanState *node)
 {
 	GpuColumnarAggState *state = (GpuColumnarAggState *) node;
+	if (state->use_child)
+		ExecReScan(state->child);
 	state->next = 0;                                   /* the aggregate rows are still there */
 }
 
@@ -730,6 +818,11 @@ GpuColumnarAgg_Explain(CustomScanState *node, List *ancestors, ExplainState *es)
 	(void) ancestors;
 	if (!state->done_scan)
 		return;
+	if (state->use_child)
+	{
+		ExplainPropertyText("GPU Path", "refused the composite key domain: the reference plan ran", es);
+		return;
+	}
 	ExplainPropertyInteger("Rows Removed by Filter", NULL, state->stats.rows_removed_by_filter, es);
 	ExplainPropertyInteger("Columnar Chunk Groups Removed by Filter", NULL, state->stats.chunk_groups_filtered, es);
 	ExplainPropertyInteger("GPU Bytes Scanned", "B", state->stats.bytes_scanned, es);

@@ -119,6 +119,7 @@ List *list_make1_impl(void *datum);
 #define list_make1(x) list_make1_impl(x)
 #define list_make2(a, b) lappend(list_make1_impl(a), b)
 void *list_nth(const List *list, int n);
+List *list_delete_ptr(List *list, void *datum);
 #define linitial(l) list_nth(l, 0)
 #define lsecond(l) list_nth(l, 1)
 #define foreach(cell, lst) for (int cell##__i = 0; (cell) = NULL, cell##__i < list_length(lst) && ((cell) = (ListCell *) &(lst)->elements[cell##__i], true); cell##__i++)
@@ -321,6 +322,11 @@ void add_path(RelOptInfo *parent_rel, Path *new_path);
 typedef struct EState { NodeTag type; Snapshot es_snapshot; MemoryContext es_query_cxt; } EState;
 typedef struct ExprContext ExprContext;
 typedef struct PlanState { NodeTag type; Plan *plan; EState *state; TupleTableSlot *ps_ResultTupleSlot; ExprContext *ps_ExprContext; } PlanState;
+/* executor/executor.h (ExecProcNode is a static inline there: the same call) */
+PlanState *ExecInitNode(Plan *node, EState *estate, int eflags);
+TupleTableSlot *ExecProcNode(PlanState *node);
+void ExecEndNode(PlanState *node);
+void ExecReScan(PlanState *node);
 typedef struct ScanState { PlanState ps; Relation ss_currentRelation; TupleTableSlot *ss_ScanTupleSlot; } ScanState;
 struct CustomExecMethods;
 typedef struct CustomScanState { ScanState ss; uint32 flags; List *custom_ps; Size pscan_len; const struct CustomExecMethods *methods; } CustomScanState;
