@@ -18,7 +18,7 @@ CG_OK, CG_EINVAL, CG_ECUDA, CG_ENOMEM, CG_ECORRUPT, CG_ETABLEFULL, CG_EUNSUPPORT
 CG_COMM_ID_BYTES = 128
 CG_COMM_SUM, CG_COMM_MIN, CG_COMM_MAX = 0, 1, 2
 CG_TYPE_INT, CG_TYPE_FLOAT = 0, 1
-CG_OP = {"<": 0, "<=": 1, "=": 2, ">=": 3, ">": 4, "<>": 5}
+CG_OP = {"<": 0, "<=": 1, "=": 2, ">=": 3, ">": 4, "<>": 5, "in": 6, "not in": 7, "is null": 8, "is not null": 9}
 CG_AGG_COUNT_STAR, CG_AGG_COUNT, CG_AGG_SUM, CG_AGG_MIN, CG_AGG_MAX = range(5)
 CG_AGG_BIT_AND, CG_AGG_BIT_OR, CG_AGG_BOOL_AND, CG_AGG_BOOL_OR = range(5, 9)
 CG_WORD_ADD, CG_WORD_MIN, CG_WORD_MAX, CG_WORD_FADD, CG_WORD_FMIN, CG_WORD_FMAX = range(6)
@@ -27,6 +27,7 @@ CG_GEN_UNIFORM, CG_GEN_SEQUENCE = 0, 1
 CG_MAX_QUALS, CG_MAX_AGGS, CG_MAX_GROUP_COLS = 8, 8, 4
 CG_MAX_QEXPR, CG_QX_AND, CG_QX_OR = 16, -1, -2
 CG_MAX_FILTER_QUALS = 8
+CG_MAX_IN_LISTS, CG_MAX_IN_VALUES, CG_IN_REFUTE_MAX = 8, 1024, 100
 
 
 class CgSkipNode(C.Structure):
@@ -65,6 +66,10 @@ class CgQual(C.Structure):
     _fields_ = [("column", C.c_int32), ("op", C.c_int32), ("konst", C.c_int64)]
 
 
+class CgInList(C.Structure):
+    _fields_ = [("first", C.c_int32), ("nvalues", C.c_int32), ("nnulls", C.c_int32), ("reserved", C.c_int32)]
+
+
 class CgAggSpec(C.Structure):
     _fields_ = [("kind", C.c_int32), ("nfactors", C.c_int32), ("column", C.c_int32 * 3),
                 ("is_float", C.c_int32), ("a", C.c_int64 * 3), ("b", C.c_int64 * 3),
@@ -81,7 +86,9 @@ class CgScanDesc(C.Structure):
                 ("nfilter_expr", C.c_int32 * CG_MAX_AGGS), ("filter_expr", (C.c_int8 * CG_MAX_QEXPR) * CG_MAX_AGGS),
                 ("narg_expr", C.c_int32 * CG_MAX_AGGS), ("arg_expr", (C.c_int8 * CG_MAX_QEXPR) * CG_MAX_AGGS),
                 ("composite_key", C.c_int32), ("key_col_min", C.c_int64 * CG_MAX_GROUP_COLS),
-                ("key_col_max", C.c_int64 * CG_MAX_GROUP_COLS)]
+                ("key_col_max", C.c_int64 * CG_MAX_GROUP_COLS),
+                ("nin_lists", C.c_int32), ("in_lists", CgInList * CG_MAX_IN_LISTS),
+                ("nin_values", C.c_int32), ("in_values", C.c_int64 * CG_MAX_IN_VALUES)]
 
 
 class CgScanStats(C.Structure):

@@ -240,8 +240,9 @@ def bool_or(tree, filter=None):
 
 
 def flatten_where(where):
-    """WHERE as a nested tuple tree -- ("and" | "or", arm, arm, ...) over atoms (column, op, constant); a plain
-    list of atoms is their AND -- to (atoms, postfix tokens).  The tokens are empty for a plain AND-list."""
+    """WHERE as a nested tuple tree -- ("and" | "or", arm, arm, ...) over atoms (column, op, constant), (column, "in" |
+    "not in", (value, ...)) and (column, "is null" | "is not null"); a plain list of atoms is their AND -- to (atoms, postfix
+    tokens).  The tokens are empty for a plain AND-list."""
     if not (isinstance(where, tuple) and where and where[0] in ("and", "or")):
         return list(where), []
     atoms, tokens = [], []
@@ -280,11 +281,45 @@ def _filter_tokens(tree, pool):
     return [index[t] if t >= 0 else t for t in tokens]
 
 
-def _set_atom(q, atom, float_cols):
-    col, op, k = atom
+def _konst(k, col, float_cols):
+    return int(np.float64(k).view(np.int64)) if col in float_cols else int(k)
+
+
+def _set_atom(q, atom, float_cols, lists):
+    """one atom: (column, op, constant); (column, "in" | "not in", (v, ...)) with None for a NULL element -- the list goes
+    to `lists`, [(elements, float?)], and konst is its index; (column, "is null" | "is not null")"""
+    col, op = atom[0], atom[1]
     q.column = col
     q.op = capi.CG_OP[op]
-    q.konst = int(np.float64(k).view(np.int64)) if col in float_cols else int(k)
+    if op in ("is null", "is not null"):
+        if len(atom) != 2:
+            raise ValueError(f"{op} takes no constant")
+        q.konst = 0
+    elif op in ("in", "not in"):
+        key = (tuple(atom[2]), col in float_cols)
+        if not key[0]:
+            raise capi.CitusGpuError(capi.CG_EUNSUPPORTED, "an empty IN list")
+        if key not in lists:
+            lists.append(key)
+        q.konst = lists.index(key)
+    else:
+        q.konst = _konst(atom[2], col, float_cols)
+
+
+def _set_lists(d, lists):
+    """the list table of a descriptor: every list's non-NULL elements back to back, in konst's convention (NULL elements
+    are only counted, so they take no room in in_values)"""
+    if len(lists) > capi.CG_MAX_IN_LISTS or sum(sum(v is not None for v in vals) for vals, _ in lists) > capi.CG_MAX_IN_VALUES:
+        raise capi.CitusGpuError(capi.CG_EUNSUPPORTED, "IN lists too large")
+    d.nin_lists = len(lists)
+    n = 0
+    for i, (values, is_float) in enumerate(lists):
+        vals = [v for v in values if v is not None]
+        d.in_lists[i].first, d.in_lists[i].nvalues, d.in_lists[i].nnulls = n, len(vals), len(values) - len(vals)
+        for v in vals:
+            d.in_values[n] = int(np.float64(v).view(np.int64)) if is_float else int(v)
+            n += 1
+    d.nin_values = n
 
 
 def make_desc(quals=(), group_cols=(), aggs=(), qual_pushdown=True, expected_groups=0, float_cols=(), composite=False,
@@ -305,8 +340,9 @@ def make_desc(quals=(), group_cols=(), aggs=(), qual_pushdown=True, expected_gro
     for i, t in enumerate(tokens):
         d.qual_expr[i] = t
     d.nquals = len(quals)
+    lists = []                   # IN / NOT IN lists of WHERE and the pool: (elements, float column?)
     for i, atom in enumerate(quals):
-        _set_atom(d.quals[i], atom, float_cols)
+        _set_atom(d.quals[i], atom, float_cols, lists)
     pool = []                    # FILTERs and bool_and / bool_or arguments share one atom pool
     for i, a in enumerate(aggs):
         for tree, n, expr, what in ((a.filter, d.nfilter_expr, d.filter_expr, "FILTER"),
@@ -321,7 +357,8 @@ def make_desc(quals=(), group_cols=(), aggs=(), qual_pushdown=True, expected_gro
                 expr[i][j] = t
     d.nfilter_quals = len(pool)
     for i, atom in enumerate(pool):
-        _set_atom(d.filter_quals[i], atom, float_cols)
+        _set_atom(d.filter_quals[i], atom, float_cols, lists)
+    _set_lists(d, lists)
     d.enable_qual_pushdown = 1 if qual_pushdown else 0
     d.ngroup_cols = len(group_cols)
     for i, c in enumerate(group_cols):

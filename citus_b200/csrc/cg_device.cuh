@@ -156,16 +156,35 @@ __device__ __forceinline__ bool qual_true(int64_t v, int op, int64_t k, bool isf
 	}
 }
 
+/* is `key` one of the sorted codes s[0 .. len)?  A branch-free lower bound: exactly `steps` = ceil(log2(len)) halvings, the
+ * same for every lane of the warp (the atom's list is uniform), so the search never diverges.  The codes are read through
+ * the read-only path with L1 allocation: the column streams bypass L1, so a list of up to 8 KB stays there. */
+__device__ __forceinline__ bool set_contains(const uint64_t *s, uint32_t len, uint32_t steps, uint64_t key)
+{
+	if (len == 0) return false;
+	const uint64_t *b = s;
+	uint32_t n = len;
+#pragma unroll 1
+	for (uint32_t i = 0; i < steps; i++)
+	{
+		const uint32_t h = n >> 1;
+		b = (__ldg(b + h) <= key) ? b + h : b;
+		n -= h;
+	}
+	return __ldg(b) == key;
+}
+
 /*
  * K3: the WHERE tree ([PG] ExecQual under ExecScan, columnar_customscan.c:1907-1913) under three-valued
  * logic: an atom on a NULL input is not TRUE, AND/OR combine "is TRUE" bits (there is no NOT node: it is
  * folded into the comparison operators), the row passes iff the root is TRUE.  Without a tree the atoms
- * are an AND-list.
+ * are an AND-list.  The list and NULL-test atoms have TRUE and FALSE of their own (include/citus_gpu.h, CgQual):
+ * IS [NOT] NULL is never UNKNOWN, and a list with a NULL element makes "not found" UNKNOWN.
  */
 template <int NCC>
 __device__ __forceinline__ uint32_t eval_atoms(const KPlan &P, const int64_t (&v)[NCC], uint32_t nullmask, int n, const uint8_t *col,
 											   const uint8_t *op, const int64_t *k, const int64_t *lo, const int64_t *hi, const uint8_t *neg,
-											   uint32_t *falsity = nullptr)
+											   const KSet *ks, uint32_t *falsity = nullptr)
 {
 	uint32_t truth = 0, fals = 0;
 #pragma unroll 1
@@ -174,9 +193,29 @@ __device__ __forceinline__ uint32_t eval_atoms(const KPlan &P, const int64_t (&v
 		int c = col[q];
 		bool isnull = (nullmask >> c) & 1u;
 		int64_t x = pick<NCC>(v, c);
-		bool t = P.isfloat[c] ? qual_true(x, op[q], k[q], true) : (((x >= lo[q]) && (x <= hi[q])) != (bool) neg[q]);
-		truth |= (uint32_t) (t && !isnull) << q;
-		fals |= (uint32_t) (!t && !isnull) << q;
+		bool t, f;
+		if (op[q] <= CG_OP_NE)
+		{
+			const bool r = P.isfloat[c] ? qual_true(x, op[q], k[q], true) : (((x >= lo[q]) && (x <= hi[q])) != (bool) neg[q]);
+			t = r && !isnull;
+			f = !r && !isnull;
+		}
+		else if (op[q] >= CG_OP_IS_NULL)
+		{
+			t = isnull == (op[q] == CG_OP_IS_NULL);
+			f = !t;
+		}
+		else
+		{
+			const KSet s = ks[q];
+			const bool found = set_contains(P.sets + s.off, s.len, s.steps, cg_set_code(x, P.isfloat[c]));
+			const bool in = op[q] == CG_OP_IN;
+			/* IN: found = TRUE, not found = FALSE without NULL elements; NOT IN the other way round; UNKNOWN otherwise */
+			t = !isnull && (in ? found : (!found && !s.nnull));
+			f = !isnull && (in ? (!found && !s.nnull) : found);
+		}
+		truth |= (uint32_t) t << q;
+		fals |= (uint32_t) f << q;
 	}
 	if (falsity) *falsity = fals;
 	return truth;
@@ -204,7 +243,7 @@ __device__ __forceinline__ bool eval_postfix(uint32_t truth, int n, const int8_t
 template <int NCC>
 __device__ __forceinline__ bool eval_where(const KPlan &P, const int64_t (&v)[NCC], uint32_t nullmask)
 {
-	uint32_t truth = eval_atoms<NCC>(P, v, nullmask, P.nquals, P.qcol, P.qop, P.qk, P.qlo, P.qhi, P.qneg);
+	uint32_t truth = eval_atoms<NCC>(P, v, nullmask, P.nquals, P.qcol, P.qop, P.qk, P.qlo, P.qhi, P.qneg, P.qset);
 	if (P.nqexpr == 0) return truth == (1u << P.nquals) - 1u;
 	return eval_postfix(truth, P.nqexpr, P.qexpr);
 }
@@ -218,7 +257,7 @@ __device__ __forceinline__ uint32_t eval_filters(const KPlan &P, const int64_t (
 	if (argtrue) *argtrue = 0u;
 	if (P.nfquals == 0) return 0u;
 	uint32_t fals = 0;
-	uint32_t truth = eval_atoms<NCC>(P, v, nullmask, P.nfquals, P.fcol, P.fop, P.fk, P.flo, P.fhi, P.fneg, &fals);
+	uint32_t truth = eval_atoms<NCC>(P, v, nullmask, P.nfquals, P.fcol, P.fop, P.fk, P.flo, P.fhi, P.fneg, P.fset, &fals);
 	uint32_t rejected = 0, at = 0;
 #pragma unroll 1
 	for (int a = 0; a < P.naggs; a++)

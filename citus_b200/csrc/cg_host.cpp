@@ -272,8 +272,24 @@ static int datum_cmp(int type_class, int64_t a, int64_t b)
  * on that column contradicts either half (backend/columnar/columnar_reader.c:1132-1187,
  * 1234-1260, 1358-1384).  A chunk without min/max (all NULL) is never skipped.
  */
-static bool atom_refuted(const CgSkipNode &node, int type_class, const CgQual &q)
+static bool atom_refuted(const CgSkipNode &node, int type_class, const CgQual &q, const CgScanDesc *d)
 {
+	if (q.op == CG_OP_IN)
+	{
+		/* [PG] predtest.c: "x = ANY(array)" of at most MAX_SAOP_ARRAY_SIZE elements is the OR of "x = element", refuted when
+		 * every arm is; an arm with a NULL constant is never strongly refuted; a longer array is an opaque clause */
+		if (q.konst < 0 || q.konst >= d->nin_lists) return false;
+		const CgInList &L = d->in_lists[q.konst];
+		if (L.nnulls > 0 || (int64_t) L.nvalues + L.nnulls > CG_IN_REFUTE_MAX) return false;
+		for (int i = 0; i < L.nvalues; i++)
+		{
+			const int64_t e = d->in_values[L.first + i];
+			if (datum_cmp(type_class, node.min_value, e) <= 0 && datum_cmp(type_class, node.max_value, e) >= 0) return false;
+		}
+		return true;
+	}
+	/* NOT IN is an AND of "<>" arms, none of which refutes; a NullTest is never pushed down (ExtractPushdownClause) */
+	if (q.op > CG_OP_NE) return false;
 	int64_t k = q.konst;
 	int cmin = datum_cmp(type_class, node.min_value, k);
 	int cmax = datum_cmp(type_class, node.max_value, k);
@@ -297,14 +313,14 @@ static bool chunk_refuted(const CgSkipNode &node, int type_class, int col, const
 	if (d->nqual_expr == 0)
 	{
 		for (int q = 0; q < d->nquals; q++)
-			if (d->quals[q].column == col && atom_refuted(node, type_class, d->quals[q])) return true;
+			if (d->quals[q].column == col && atom_refuted(node, type_class, d->quals[q], d)) return true;
 		return false;
 	}
 	uint32_t st = 0;
 	for (int i = 0; i < d->nqual_expr; i++)
 	{
 		int t = d->qual_expr[i];
-		if (t >= 0) st = (st << 1) | (uint32_t) (d->quals[t].column == col && atom_refuted(node, type_class, d->quals[t]));
+		if (t >= 0) st = (st << 1) | (uint32_t) (d->quals[t].column == col && atom_refuted(node, type_class, d->quals[t], d));
 		else
 		{
 			uint32_t b = st & 1u, a = (st >> 1) & 1u;
@@ -1044,6 +1060,36 @@ static int stats_end(CgContext *ctx, CgPartial *p, const unsigned long long befo
 	return CG_OK;
 }
 
+/* the plan's IN / NOT IN codes to the partial's device buffer.  Codes equal to the last ones written are already there (the
+ * common case: one query over many shards).  Otherwise the copy is enqueued on the compute stream, so it runs after every
+ * launch enqueued there before -- an earlier scan into this partial, still in flight, reads its own lists to the end -- and
+ * before this scan's launches.  Its source is a pinned slot of a ring (a pageable source may make cudaMemcpyAsync wait
+ * for the stream); a slot is reused only after its previous copy has run (its event). */
+static int upload_sets(CgContext *ctx, CgPartial *p, const std::vector<uint64_t> &codes, KPlan *plan)
+{
+	if (codes.empty()) return CG_OK;
+	const size_t cap = 2 * CG_MAX_IN_VALUES;
+	if (codes.size() > cap) return cg_set_error(CG_EINVAL, "%zu list codes", codes.size());
+	if (!p->d_sets && cudaMalloc(&p->d_sets, cap * sizeof(uint64_t)) != cudaSuccess)
+	{
+		p->d_sets = nullptr;
+		return cg_set_error(CG_ENOMEM, "cudaMalloc for the IN lists failed");
+	}
+	plan->sets = p->d_sets;
+	if (codes == p->sets_last) return CG_OK;
+	const int slot = p->sets_slot;
+	p->sets_slot = (slot + 1) % CgPartial::kSetSlots;
+	if (!p->h_sets[slot]) CG_CUDA(cudaHostAlloc((void **) &p->h_sets[slot], cap * sizeof(uint64_t), cudaHostAllocDefault));
+	if (!p->sets_copied[slot]) CG_CUDA(cudaEventCreateWithFlags(&p->sets_copied[slot], cudaEventDisableTiming));
+	CG_CUDA(cudaEventSynchronize(p->sets_copied[slot]));       /* the slot's previous copy has read it */
+	memcpy(p->h_sets[slot], codes.data(), codes.size() * sizeof(uint64_t));
+	p->sets_last.clear();                                      /* the buffer's content is unknown until the copy is enqueued */
+	CG_CUDA(cudaMemcpyAsync(p->d_sets, p->h_sets[slot], codes.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->compute));
+	CG_CUDA(cudaEventRecord(p->sets_copied[slot], ctx->compute));
+	p->sets_last = codes;
+	return CG_OK;
+}
+
 extern "C" int cg_scan_shard(const CgShard *sh, const CgScanDesc *desc, CgPartial *into, CgScanStats *stats)
 {
 	CgContext *ctx = cg_ctx();
@@ -1051,7 +1097,8 @@ extern "C" int cg_scan_shard(const CgShard *sh, const CgScanDesc *desc, CgPartia
 	if (!sh || !desc || !into) return cg_set_error(CG_EINVAL, "NULL argument");
 	KPlan plan;
 	bool all8 = false;
-	int rc = cg_build_plan(desc, sh->columns.data(), sh->natts, &sh->slot_of_att, into, &plan, &all8);
+	std::vector<uint64_t> codes;
+	int rc = cg_build_plan(desc, sh->columns.data(), sh->natts, &sh->slot_of_att, into, &plan, &all8, &codes);
 	if (rc) return rc;
 	rc = before_scan(ctx, into);
 	if (rc) return rc;
@@ -1062,7 +1109,8 @@ extern "C" int cg_scan_shard(const CgShard *sh, const CgScanDesc *desc, CgPartia
 	std::vector<uint8_t> slots(plan.slot, plan.slot + plan.ncols);
 	bool same = msh->sel_valid && msh->sel_pushdown == desc->enable_qual_pushdown && msh->sel_nquals == desc->nquals &&
 				memcmp(msh->sel_quals, desc->quals, sizeof(CgQual) * desc->nquals) == 0 && msh->sel_slots == slots &&
-				msh->sel_nqexpr == desc->nqual_expr && memcmp(msh->sel_qexpr, desc->qual_expr, (size_t) desc->nqual_expr) == 0;
+				msh->sel_nqexpr == desc->nqual_expr && memcmp(msh->sel_qexpr, desc->qual_expr, (size_t) desc->nqual_expr) == 0 &&
+				msh->sel_lists == cg_where_lists(desc);
 	if (!same)
 	{
 		std::vector<uint32_t> fastl, slowl;
@@ -1108,6 +1156,7 @@ extern "C" int cg_scan_shard(const CgShard *sh, const CgScanDesc *desc, CgPartia
 		msh->sel_nqexpr = desc->nqual_expr;
 		memcpy(msh->sel_qexpr, desc->qual_expr, (size_t) desc->nqual_expr);
 		memcpy(msh->sel_quals, desc->quals, sizeof(CgQual) * desc->nquals);
+		msh->sel_lists = cg_where_lists(desc);
 		msh->sel_slots = slots;
 		msh->sel_valid = true;
 	}
@@ -1122,6 +1171,8 @@ extern "C" int cg_scan_shard(const CgShard *sh, const CgScanDesc *desc, CgPartia
 	if (rc) return rc;
 	if (!selected.empty())
 	{
+		rc = upload_sets(ctx, into, codes, &plan);
+		if (rc) return rc;
 		plan.arena = sh->d_arena;
 		plan.chunkcols = sh->d_chunkcols;
 		plan.nstaged = (int32_t) sh->staged.size();
@@ -1344,9 +1395,12 @@ extern "C" int cg_scan_relation(const CgRelation *rel, const CgScanDesc *desc, C
 
 	KPlan plan;
 	bool all8 = false;
-	rc = cg_build_plan(desc, rel->columns, rel->natts, &slot_of_att, into, &plan, &all8);
+	std::vector<uint64_t> codes;
+	rc = cg_build_plan(desc, rel->columns, rel->natts, &slot_of_att, into, &plan, &all8, &codes);
 	if (rc) return rc;
 	rc = before_scan(ctx, into);
+	if (rc) return rc;
+	rc = upload_sets(ctx, into, codes, &plan);
 	if (rc) return rc;
 
 	std::vector<std::vector<uint8_t>> select(rel->nstripes);

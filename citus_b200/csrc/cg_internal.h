@@ -130,6 +130,7 @@ struct CgShard
 	CgQual sel_quals[CG_MAX_QUALS];
 	int32_t sel_nqexpr = 0;
 	int8_t sel_qexpr[CG_MAX_QEXPR];
+	std::vector<int64_t> sel_lists;          /* the IN lists the WHERE atoms of that list read (cg_where_lists) */
 	int64_t sel_filtered = 0;
 	uint32_t sel_nullmask = 0;               /* plan columns that have NULLs in some chunk group of the second part */
 	/* the list is ordered [chunk groups without NULLs in the plan columns | the rest] */
@@ -175,6 +176,28 @@ struct KAgg
 	int64_t bound;      /* nlimbs == 1: every |term| must be <= bound */
 	int64_t tbound;     /* integer SUM: the caller-proven bound on |term| whatever nlimbs is (0 = unknown) */
 };
+
+/* the list of one IN / NOT IN atom: codes sets[off .. off + len), len = 0 for a list of NULLs only; steps = ceil(log2(len)),
+ * the fixed length of its binary search; nnull = the list has a NULL element */
+struct KSet
+{
+	uint16_t off;
+	uint16_t len;
+	uint8_t steps;
+	uint8_t nnull;
+	uint8_t pad[2];
+};
+
+/* the code of a value in its column's comparison order, as unsigned: an integer with its sign bit flipped; a float8 (bits)
+ * through f8_ordered after -0.0 -> +0.0 (every NaN already maps to one code) */
+static inline __host__ __device__ uint64_t cg_set_code(int64_t v, bool isfloat)
+{
+	if (!isfloat) return (uint64_t) v ^ 0x8000000000000000ull;
+	uint64_t u = (uint64_t) v;
+	if (u == 0x8000000000000000ull) u = 0;
+	if ((u & 0x7fffffffffffffffull) > 0x7ff0000000000000ull) return ~0ull;
+	return (u >> 63) ? ~u : (u | 0x8000000000000000ull);
+}
 
 struct KPlan
 {
@@ -258,6 +281,12 @@ struct KPlan
 	int32_t composite;
 	int64_t kmin[CG_MAX_GROUP_COLS];
 	uint64_t kradix[CG_MAX_GROUP_COLS];
+	/* IN / NOT IN atoms (qop / fop CG_OP_IN, CG_OP_NOT_IN): sets = every list's sorted, distinct codes (cg_set_code), back to
+	 * back in device memory; an atom's list is qset / fset [q].  Behind the composite key, so that the generated kernels of
+	 * plans without lists restate the struct without them (cg_jit.cpp) */
+	const uint64_t *sets;
+	KSet qset[CG_MAX_QUALS];
+	KSet fset[CG_MAX_FILTER_QUALS];
 };
 
 static inline bool cg_desc_has_filters(const CgScanDesc *d)
@@ -376,6 +405,17 @@ struct CgPartial
 	/* pinned host buffer the result rows are fetched through */
 	uint8_t *h_out = nullptr;
 	size_t h_out_cap = 0;
+	/* the codes of the IN / NOT IN lists of the scan in flight (2 * CG_MAX_IN_VALUES words, allocated by the first scan with a
+	 * list): written with cudaMemcpyAsync on the compute stream before a launch whose codes differ from the last ones
+	 * written (sets_last), so that the copy is ordered behind every earlier launch that reads the buffer (cg_set_stream
+	 * synchronises the old stream before switching).  The copies come from a ring of pinned slots: a slot is rewritten once
+	 * the copy recorded in its event has run, so the host does not wait behind the stream's earlier kernels */
+	uint64_t *d_sets = nullptr;
+	std::vector<uint64_t> sets_last;
+	static const int kSetSlots = 4;
+	uint64_t *h_sets[kSetSlots] = {nullptr, nullptr, nullptr, nullptr};
+	cudaEvent_t sets_copied[kSetSlots] = {nullptr, nullptr, nullptr, nullptr};
+	int sets_slot = 0;
 };
 
 /* cg_scan.cu */
@@ -496,8 +536,12 @@ uint64_t cg_key_codec_id(const CgScanDesc *desc);
 int cg_partial_shape(CgPartial *p, const CgScanDesc *desc, const CgColumnDesc *columns, int32_t natts,
 					 int64_t key_min, int64_t key_max, int64_t max_rows);
 bool cg_build_fast_plan(const CgScanDesc *desc, const KPlan &plan, bool all8, FPlan *fast);
+/* set_codes (may be NULL): receives the codes plan->qset / fset index (KPlan.sets is left NULL for the caller to point at
+ * their device copy) */
 int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts,
 				  const std::vector<int32_t> *slot_of_att, CgPartial *partial, KPlan *plan,
-				  bool *all8);
+				  bool *all8, std::vector<uint64_t> *set_codes = nullptr);
+/* what of the IN lists a WHERE list reads, for comparing two WHERE lists (empty without IN / NOT IN atoms) */
+std::vector<int64_t> cg_where_lists(const CgScanDesc *desc);
 
 #endif

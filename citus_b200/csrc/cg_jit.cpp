@@ -309,6 +309,16 @@ static bool plan_has_args(const KPlan &plan)
 	return false;
 }
 
+static bool op_is_list(int op) { return op == CG_OP_IN || op == CG_OP_NOT_IN; }
+
+/* some WHERE or pool atom is IN / NOT IN: the kernel reads P.sets and the atoms' KSet entries */
+static bool plan_has_sets(const KPlan &plan)
+{
+	for (int q = 0; q < plan.nquals; q++) if (op_is_list(plan.qop[q])) return true;
+	for (int q = 0; q < plan.nfquals; q++) if (op_is_list(plan.fop[q])) return true;
+	return false;
+}
+
 /* The host's structs restated for NVRTC.  A plan without bool_and / bool_or arguments restates KPlan up to fexpr and
  * KAgg's barg byte as padding: its kernel reads nothing behind them (the arguments' trees are written out as code), so
  * the plan parameter it declares is a prefix of the one the host passes, and its source is the one such plans had
@@ -323,12 +333,16 @@ static_assert(offsetof(KPlan, naggs) == offsetof(KPlan, gcol) + 4 && (offsetof(K
 static void gen_prelude(std::string &s, const KPlan &plan)
 {
 	const bool args = plan_has_args(plan);
-	/* plans with a composite key restate the whole struct; the others stop at fexpr or argexpr as before */
-	const bool tail = args || plan.composite;
+	const bool sets = plan_has_sets(plan);
+	/* plans with IN lists restate the whole struct, plans with a composite key all but the lists; the others stop at fexpr
+	 * or argexpr as before */
+	const bool composite = plan.composite || sets;
+	const bool tail = args || composite;
 	s +=
 		"typedef unsigned long long uint64_t; typedef long long int64_t; typedef unsigned int uint32_t; typedef int int32_t;\n"
 		"typedef unsigned short uint16_t; typedef short int16_t; typedef unsigned char uint8_t; typedef signed char int8_t;\n"
 		"struct DevChunkCol { uint64_t values_off; uint64_t exists_off; uint64_t rank_off; uint32_t value_count; uint32_t row_count; };\n";
+	if (sets) s += "struct KSet { uint16_t off; uint16_t len; uint8_t steps; uint8_t nnull; uint8_t pad[2]; };\n";
 	s += args ? "struct KAgg { int8_t kind; int8_t nfactors; int8_t is_float; int8_t nlimbs; int8_t pcol[3]; int8_t word0; int8_t nullword; int8_t ovchk; int8_t filt; int8_t barg;\n"
 			  : "struct KAgg { int8_t kind; int8_t nfactors; int8_t is_float; int8_t nlimbs; int8_t pcol[3]; int8_t word0; int8_t nullword; int8_t ovchk; int8_t filt; int8_t pad;\n";
 	s += "  int64_t a[3]; int64_t b[3]; int64_t bound; int64_t tbound; };\n";
@@ -347,15 +361,17 @@ static void gen_prelude(std::string &s, const KPlan &plan)
 		 KPLAN_GCOL_RESTATED, CG_MAX_AGGS, CG_KMAX_WORDS, CG_KMAX_WORDS, CG_MAX_QEXPR, CG_MAX_FILTER_QUALS, CG_MAX_FILTER_QUALS,
 		 CG_MAX_FILTER_QUALS, CG_MAX_FILTER_QUALS, CG_MAX_FILTER_QUALS, CG_MAX_FILTER_QUALS, CG_MAX_AGGS, CG_MAX_AGGS, CG_MAX_QEXPR,
 		 tail ? "\n" : " };\n");
-	if (tail) addf(s, "  int32_t nargexpr[%d]; int8_t argexpr[%d][%d];%s", CG_MAX_AGGS, CG_MAX_AGGS, CG_MAX_QEXPR, plan.composite ? "\n" : " };\n");
-	if (plan.composite) addf(s, "  int32_t composite; int64_t kmin[%d]; uint64_t kradix[%d]; };\n", CG_MAX_GROUP_COLS, CG_MAX_GROUP_COLS);
+	if (tail) addf(s, "  int32_t nargexpr[%d]; int8_t argexpr[%d][%d];%s", CG_MAX_AGGS, CG_MAX_AGGS, CG_MAX_QEXPR, composite ? "\n" : " };\n");
+	if (composite) addf(s, "  int32_t composite; int64_t kmin[%d]; uint64_t kradix[%d];%s", CG_MAX_GROUP_COLS, CG_MAX_GROUP_COLS, sets ? "\n" : " };\n");
+	if (sets) addf(s, "  const uint64_t *sets; KSet qset[%d]; KSet fset[%d]; };\n", CG_MAX_QUALS, CG_MAX_FILTER_QUALS);
 	/* the text above must describe the host's structs exactly (without arguments: the prefix up to fexpr; with arguments
-	 * only: the prefix up to argexpr) */
-	const size_t prefix = (offsetof(KPlan, nargexpr) + alignof(KPlan) - 1) / alignof(KPlan) * alignof(KPlan);
-	const size_t prefix_args = (offsetof(KPlan, composite) + alignof(KPlan) - 1) / alignof(KPlan) * alignof(KPlan);
+	 * only: the prefix up to argexpr; with a composite key: the prefix up to the lists) */
+	const auto upto = [](size_t off) { return (off + alignof(KPlan) - 1) / alignof(KPlan) * alignof(KPlan); };
+	const size_t size = sets ? sizeof(KPlan) : composite ? upto(offsetof(KPlan, sets)) : args ? upto(offsetof(KPlan, composite))
+																					   : upto(offsetof(KPlan, nargexpr));
 	addf(s, "static_assert(sizeof(DevChunkCol) == %zu, \"DevChunkCol\");\n", sizeof(DevChunkCol));
 	addf(s, "static_assert(sizeof(KAgg) == %zu, \"KAgg\");\n", sizeof(KAgg));
-	addf(s, "static_assert(sizeof(KPlan) == %zu, \"KPlan\");\n", plan.composite ? sizeof(KPlan) : args ? prefix_args : prefix);
+	addf(s, "static_assert(sizeof(KPlan) == %zu, \"KPlan\");\n", size);
 	/* (NVRTC has no offsetof; same field order + same total size is the check) */
 	s +=
 		"#define EMPTY_KEY ((int64_t) 0x8000000000000000ull)\n"
@@ -390,6 +406,18 @@ static void gen_prelude(std::string &s, const KPlan &plan)
 		"    if (cur == EMPTY_KEY) { long long old = (long long) atomicCAS(kp, (unsigned long long) EMPTY_KEY, (unsigned long long) key); if (old == EMPTY_KEY || old == key) return h; }\n"
 		"    h = (h + 1) & mask; }\n"
 		"  raise_flag(P.stats, 1ull); return ~0ull; }\n";
+	if (sets)
+		/* cg_set_code (cg_internal.h) and the branch-free membership search of cg_device.cuh's set_contains: a fixed number of
+		 * halvings per list, L1-allocating read-only loads of the codes */
+		s +=
+			"__device__ __forceinline__ uint64_t set_code_i(int64_t v) { return (uint64_t) v ^ 0x8000000000000000ull; }\n"
+			"__device__ __forceinline__ uint64_t set_code_f(int64_t v) { uint64_t u = (uint64_t) v; if (u == 0x8000000000000000ull) u = 0;\n"
+			"  if ((u & 0x7fffffffffffffffull) > 0x7ff0000000000000ull) return ~0ull; return (u >> 63) ? ~u : (u | 0x8000000000000000ull); }\n"
+			"__device__ __forceinline__ bool in_set(const uint64_t *sets, const KSet &k, uint64_t key) {\n"
+			"  if (k.len == 0) return false;\n"
+			"  const uint64_t *b = sets + k.off; uint32_t n = k.len;\n"
+			"  for (uint32_t i = 0; i < k.steps; i++) { const uint32_t h = n >> 1; b = (__ldg(b + h) <= key) ? b + h : b; n -= h; }\n"
+			"  return __ldg(b) == key; }\n";
 }
 
 static bool col_nullable(const JitShape &sh, int c) { return (sh.nullable >> c) & 1u; }
@@ -536,12 +564,29 @@ static std::string tree_expr(int n, const int8_t *expr, const char *prefix, bool
 	return st.back();
 }
 
+/* "the row's value is in the list of atom q" (IN / NOT IN), as the variable h<prefix><q> the row block defines first */
+static std::string found_var(const char *prefix, int q) { return "h" + std::string(prefix) + std::to_string(q); }
+
 /* one atom "column <op> constant" on plan column c, its constants in P.<arr>k / <arr>lo / <arr>hi / <arr>neg [q]; an atom
- * on a NULL input is not TRUE (three-valued logic) */
-static std::string atom_expr(const KPlan &plan, const JitShape &sh, int c, int op, bool neg, const char *arr, int q)
+ * on a NULL input is not TRUE (three-valued logic).  IS [NOT] NULL reads only the NULL flag (in the plain form, where the
+ * column has no NULL, it is a constant); IN / NOT IN read found_var(prefix, q) and the list's NULL flag P.<arr>set[q].nnull */
+static std::string atom_expr(const KPlan &plan, const JitShape &sh, int c, int op, bool neg, const char *arr, int q, const char *prefix)
 {
 	char buf[256], nn[32] = "";
+	if (op == CG_OP_IS_NULL || op == CG_OP_IS_NOT_NULL)
+	{
+		if (!col_nullable(sh, c)) return op == CG_OP_IS_NULL ? "false" : "true";
+		snprintf(buf, sizeof buf, "%sz%d", op == CG_OP_IS_NULL ? "" : "!", c);
+		return buf;
+	}
 	if (col_nullable(sh, c)) snprintf(nn, sizeof nn, "!z%d && ", c);
+	if (op_is_list(op))
+	{
+		const std::string h = found_var(prefix, q);
+		if (op == CG_OP_IN) snprintf(buf, sizeof buf, "%s%s", nn, h.c_str());
+		else snprintf(buf, sizeof buf, "%s!%s && !P.%sset[%d].nnull", nn, h.c_str(), arr, q);
+		return buf;
+	}
 	if (plan.isfloat[c])
 	{
 		const char *ops[] = {"<", "<=", "==", ">=", ">", "!="};
@@ -618,12 +663,21 @@ static void gen_row(std::string &s, const KPlan &plan, const JitShape &sh, int u
 		addf(s, "%sconst int64_t v%d = %s;\n", T, c, col_value(plan, sh, c, u, j).c_str());
 		if (col_nullable(sh, c)) addf(s, "%sconst bool z%d = !((e%d_%d >> %d) & 1u);\n", T, c, c, u, j);
 	}
+	/* list membership of the IN / NOT IN atoms (the lists stay kernel parameters: P.sets, P.qset / P.fset) */
+	auto gen_found = [&](int n, const uint8_t *col, const uint8_t *op, const char *arr, const char *prefix) {
+		for (int q = 0; q < n; q++)
+			if (op_is_list(op[q]))
+				addf(s, "%sconst bool %s = in_set(P.sets, P.%sset[%d], set_code_%c(v%d));\n", T, found_var(prefix, q).c_str(), arr, q,
+					 plan.isfloat[col[q]] ? 'f' : 'i', col[q]);
+	};
 	/* K3: the WHERE tree; an atom on a NULL input is not TRUE (three-valued logic) */
+	gen_found(plan.nquals, plan.qcol, plan.qop, "q", "t");
 	for (int q = 0; q < plan.nquals; q++)
-		addf(s, "%sconst bool t%d = %s;\n", T, q, atom_expr(plan, sh, plan.qcol[q], plan.qop[q], plan.qneg[q], "q", q).c_str());
+		addf(s, "%sconst bool t%d = %s;\n", T, q, atom_expr(plan, sh, plan.qcol[q], plan.qop[q], plan.qneg[q], "q", q, "t").c_str());
 	/* aggregate FILTERs: atoms u<q> of their own pool, f<a> = aggregate a's tree is TRUE */
+	gen_found(plan.nfquals, plan.fcol, plan.fop, "f", "u");
 	for (int q = 0; q < plan.nfquals; q++)
-		addf(s, "%sconst bool u%d = %s;\n", T, q, atom_expr(plan, sh, plan.fcol[q], plan.fop[q], plan.fneg[q], "f", q).c_str());
+		addf(s, "%sconst bool u%d = %s;\n", T, q, atom_expr(plan, sh, plan.fcol[q], plan.fop[q], plan.fneg[q], "f", q, "u").c_str());
 	for (int a = 0; a < plan.naggs; a++)
 		if (plan.nfexpr[a] > 0) addf(s, "%sconst bool f%d = %s;\n", T, a, tree_expr(plan.nfexpr[a], plan.fexpr[a], "u").c_str());
 	/* bool_and / bool_or arguments, three-valued on two rails: uf<q> = atom q is FALSE (not NULL, not TRUE); at<a> = the
@@ -633,7 +687,12 @@ static void gen_row(std::string &s, const KPlan &plan, const JitShape &sh, int u
 		for (int q = 0; q < plan.nfquals; q++)
 		{
 			const int c = plan.fcol[q];
-			if (col_nullable(sh, c)) addf(s, "%sconst bool uf%d = !z%d && !u%d;\n", T, q, c, q);
+			const int op = plan.fop[q];
+			std::string nn = col_nullable(sh, c) ? "!z" + std::to_string(c) + " && " : std::string();
+			if (op == CG_OP_IS_NULL || op == CG_OP_IS_NOT_NULL) addf(s, "%sconst bool uf%d = !u%d;\n", T, q, q);     /* never UNKNOWN */
+			else if (op == CG_OP_IN) addf(s, "%sconst bool uf%d = %s!%s && !P.fset[%d].nnull;\n", T, q, nn.c_str(), found_var("u", q).c_str(), q);
+			else if (op == CG_OP_NOT_IN) addf(s, "%sconst bool uf%d = %s%s;\n", T, q, nn.c_str(), found_var("u", q).c_str());
+			else if (col_nullable(sh, c)) addf(s, "%sconst bool uf%d = !z%d && !u%d;\n", T, q, c, q);
 			else addf(s, "%sconst bool uf%d = !u%d;\n", T, q, q);
 		}
 		for (int a = 0; a < plan.naggs; a++)

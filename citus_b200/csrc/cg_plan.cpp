@@ -44,16 +44,51 @@ static int validate_postfix(const char *what, const int8_t *expr, int n, int nat
 	return CG_OK;
 }
 
-static int validate_atoms(const char *what, const CgQual *quals, int n, int natts)
+static int validate_atoms(const char *what, const CgQual *quals, int n, int natts, int nin_lists)
 {
 	for (int q = 0; q < n; q++)
 	{
 		if (quals[q].column < 0 || quals[q].column >= natts)
 			return cg_set_error(CG_EINVAL, "%s %d: column %d out of range", what, q, quals[q].column);
-		if (quals[q].op < CG_OP_LT || quals[q].op > CG_OP_NE)
+		if (quals[q].op < CG_OP_LT || quals[q].op > CG_OP_IS_NOT_NULL)
 			return cg_set_error(CG_EINVAL, "%s %d: bad operator", what, q);
+		if ((quals[q].op == CG_OP_IN || quals[q].op == CG_OP_NOT_IN) && (quals[q].konst < 0 || quals[q].konst >= nin_lists))
+			return cg_set_error(CG_EINVAL, "%s %d: list %lld of %d", what, q, (long long) quals[q].konst, nin_lists);
+		if ((quals[q].op == CG_OP_IS_NULL || quals[q].op == CG_OP_IS_NOT_NULL) && quals[q].konst != 0)
+			return cg_set_error(CG_EINVAL, "%s %d: IS [NOT] NULL with a constant", what, q);
 	}
 	return CG_OK;
+}
+
+/* the IN / NOT IN list table (CgScanDesc.in_lists / in_values) */
+static int validate_lists(const CgScanDesc *d)
+{
+	if (d->nin_lists < 0 || d->nin_lists > CG_MAX_IN_LISTS) return cg_set_error(CG_EINVAL, "nin_lists %d out of range", d->nin_lists);
+	if (d->nin_values < 0 || d->nin_values > CG_MAX_IN_VALUES) return cg_set_error(CG_EINVAL, "nin_values %d out of range", d->nin_values);
+	for (int l = 0; l < d->nin_lists; l++)
+	{
+		const CgInList &L = d->in_lists[l];
+		if (L.first < 0 || L.nvalues < 0 || L.nnulls < 0) return cg_set_error(CG_EINVAL, "list %d: negative field", l);
+		if ((int64_t) L.nvalues + L.nnulls == 0) return cg_set_error(CG_EINVAL, "list %d is empty", l);
+		if ((int64_t) L.first + L.nvalues > d->nin_values)
+			return cg_set_error(CG_EINVAL, "list %d: values [%d, %lld) beyond nin_values %d", l, L.first, (long long) L.first + L.nvalues, d->nin_values);
+	}
+	return CG_OK;
+}
+
+static inline bool op_is_list(int op) { return op == CG_OP_IN || op == CG_OP_NOT_IN; }
+
+std::vector<int64_t> cg_where_lists(const CgScanDesc *d)
+{
+	std::vector<int64_t> out;
+	for (int q = 0; q < d->nquals && q < CG_MAX_QUALS; q++)
+	{
+		if (!op_is_list(d->quals[q].op) || d->quals[q].konst < 0 || d->quals[q].konst >= d->nin_lists || d->nin_lists > CG_MAX_IN_LISTS) continue;
+		const CgInList &L = d->in_lists[d->quals[q].konst];
+		out.push_back(q); out.push_back(L.nvalues); out.push_back(L.nnulls);
+		for (int i = 0; i < L.nvalues && L.first + i < CG_MAX_IN_VALUES; i++) out.push_back(d->in_values[L.first + i]);
+	}
+	return out;
 }
 
 static int validate_desc(const CgScanDesc *d, const CgColumnDesc *columns, int natts)
@@ -82,13 +117,14 @@ static int validate_desc(const CgScanDesc *d, const CgColumnDesc *columns, int n
 		if (columns[c].type_class == CG_TYPE_FLOAT && l != 4 && l != 8)
 			return cg_set_error(CG_EINVAL, "column %d: float with attlen %d", c, l);
 	}
-	int rc = validate_atoms("qual", d->quals, d->nquals, natts);
+	int rc = validate_lists(d);
 	if (rc) return rc;
+	if ((rc = validate_atoms("qual", d->quals, d->nquals, natts, d->nin_lists))) return rc;
 	if (d->nqual_expr < 0 || d->nqual_expr > CG_MAX_QEXPR) return cg_set_error(CG_EINVAL, "nqual_expr %d out of range", d->nqual_expr);
 	if (d->nqual_expr > 0 && (rc = validate_postfix("qual_expr", d->qual_expr, d->nqual_expr, d->nquals))) return rc;
 	if (d->nfilter_quals < 0 || d->nfilter_quals > CG_MAX_FILTER_QUALS)
 		return cg_set_error(CG_EINVAL, "nfilter_quals %d out of range", d->nfilter_quals);
-	if ((rc = validate_atoms("filter qual", d->filter_quals, d->nfilter_quals, natts))) return rc;
+	if ((rc = validate_atoms("filter qual", d->filter_quals, d->nfilter_quals, natts, d->nin_lists))) return rc;
 	for (int a = 0; a < CG_MAX_AGGS; a++)
 	{
 		const int n = d->nfilter_expr[a];
@@ -455,7 +491,12 @@ extern "C" void cg_partial_free(CgPartial *p)
 {
 	if (!p) return;
 	cudaFree(p->d_table); cudaFree(p->d_stats); cudaFree(p->d_out_keys); cudaFree(p->d_out_words); cudaFree(p->d_packed);
-	cudaFree(p->d_out_nulls); cudaFree(p->d_out_count);
+	cudaFree(p->d_out_nulls); cudaFree(p->d_out_count); cudaFree(p->d_sets);
+	for (int i = 0; i < CgPartial::kSetSlots; i++)
+	{
+		if (p->sets_copied[i]) { cudaEventSynchronize(p->sets_copied[i]); cudaEventDestroy(p->sets_copied[i]); }
+		if (p->h_sets[i]) cudaFreeHost(p->h_sets[i]);
+	}
 	if (p->h_out) cudaFreeHost(p->h_out);
 	if (p->h_ret) cudaFreeHost(p->h_ret);
 	delete p;
@@ -491,7 +532,8 @@ extern "C" int cg_partial_layout(const CgPartial *p, int32_t *nwords, int32_t *w
  * only the columns the quals, group keys and aggregate arguments reference are read).
  */
 int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts,
-				  const std::vector<int32_t> *slot_of_att, CgPartial *partial, KPlan *plan, bool *all8)
+				  const std::vector<int32_t> *slot_of_att, CgPartial *partial, KPlan *plan, bool *all8,
+				  std::vector<uint64_t> *set_codes)
 {
 	int rc = validate_desc(desc, columns, natts);
 	if (rc) return rc;
@@ -552,6 +594,33 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 		}
 		*lo_out = lo; *hi_out = hi; *neg_out = neg;
 	};
+	/* IN / NOT IN lists: each atom's list as sorted, distinct codes in its column's order (cg_set_code); the atoms of one
+	 * list on columns of one kind (integer / float) share them.  A list of NULLs only has no code (len 0): no row is found
+	 * in it, and nnull decides. */
+	std::vector<uint64_t> codes;
+	int list_at[CG_MAX_IN_LISTS][2];
+	for (int l = 0; l < CG_MAX_IN_LISTS; l++) list_at[l][0] = list_at[l][1] = -1;
+	auto set_of = [&](const CgQual &q, bool isfloat, KSet *ks) {
+		memset(ks, 0, sizeof *ks);
+		if (!op_is_list(q.op)) return;
+		const CgInList &L = desc->in_lists[q.konst];
+		int &at = list_at[q.konst][isfloat];
+		std::vector<uint64_t> c;
+		for (int i = 0; i < L.nvalues; i++) c.push_back(cg_set_code(desc->in_values[L.first + i], isfloat));
+		std::sort(c.begin(), c.end());
+		c.erase(std::unique(c.begin(), c.end()), c.end());
+		if (at < 0)
+		{
+			at = (int) codes.size();
+			codes.insert(codes.end(), c.begin(), c.end());
+		}
+		ks->off = (uint16_t) at;
+		ks->len = (uint16_t) c.size();
+		int steps = 0;
+		while ((1u << steps) < c.size()) steps++;
+		ks->steps = (uint8_t) steps;
+		ks->nnull = (uint8_t) (L.nnulls > 0);
+	};
 	plan->nquals = desc->nquals;
 	for (int q = 0; q < desc->nquals; q++)
 	{
@@ -560,6 +629,7 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 		plan->qop[q] = (uint8_t) desc->quals[q].op;
 		plan->qk[q] = desc->quals[q].konst;
 		atom_range(desc->quals[q], &plan->qlo[q], &plan->qhi[q], &plan->qneg[q]);
+		set_of(desc->quals[q], plan->isfloat[pc], &plan->qset[q]);
 	}
 	plan->slices = 1; plan->slice_rows = 1u << 30; plan->max_cg_rows = 0;
 	plan->nqexpr = desc->nqual_expr;
@@ -599,6 +669,7 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 			plan->fop[q] = (uint8_t) desc->filter_quals[q].op;
 			plan->fk[q] = desc->filter_quals[q].konst;
 			atom_range(desc->filter_quals[q], &plan->flo[q], &plan->fhi[q], &plan->fneg[q]);
+			set_of(desc->filter_quals[q], plan->isfloat[pc], &plan->fset[q]);
 		}
 		for (int a = 0; a < desc->naggs; a++)
 		{
@@ -608,6 +679,8 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 			for (int i = 0; i < desc->narg_expr[a]; i++) plan->argexpr[a][i] = desc->arg_expr[a][i];
 		}
 	}
+	plan->sets = nullptr;
+	if (set_codes) set_codes->swap(codes);
 	plan->ncols = ncols;
 	bool a8 = true;
 	for (int c = 0; c < ncols; c++) if (plan->len[c] != 8) a8 = false;
@@ -644,6 +717,7 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 bool cg_build_fast_plan(const CgScanDesc *desc, const KPlan &plan, bool all8, FPlan *fast)
 {
 	if (!all8 || plan.ngroup > 1 || plan.composite || plan.nqexpr != 0 || plan.nfquals != 0) return false;
+	for (int q = 0; q < plan.nquals; q++) if (plan.qop[q] > CG_OP_NE) return false;     /* IN lists and NULL tests */
 	for (int c = 0; c < plan.ncols; c++) if (plan.isfloat[c]) return false;
 	memset(fast, 0, sizeof *fast);
 	bool used[CG_KMAX_COLS] = {false};

@@ -170,15 +170,45 @@ typedef struct CgRelation
  *  backend/columnar/columnar_customscan.c:1907-1913 + the worker half of the aggregate
  *  split planner/multi_logical_optimizer.c:3160-3484.
  * ---------------------------------------------------------------------------------- */
-enum { CG_OP_LT = 0, CG_OP_LE = 1, CG_OP_EQ = 2, CG_OP_GE = 3, CG_OP_GT = 4, CG_OP_NE = 5 };
+enum { CG_OP_LT = 0, CG_OP_LE = 1, CG_OP_EQ = 2, CG_OP_GE = 3, CG_OP_GT = 4, CG_OP_NE = 5,
+	   CG_OP_IN = 6, CG_OP_NOT_IN = 7, CG_OP_IS_NULL = 8, CG_OP_IS_NOT_NULL = 9 };
 
-/* one conjunct "column <op> constant" of the WHERE list (btree operators) */
+/* one atom of a predicate tree: "column <op> constant" (btree operators), a list membership test or a NULL test.
+ * CG_OP_IN / CG_OP_NOT_IN ([PG] ScalarArrayOpExpr "x = ANY(array)" / "x <> ALL(array)", which is how IN and NOT IN lists
+ * are planned): konst is the index of a list in CgScanDesc.in_lists.  CG_OP_IS_NULL / CG_OP_IS_NOT_NULL ([PG] NullTest):
+ * konst must be 0.  Any atom may use them, in the WHERE quals and in the filter_quals pool alike.  With x the row's value,
+ * S the list's non-NULL elements and nnulls its NULL elements (three-valued, as ExecEvalScalarArrayOp / ExecEvalNullTest):
+ *                       x is NULL   x in S   x not in S, nnulls > 0   x not in S, nnulls = 0
+ *     x IN (...)        UNKNOWN     TRUE     UNKNOWN                  FALSE
+ *     x NOT IN (...)    UNKNOWN     FALSE    UNKNOWN                  TRUE
+ *     x IS NULL         TRUE        FALSE    FALSE                    FALSE
+ *     x IS NOT NULL     FALSE       TRUE     TRUE                     TRUE
+ * so an IS test is never UNKNOWN.  Membership is equality in the column's btree order: a float column compares as float8
+ * (every NaN equals every NaN, -0.0 equals +0.0); an integer-like column compares the decoded value, as konst does
+ * (int1 / 2 / 4 / 8, date, timestamp, bool 0 / 1, char(1) as an unsigned byte, numeric(p, s) as value * 10^s).
+ * Chunk-group skipping follows the reference ([PG] predicate_refuted_by with weak = false over the pushed-down clauses):
+ * an IS test is never pushed down and refutes nothing; NOT IN refutes nothing (as <> does); IN refutes a chunk's
+ * [min, max] iff its list has at most 100 elements (nvalues + nnulls, duplicates included), no NULL element, and every
+ * element lies outside [min, max]. */
 typedef struct CgQual
 {
 	int32_t column;   /* 0-based attribute index */
 	int32_t op;       /* CG_OP_* */
-	int64_t konst;    /* integer, or float8 bits for float columns */
+	int64_t konst;    /* integer, or float8 bits for float columns; IN / NOT IN: list index; IS [NOT] NULL: 0 */
 } CgQual;
+
+#define CG_MAX_IN_LISTS 8
+#define CG_MAX_IN_VALUES 1024          /* the elements of all lists of a query together */
+#define CG_IN_REFUTE_MAX 100           /* [PG] MAX_SAOP_ARRAY_SIZE: a longer list refutes no chunk group */
+/* one IN / NOT IN list: the array's elements as written (any order, duplicates allowed); the library sorts, removes
+ * duplicates and canonicalises them.  A list has at least one element (nvalues + nnulls > 0). */
+typedef struct CgInList
+{
+	int32_t first;     /* its non-NULL elements are in_values[first .. first + nvalues) */
+	int32_t nvalues;
+	int32_t nnulls;    /* its NULL elements */
+	int32_t reserved;
+} CgInList;
 
 enum { CG_AGG_COUNT_STAR = 0, CG_AGG_COUNT = 1, CG_AGG_SUM = 2, CG_AGG_MIN = 3, CG_AGG_MAX = 4,
 	   CG_AGG_BIT_AND = 5, CG_AGG_BIT_OR = 6, CG_AGG_BOOL_AND = 7, CG_AGG_BOOL_OR = 8 };
@@ -280,6 +310,14 @@ typedef struct CgScanDesc
 	int32_t composite_key;
 	int64_t key_col_min[CG_MAX_GROUP_COLS];
 	int64_t key_col_max[CG_MAX_GROUP_COLS];
+	/* The lists of the CG_OP_IN / CG_OP_NOT_IN atoms (see CgQual), shared by the WHERE quals and the filter_quals pool:
+	 * in_lists[0 .. nin_lists), their non-NULL elements in in_values[0 .. nin_values) in konst's convention (decoded integer,
+	 * or float8 bits).  They are held in the descriptor, not behind a pointer, so that a copy of it is a whole query.  A
+	 * zero-filled tail is a query without lists. */
+	int32_t nin_lists;
+	CgInList in_lists[CG_MAX_IN_LISTS];
+	int32_t nin_values;
+	int64_t in_values[CG_MAX_IN_VALUES];
 } CgScanDesc;
 
 /* EXPLAIN ANALYZE counters (columnar_customscan.c:1966-1999 and ExecScan instrumentation) */

@@ -36,6 +36,7 @@
 #include "optimizer/pathnode.h"
 #include "optimizer/planner.h"
 #include "storage/bufmgr.h"
+#include "utils/array.h"
 #include "utils/builtins.h"
 #include "utils/lsyscache.h"
 #include "utils/memutils.h"
@@ -211,6 +212,69 @@ translate_atom(OpExpr *op, TupleDesc tupdesc, CgQual *qual)
 	return true;
 }
 
+static int64 datum_to_i64(Datum d, Oid type);
+
+/* "x = ANY(array)" / "x <> ALL(array)" -- how PostgreSQL plans IN and NOT IN lists -- over a non-NULL constant array of the
+ * column's own type, with the type's btree equality (or its negator) -> a CG_OP_IN / CG_OP_NOT_IN atom whose list is appended
+ * to desc's list table: the elements as written, NULLs counted.  false for anything else, an empty array, or a full table */
+static bool
+translate_saop(ScalarArrayOpExpr *saop, TupleDesc tupdesc, CgScanDesc *desc, CgQual *qual)
+{
+	if (list_length(saop->args) != 2)
+		return false;
+	Var *var = strip_to_var((Node *) linitial(saop->args));
+	Node *r = (Node *) lsecond(saop->args);
+	Const *arr = (r && IsA(r, Const)) ? (Const *) r : NULL;
+	if (var == NULL || arr == NULL || arr->constisnull || var->varattno <= 0 || var->varattno > tupdesc->natts)
+		return false;
+	int attlen, type_class;
+	if (!type_is_supported(var->vartype, &attlen, &type_class) || get_element_type(arr->consttype) != var->vartype)
+		return false;
+	if (saop->useOr ? btree_strategy(saop->opno, var->vartype) != BTEqualStrategyNumber
+					: (get_negator(saop->opno) == InvalidOid || btree_strategy(get_negator(saop->opno), var->vartype) != BTEqualStrategyNumber))
+		return false;
+	int16 typlen;
+	bool typbyval;
+	char typalign;
+	get_typlenbyvalalign(var->vartype, &typlen, &typbyval, &typalign);
+	Datum *elems;
+	bool *nulls;
+	int n;
+	deconstruct_array(DatumGetArrayTypeP(arr->constvalue), var->vartype, typlen, typbyval, typalign, &elems, &nulls, &n);
+	int nvalues = 0;
+	for (int i = 0; i < n; i++)
+		nvalues += !nulls[i];
+	if (n == 0 || desc->nin_lists >= CG_MAX_IN_LISTS || desc->nin_values + nvalues > CG_MAX_IN_VALUES)
+		return false;
+	CgInList *list = &desc->in_lists[desc->nin_lists];
+	list->first = desc->nin_values;
+	list->nvalues = nvalues;
+	list->nnulls = n - nvalues;
+	list->reserved = 0;
+	for (int i = 0; i < n; i++)
+		if (!nulls[i])
+			desc->in_values[desc->nin_values++] = datum_to_i64(elems[i], var->vartype);     /* konst's convention */
+	qual->column = var->varattno - 1;
+	qual->op = saop->useOr ? CG_OP_IN : CG_OP_NOT_IN;
+	qual->konst = desc->nin_lists++;
+	return true;
+}
+
+/* "x IS [NOT] NULL" over a column of a supported type -> CG_OP_IS_NULL / CG_OP_IS_NOT_NULL */
+static bool
+translate_nulltest(NullTest *nt, TupleDesc tupdesc, CgQual *qual)
+{
+	Var *var = strip_to_var((Node *) nt->arg);
+	int attlen, type_class;
+	if (nt->argisrow || var == NULL || var->varattno <= 0 || var->varattno > tupdesc->natts ||
+		!type_is_supported(var->vartype, &attlen, &type_class))
+		return false;
+	qual->column = var->varattno - 1;
+	qual->op = nt->nulltesttype == IS_NULL ? CG_OP_IS_NULL : CG_OP_IS_NOT_NULL;
+	qual->konst = 0;
+	return true;
+}
+
 /* a bare bool column `flag` as the atom "flag = 1", and NOT flag as "flag = 0" (a NULL flag stays UNKNOWN either way) */
 static bool
 translate_bool_var(Node *node, bool negated, TupleDesc tupdesc, CgQual *qual)
@@ -227,9 +291,11 @@ translate_bool_var(Node *node, bool negated, TupleDesc tupdesc, CgQual *qual)
 /* boolean tree -> atoms appended to atoms[0 .. *natoms) (at most max_atoms) + postfix tokens appended to tokens[0 .. *ntokens)
  * (at most CG_MAX_QEXPR): the WHERE list (quals / qual_expr), aggregate FILTERs (filter_quals / filter_expr[a]) and the
  * predicate arguments of bool_and / bool_or / every (filter_quals / arg_expr[a]).  An atom is "Var op Const", a bare bool
- * Var, or NOT over a bare bool Var.  false when a node is anything else or the tree is too big */
+ * Var, NOT over a bare bool Var, an IN / NOT IN list over a Var (its list goes to desc's list table) or "Var IS [NOT] NULL".
+ * false when a node is anything else or the tree is too big */
 static bool
-translate_where(Node *node, TupleDesc tupdesc, CgQual *atoms, int32_t *natoms, int max_atoms, int8_t *tokens, int32_t *ntokens)
+translate_where(Node *node, TupleDesc tupdesc, CgScanDesc *desc, CgQual *atoms, int32_t *natoms, int max_atoms, int8_t *tokens,
+				int32_t *ntokens)
 {
 	if (IsA(node, BoolExpr))
 	{
@@ -247,7 +313,7 @@ translate_where(Node *node, TupleDesc tupdesc, CgQual *atoms, int32_t *natoms, i
 		int n = 0;
 		foreach(lc, b->args)
 		{
-			if (!translate_where((Node *) lfirst(lc), tupdesc, atoms, natoms, max_atoms, tokens, ntokens))
+			if (!translate_where((Node *) lfirst(lc), tupdesc, desc, atoms, natoms, max_atoms, tokens, ntokens))
 				return false;
 			if (n++ > 0)
 			{
@@ -260,7 +326,16 @@ translate_where(Node *node, TupleDesc tupdesc, CgQual *atoms, int32_t *natoms, i
 	}
 	if (*natoms >= max_atoms || *ntokens >= CG_MAX_QEXPR)
 		return false;
-	if (IsA(node, OpExpr) ? !translate_atom((OpExpr *) node, tupdesc, &atoms[*natoms]) : !translate_bool_var(node, false, tupdesc, &atoms[*natoms]))
+	bool ok;
+	if (IsA(node, OpExpr))
+		ok = translate_atom((OpExpr *) node, tupdesc, &atoms[*natoms]);
+	else if (IsA(node, ScalarArrayOpExpr))
+		ok = translate_saop((ScalarArrayOpExpr *) node, tupdesc, desc, &atoms[*natoms]);
+	else if (IsA(node, NullTest))
+		ok = translate_nulltest((NullTest *) node, tupdesc, &atoms[*natoms]);
+	else
+		ok = translate_bool_var(node, false, tupdesc, &atoms[*natoms]);
+	if (!ok)
 		return false;
 	tokens[(*ntokens)++] = (int8_t) (*natoms)++;
 	return true;
@@ -280,7 +355,7 @@ translate_aggref(Aggref *agg, TupleDesc tupdesc, CgScanDesc *desc, GpuOutColumn 
 	 * sum and count parts are one aggregate here: its non-NULL count rides along with the sum, under the same filter.) */
 	desc->nfilter_expr[desc->naggs] = 0;
 	if (agg->aggfilter != NULL &&
-		!translate_where((Node *) agg->aggfilter, tupdesc, desc->filter_quals, &desc->nfilter_quals, CG_MAX_FILTER_QUALS,
+		!translate_where((Node *) agg->aggfilter, tupdesc, desc, desc->filter_quals, &desc->nfilter_quals, CG_MAX_FILTER_QUALS,
 						 desc->filter_expr[desc->naggs], &desc->nfilter_expr[desc->naggs]))
 		return false;
 	out->index = desc->naggs;
@@ -301,7 +376,7 @@ translate_aggref(Aggref *agg, TupleDesc tupdesc, CgScanDesc *desc, GpuOutColumn 
 		 * shares with the FILTERs; three-valued: an UNKNOWN row is no input, no input at all is NULL (count 0) */
 		spec->kind = strcmp(name, "bool_or") == 0 ? CG_AGG_BOOL_OR : CG_AGG_BOOL_AND;
 		desc->narg_expr[desc->naggs] = 0;
-		if (!translate_where(arg, tupdesc, desc->filter_quals, &desc->nfilter_quals, CG_MAX_FILTER_QUALS, desc->arg_expr[desc->naggs],
+		if (!translate_where(arg, tupdesc, desc, desc->filter_quals, &desc->nfilter_quals, CG_MAX_FILTER_QUALS, desc->arg_expr[desc->naggs],
 							 &desc->narg_expr[desc->naggs]))
 			return false;
 		out->kind = GPU_OUT_MINMAX; out->type = BOOLOID;
@@ -375,7 +450,7 @@ translate_query(PlannerInfo *root, RelOptInfo *input_rel, GpuAggPlan *plan)
 	foreach(lc, input_rel->baserestrictinfo)
 	{
 		RestrictInfo *ri = (RestrictInfo *) lfirst(lc);
-		if (!(ok = translate_where((Node *) ri->clause, tupdesc, plan->desc.quals, &plan->desc.nquals, CG_MAX_QUALS, plan->desc.qual_expr,
+		if (!(ok = translate_where((Node *) ri->clause, tupdesc, &plan->desc, plan->desc.quals, &plan->desc.nquals, CG_MAX_QUALS, plan->desc.qual_expr,
 								   &plan->desc.nqual_expr)))
 			break;
 		if (nclauses++ > 0)

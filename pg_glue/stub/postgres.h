@@ -128,7 +128,7 @@ List *list_delete_ptr(List *list, void *datum);
 
 /* ---- nodes ---- */
 typedef enum NodeTag { T_Invalid = 0, T_Var, T_Const, T_OpExpr, T_BoolExpr, T_Aggref, T_TargetEntry, T_RelabelType, T_CustomScan, T_CustomScanState,
-					   T_CustomPath, T_Query, T_NullTest, T_FuncExpr } NodeTag;
+					   T_CustomPath, T_Query, T_NullTest, T_FuncExpr, T_ScalarArrayOpExpr } NodeTag;
 typedef struct Node { NodeTag type; } Node;
 #define nodeTag(nodeptr) (((const Node *) (nodeptr))->type)
 #define IsA(nodeptr, _type_) (nodeTag(nodeptr) == T_##_type_)
@@ -143,6 +143,9 @@ typedef struct OpExpr { Expr xpr; Oid opno; Oid opfuncid; Oid opresulttype; bool
 typedef enum BoolExprType { AND_EXPR, OR_EXPR, NOT_EXPR } BoolExprType;
 typedef struct BoolExpr { Expr xpr; BoolExprType boolop; List *args; } BoolExpr;
 typedef struct RelabelType { Expr xpr; Expr *arg; Oid resulttype; } RelabelType;
+typedef struct ScalarArrayOpExpr { Expr xpr; Oid opno; Oid opfuncid; Oid hashfuncid; Oid negfuncid; bool useOr; Oid inputcollid; List *args; int location; } ScalarArrayOpExpr;
+typedef enum NullTestType { IS_NULL, IS_NOT_NULL } NullTestType;
+typedef struct NullTest { Expr xpr; Expr *arg; NullTestType nulltesttype; bool argisrow; int location; } NullTest;
 typedef struct Aggref { Expr xpr; Oid aggfnoid; Oid aggtype; List *args; List *aggorder; List *aggdistinct; Expr *aggfilter; bool aggstar; char aggkind; } Aggref;
 typedef struct TargetEntry { Expr xpr; Expr *expr; AttrNumber resno; char *resname; unsigned ressortgroupref; bool resjunk; } TargetEntry;
 typedef struct SortGroupClause { NodeTag type; unsigned tleSortGroupRef; Oid eqop; } SortGroupClause;
@@ -180,6 +183,8 @@ Oid GetDefaultOpClass(Oid type_id, Oid am_id);
 Oid get_opclass_family(Oid opclass);
 void get_typlenbyvalalign(Oid typid, int16 *typlen, bool *typbyval, char *typalign);
 Oid get_commutator(Oid opno);
+Oid get_negator(Oid opno);
+Oid get_element_type(Oid typid);
 
 /* ---- fmgr.h ---- */
 typedef struct FmgrInfo { void *fn_addr; Oid fn_oid; short fn_nargs; bool fn_strict; void *fn_extra; MemoryContext fn_mcxt; Node *fn_expr; } FmgrInfo;
@@ -217,6 +222,7 @@ Datum int8out(PG_FUNCTION_ARGS);
 char *text_to_cstring(const text *t);
 text *cstring_to_text(const char *s);
 typedef struct ArrayType ArrayType;
+ArrayType *DatumGetArrayTypeP(Datum d);
 void deconstruct_array(ArrayType *array, Oid elmtype, int elmlen, bool elmbyval, char elmalign, Datum **elemsp, bool **nullsp, int *nelemsp);
 void getTypeOutputInfo(Oid type, Oid *typOutput, bool *typIsVarlena);
 char *OidOutputFunctionCall(Oid functionId, Datum val);
