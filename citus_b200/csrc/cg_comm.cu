@@ -527,6 +527,7 @@ extern "C" int cg_comm_combine(CgPartial *p, int32_t root, int32_t local_status)
 {
 	CgContext *ctx = cg_ctx();
 	if (!ctx) return CG_EINVAL;
+	if (int rc0 = cg_chain_end(ctx, ctx->compute)) return rc0;
 	if (!g_comm.ready) return cg_set_error(CG_EINVAL, "cg_comm_init() has not been called");
 	if (!p) return cg_set_error(CG_EINVAL, "NULL partial");
 	if (root < 0 || root >= g_comm.nranks) return cg_set_error(CG_EINVAL, "root %d of %d ranks", root, g_comm.nranks);
@@ -888,6 +889,7 @@ extern "C" int cg_comm_repartition_exchange(int32_t slot, const int64_t *const *
 {
 	CgContext *ctx = cg_ctx();
 	if (!ctx) return CG_EINVAL;
+	if (int rc0 = cg_chain_end(ctx, ctx->compute)) return rc0;
 	if (!g_comm.ready) return cg_set_error(CG_EINVAL, "cg_comm_init() has not been called");
 	if (slot < 0 || slot >= 4) return cg_set_error(CG_EINVAL, "slot %d", slot);
 	if (ncols < 1 || ncols > 8 || !d_cols || n < 0) return cg_set_error(CG_EINVAL, "bad argument");
@@ -1013,6 +1015,7 @@ extern "C" int cg_comm_exchange_wait(int32_t slot)
 {
 	CgContext *ctx = cg_ctx();
 	if (!ctx) return CG_EINVAL;
+	if (int rc0 = cg_chain_end(ctx, ctx->compute)) return rc0;
 	if (slot < 0 || slot >= 4 || !g_comm.slots[slot].done) return cg_set_error(CG_EINVAL, "no exchange in slot %d", slot);
 	CG_CUDA(cudaStreamWaitEvent(ctx->compute, g_comm.slots[slot].done, 0));
 	return CG_OK;

@@ -575,6 +575,8 @@ int cg_launch_decompress(CgContext *ctx, uint8_t *arena, const DecodeItem *items
 						 unsigned long long *err, unsigned long long flag, cudaStream_t stream)
 {
 	if (nitems == 0) return CG_OK;
+	int rc = cg_chain_end(ctx, stream);
+	if (rc) return rc;
 	if (g_lz4_lanes < 0) { const char *e = getenv("CG_LZ4_LANES"); g_lz4_lanes = e ? atoi(e) : CG_LZ4_LANES_DEFAULT; if (g_lz4_lanes < 0 || g_lz4_lanes > 2) g_lz4_lanes = CG_LZ4_LANES_DEFAULT; }
 	const int use_lanes = g_lz4_lanes == 2 ? (nitems <= (uint64_t) ctx->sm_count * CG_LZ4_LANES_MAX_WARPS_PER_SM ? 1 : 0) : g_lz4_lanes;
 	bool any_lz = false, any_zstd = false, any_lz4 = false;

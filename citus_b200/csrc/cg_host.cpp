@@ -165,21 +165,71 @@ extern "C" int cg_set_stream(void *cuda_stream)
 {
 	CgContext *ctx = cg_ctx();
 	if (!ctx) return CG_EINVAL;
+	int rc = cg_chain_end(ctx, ctx->compute);
+	if (rc) return rc;
 	CG_CUDA(cudaStreamSynchronize(ctx->compute));
 	ctx->compute = cuda_stream ? (cudaStream_t) cuda_stream : ctx->own_compute;
 	return CG_OK;
 }
 
-int cg_prof_mark(CgContext *ctx, cudaStream_t stream)
+/* ------------------------------------------------------------------------------ *
+ *  Chains of scan launches.
+ *
+ *  The scans of one query -- one call per shard -- follow each other on the compute stream.  Left alone, every launch
+ *  ends with a ramp-down in which the SMs run fewer and fewer CTAs, and the next launch waits for the last one.  So a
+ *  fast or generated scan kernel launched right after another scan launch is launched with programmatic stream
+ *  serialization, and those kernels execute griddepcontrol.launch_dependents as they start (never
+ *  griddepcontrol.wait): the next launch's CTAs take the SM slots the previous launch's last CTAs leave free.
+ *
+ *  Why that is correct.  A chained scan reads only inputs that were complete before the head of its chain started:
+ *  the staged arena, the chunk descriptors, the selected chunk-group list and the IN lists, which host copies and
+ *  kernels enqueued before the head wrote (any such enqueue in between ends the chain).  It writes only commutative
+ *  updates -- red.add / atomicAdd / atomicMin / atomicMax / atomicOr into the group table and the statistics words,
+ *  the CAS insert of a key into a hash table -- so any interleaving of two chained launches leaves the same table.
+ *  Everything that reads or rewrites the table (drain, export, merge, reset, statistics copies, the combine) is an
+ *  ordinary stream operation and waits for the whole chain.  The interpretive kernels do not trigger early; they
+ *  are launched without the attribute and end a chain.
+ *
+ *  The rule needs one fact, ctx->scan_chain: was the library's last enqueue on the compute stream a chainable scan
+ *  launch?  cg_chain_scan() is the only place that sets it; cg_chain_end(), which every other enqueue on the compute
+ *  stream calls first, clears it.
+ *
+ *  Profiling (cg_profile_begin) records one event before the first launch of a chain and one when the chain ends, so
+ *  no mark stands between two chained launches.
+ * ------------------------------------------------------------------------------ */
+static int prof_record(CgContext *ctx)
 {
-	if (!ctx->profiling) return CG_OK;
 	if (ctx->prof_used == ctx->prof_events.size())
 	{
 		cudaEvent_t e;
 		CG_CUDA(cudaEventCreate(&e));
 		ctx->prof_events.push_back(e);
 	}
-	CG_CUDA(cudaEventRecord(ctx->prof_events[ctx->prof_used++], stream));
+	CG_CUDA(cudaEventRecord(ctx->prof_events[ctx->prof_used++], ctx->compute));
+	return CG_OK;
+}
+
+int cg_chain_end(CgContext *ctx, cudaStream_t stream)
+{
+	if (stream != ctx->compute || ctx->scan_chain == CG_CHAIN_NONE) return CG_OK;
+	ctx->scan_chain = CG_CHAIN_NONE;
+	return (ctx->profiling && ctx->prof_used % 2 == 1) ? prof_record(ctx) : CG_OK;
+}
+
+int cg_chain_scan(CgContext *ctx, cudaStream_t stream, bool chainable, bool *overlap)
+{
+	*overlap = false;
+	if (stream != ctx->compute) return CG_OK;
+	if (ctx->scan_chain == CG_CHAIN_OPEN && chainable) *overlap = true;
+	else
+	{
+		int rc = cg_chain_end(ctx, stream);
+		if (rc) return rc;
+		if (ctx->profiling) rc = prof_record(ctx);
+		if (rc) return rc;
+	}
+	if (ctx->profiling) ctx->prof_launches++;
+	ctx->scan_chain = chainable ? CG_CHAIN_OPEN : CG_CHAIN_CLOSED;
 	return CG_OK;
 }
 
@@ -187,8 +237,18 @@ extern "C" int cg_profile_begin(void)
 {
 	CgContext *ctx = cg_ctx();
 	if (!ctx) return CG_EINVAL;
+	int rc = cg_chain_end(ctx, ctx->compute);      /* a chain that started unprofiled has no start mark */
+	if (rc) return rc;
+	/* events for 128 chains, created here rather than between the launches that are being timed */
+	while (ctx->prof_events.size() < 256)
+	{
+		cudaEvent_t e;
+		CG_CUDA(cudaEventCreate(&e));
+		ctx->prof_events.push_back(e);
+	}
 	ctx->profiling = true;
 	ctx->prof_used = 0;
+	ctx->prof_launches = 0;
 	return CG_OK;
 }
 
@@ -196,6 +256,8 @@ extern "C" int cg_profile_collect(int32_t *launches, double *total_ms, double *m
 {
 	CgContext *ctx = cg_ctx();
 	if (!ctx) return CG_EINVAL;
+	int rc = cg_chain_end(ctx, ctx->compute);
+	if (rc) return rc;
 	ctx->profiling = false;
 	double total = 0, mx = 0;
 	size_t n = ctx->prof_used / 2;
@@ -207,10 +269,11 @@ extern "C" int cg_profile_collect(int32_t *launches, double *total_ms, double *m
 		total += ms;
 		if (ms > mx) mx = ms;
 	}
-	if (launches) *launches = (int32_t) n;
+	if (launches) *launches = (int32_t) ctx->prof_launches;
 	if (total_ms) *total_ms = total;
 	if (max_ms) *max_ms = mx;
 	ctx->prof_used = 0;
+	ctx->prof_launches = 0;
 	return CG_OK;
 }
 
@@ -818,6 +881,8 @@ extern "C" int cg_shard_stage(const CgRelation *rel, const int32_t *columns, int
 	VarlenaItem *d_varlena = nullptr;
 	if (!sp.decode.empty() || !sp.varlena.empty())
 	{
+		rc = cg_chain_end(ctx, ctx->compute);
+		if (rc) { cg_shard_free(sh); return rc; }
 		if ((!sp.decode.empty() && (cudaMalloc(&d_decode, sp.decode.size() * sizeof(DecodeItem)) != cudaSuccess ||
 									cudaMemcpy(d_decode, sp.decode.data(), sp.decode.size() * sizeof(DecodeItem), cudaMemcpyHostToDevice) != cudaSuccess)) ||
 			(!sp.varlena.empty() && (cudaMalloc(&d_varlena, sp.varlena.size() * sizeof(VarlenaItem)) != cudaSuccess ||
@@ -833,8 +898,9 @@ extern "C" int cg_shard_stage(const CgRelation *rel, const int32_t *columns, int
 		uint32_t f = sp.dec_first[cg0], l = sp.dec_first[cg1];
 		uint32_t vf = sp.vl_first[cg0], vl = sp.vl_first[cg1];
 		if (f == l && vf == vl) return CG_OK;
+		int r = cg_chain_end(ctx, ctx->compute);
+		if (r) return r;
 		CG_CUDA(cudaStreamWaitEvent(ctx->compute, copied, 0));
-		int r = CG_OK;
 		if (f != l)
 			r = cg_launch_decompress(ctx, sh->d_arena, d_decode + f, sp.decode.data() + f, l - f, ctx->d_stage_err, CG_ERRFLAG_DECOMPRESS,
 									 ctx->compute);
@@ -1029,6 +1095,8 @@ static int stats_begin(CgContext *ctx, CgPartial *p, const CgScanStats *stats, u
 {
 	before[0] = before[1] = before[2] = 0;
 	if (!stats) return CG_OK;
+	int rc = cg_chain_end(ctx, ctx->compute);
+	if (rc) return rc;
 	CG_CUDA(cudaMemcpyAsync(before, p->d_stats, 3 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->compute));
 	CG_CUDA(cudaStreamSynchronize(ctx->compute));
 	return CG_OK;
@@ -1041,9 +1109,11 @@ static int stats_end(CgContext *ctx, CgPartial *p, const unsigned long long befo
 	if (!stats) return CG_OK;
 	memset(stats, 0, sizeof *stats);
 	unsigned long long after[3];
+	int rc = cg_chain_end(ctx, ctx->compute);
+	if (rc) return rc;
 	CG_CUDA(cudaMemcpyAsync(after, p->d_stats, sizeof after, cudaMemcpyDeviceToHost, ctx->compute));
 	CG_CUDA(cudaStreamSynchronize(ctx->compute));
-	int rc = check_error_flags(p, after[2]);
+	rc = check_error_flags(p, after[2]);
 	if (rc) return rc;
 	stats->rows_scanned = (int64_t) (after[0] - before[0]);
 	stats->rows_removed_by_filter = (int64_t) (after[1] - before[1]);
@@ -1084,6 +1154,8 @@ static int upload_sets(CgContext *ctx, CgPartial *p, const std::vector<uint64_t>
 	CG_CUDA(cudaEventSynchronize(p->sets_copied[slot]));       /* the slot's previous copy has read it */
 	memcpy(p->h_sets[slot], codes.data(), codes.size() * sizeof(uint64_t));
 	p->sets_last.clear();                                      /* the buffer's content is unknown until the copy is enqueued */
+	int rc = cg_chain_end(ctx, ctx->compute);
+	if (rc) return rc;
 	CG_CUDA(cudaMemcpyAsync(p->d_sets, p->h_sets[slot], codes.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->compute));
 	CG_CUDA(cudaEventRecord(p->sets_copied[slot], ctx->compute));
 	p->sets_last = codes;
@@ -1142,6 +1214,8 @@ extern "C" int cg_scan_shard(const CgShard *sh, const CgScanDesc *desc, CgPartia
 		}
 		msh->sel_nfast = (uint32_t) fastl.size();
 		fastl.insert(fastl.end(), slowl.begin(), slowl.end());
+		rc = cg_chain_end(ctx, ctx->compute);             /* the launches after the rewrite read the new list */
+		if (rc) return rc;
 		CG_CUDA(cudaStreamSynchronize(ctx->compute));     /* an earlier scan may still read the old list */
 		if (!fastl.empty())
 			CG_CUDA(cudaMemcpy(msh->d_selected, fastl.data(), fastl.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
@@ -1181,9 +1255,7 @@ extern "C" int cg_scan_shard(const CgShard *sh, const CgScanDesc *desc, CgPartia
 		plan.max_cg_rows = sh->sel_max_cg_rows;
 		FPlan fplan;
 		const FPlan *fast = fast_eligible(desc, plan, all8, &fplan) ? &fplan : nullptr;
-		if (stats) CG_CUDA(cudaEventRecord(ctx->ev_a, ctx->compute));
-		rc = cg_prof_mark(ctx, ctx->compute);
-		if (rc) return rc;
+		if (stats) CG_CUDA(cudaEventRecord(ctx->ev_a, ctx->compute));     /* stats_begin has ended the chain */
 		/* the chunk groups without NULLs in the plan columns come first in the selection; when no specialised kernel
 		 * takes them they join the rest */
 		KPlan rest = plan;
@@ -1211,9 +1283,12 @@ extern "C" int cg_scan_shard(const CgShard *sh, const CgScanDesc *desc, CgPartia
 			if (rc == CG_OK && !taken) rc = scan_interpretive(ctx, into, rest, all8, rest_rows);
 			if (rc) return rc;
 		}
-		rc = cg_prof_mark(ctx, ctx->compute);
-		if (rc) return rc;
-		if (stats) CG_CUDA(cudaEventRecord(ctx->ev_b, ctx->compute));
+		if (stats)
+		{
+			rc = cg_chain_end(ctx, ctx->compute);
+			if (rc) return rc;
+			CG_CUDA(cudaEventRecord(ctx->ev_b, ctx->compute));
+		}
 	}
 	return stats_end(ctx, into, before, filtered, selected.size(), bytes, stats);
 }
@@ -1470,6 +1545,7 @@ extern "C" int cg_scan_relation(const CgRelation *rel, const CgScanDesc *desc, C
 				if (!armed) return;
 				cudaStreamSynchronize(ctx->copy);
 				if (side) cudaStreamSynchronize(side);
+				cg_chain_end(ctx, ctx->compute);
 				cudaEventRecord(ctx->dma_done[slot], ctx->compute);
 			}
 		} slot_guard{ctx, mslot};
@@ -1515,13 +1591,16 @@ extern "C" int cg_scan_relation(const CgRelation *rel, const CgScanDesc *desc, C
 					const DevChunkCol &d = sp.cols[g * ns + plan.slot[c]];
 					if (d.value_count != d.row_count) nullable |= 1u << c;
 				}
+		rc = cg_chain_end(ctx, ctx->compute);
+		if (rc) return rc;
 		if (stats) CG_CUDA(cudaEventRecord(ctx->ev_a, ctx->compute));
 		bool decode_done = false;          /* the DMA path may decode on a side stream before launch_block runs */
 		auto block_rows = [&](uint64_t cg0, uint64_t cg1) { uint64_t n = 0; for (uint64_t g = cg0; g < cg1; g++) n += sp.cg_rows[g]; return n; };
 		auto launch_block = [&](uint64_t cg0, uint64_t cg1, cudaEvent_t copied) -> int {
+			int r = cg_chain_end(ctx, ctx->compute);
+			if (r) return r;
 			CG_CUDA(cudaStreamWaitEvent(ctx->compute, copied, 0));
 			/* K7: compressed value streams of the block -> their value slots */
-			int r = CG_OK;
 			if (!decode_done)
 			{
 				r = cg_launch_decompress(ctx, d_arena, d_decode + sp.dec_first[cg0], sp.decode.data() + sp.dec_first[cg0],
@@ -1536,8 +1615,6 @@ extern "C" int cg_scan_relation(const CgRelation *rel, const CgScanDesc *desc, C
 				r = cg_launch_rank(ctx, d_arena, d_cols, cg0 * ns, (cg1 - cg0) * ns, ctx->compute);
 				if (r) return r;
 			}
-			r = cg_prof_mark(ctx, ctx->compute);
-			if (r) return r;
 			KPlan blk = plan;
 			blk.selected = d_ids + cg0;
 			blk.nselected = (uint32_t) (cg1 - cg0);
@@ -1545,8 +1622,7 @@ extern "C" int cg_scan_relation(const CgRelation *rel, const CgScanDesc *desc, C
 			bool taken = false;
 			r = scan_specialised(ctx, into, blk, fast, nullable, rows, &taken);
 			if (r == CG_OK && !taken) r = scan_interpretive(ctx, into, blk, all8, rows);
-			if (r) return r;
-			return cg_prof_mark(ctx, ctx->compute);
+			return r;
 		};
 		if (dma)
 		{
@@ -1605,7 +1681,7 @@ extern "C" int cg_scan_relation(const CgRelation *rel, const CgScanDesc *desc, C
 			}
 			else
 			{
-				CG_CUDA(cudaStreamWaitEvent(ctx->compute, ctx->dma_copied, 0));
+				CG_CUDA(cudaStreamWaitEvent(ctx->compute, ctx->dma_copied, 0));     /* the chain ended above */
 				rc = cg_launch_realign(d_raw, d_arena, (const RealignItem *) (d_meta + off_items), items.size(), ctx->compute);
 			}
 			if (trace) cudaEventRecord(k1, ctx->compute);
@@ -1625,8 +1701,10 @@ extern "C" int cg_scan_relation(const CgRelation *rel, const CgScanDesc *desc, C
 		}
 		else
 			rc = stream_to_device(ctx, rel, sp, ns, d_arena, launch_block);
-		if (stats && rc == CG_OK) CG_CUDA(cudaEventRecord(ctx->ev_b, ctx->compute));
 		if (rc) return rc;                  /* slot_guard drains the side streams and records the event */
+		rc = cg_chain_end(ctx, ctx->compute);
+		if (rc) return rc;
+		if (stats) CG_CUDA(cudaEventRecord(ctx->ev_b, ctx->compute));
 		CG_CUDA(cudaEventRecord(ctx->dma_done[mslot], ctx->compute));
 		slot_guard.armed = false;
 	}
@@ -1658,7 +1736,8 @@ static int ensure_out(CgPartial *p, uint64_t cap)
 /* makes the exact accumulators current (drains packed words), then surfaces kernel-side errors */
 static int pending_errors(CgContext *ctx, CgPartial *p)
 {
-	int rc = cg_launch_drain(p, ctx->compute);
+	int rc = cg_chain_end(ctx, ctx->compute);
+	if (rc == CG_OK) rc = cg_launch_drain(p, ctx->compute);
 	if (rc) return rc;
 	unsigned long long st[5];
 	CG_CUDA(cudaMemcpyAsync(st, p->d_stats, sizeof st, cudaMemcpyDeviceToHost, ctx->compute));
@@ -1688,7 +1767,8 @@ static int export_rows(CgContext *ctx, CgPartial *p, uint64_t capacity, int64_t 
 	/* the packed export's key of entry e is key_min + e: one-column keys and composite codes */
 	const bool direct = p->d_packed && p->packed_dirty && !p->wide_dirty && p->mode == CG_MODE_DENSE &&
 						(p->desc.ngroup_cols == 1 || p->desc.composite_key);
-	int rc;
+	int rc = cg_chain_end(ctx, ctx->compute);
+	if (rc) return rc;
 	if (direct)
 	{
 		rc = cg_launch_export_packed(p, capacity, d_keys, d_nulls, d_words, p->d_out_count, ctx->compute);

@@ -74,12 +74,21 @@ struct CgContext
 	uint8_t *zstd_scratch = nullptr;             /* literal buffers of the resident zstd decoders */
 	size_t zstd_scratch_bytes = 0;
 	unsigned long long *d_stage_err = nullptr;   /* error flags raised by staging kernels of cg_shard_stage */
-	/* per-launch profiling */
+	/* the library's last enqueue on the compute stream was a scan launch: CG_CHAIN_* (see cg_chain_scan) */
+	int scan_chain = 0;
+	/* scan profiling: one (start, end) event pair per chain of scan launches */
 	bool profiling = false;
-	std::vector<cudaEvent_t> prof_events;   /* pairs */
+	std::vector<cudaEvent_t> prof_events;
 	size_t prof_used = 0;
+	uint64_t prof_launches = 0;
 };
-int cg_prof_mark(CgContext *ctx, cudaStream_t stream);   /* records the next event of the pool when profiling */
+enum { CG_CHAIN_NONE = 0, CG_CHAIN_OPEN = 1, CG_CHAIN_CLOSED = 2 };
+/* called by the scan launch helpers right before a scan launch on `stream`; *overlap = true: launch it with programmatic
+ * stream serialization (it may overlap the previous scan launch).  chainable = false for the interpretive kernels. */
+int cg_chain_scan(CgContext *ctx, cudaStream_t stream, bool chainable, bool *overlap);
+/* called before every other enqueue of the library on `stream`: ends the chain of scan launches when `stream` is the
+ * compute stream */
+int cg_chain_end(CgContext *ctx, cudaStream_t stream);
 CgContext *cg_ctx(void);   /* NULL + error set if cg_init has not run */
 int cg_ensure_pinned(CgContext *ctx);
 

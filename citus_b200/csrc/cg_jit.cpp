@@ -41,9 +41,11 @@
 #include <string>
 #include <vector>
 
+#include <cuda.h>      /* types only (CUlaunchConfig); the driver API itself is resolved with dlsym */
+
 #include "cg_internal.h"
 
-/* ---- minimal NVRTC / driver API surface (headers are not needed: opaque handles + ints) ---- */
+/* ---- minimal NVRTC / driver API surface (opaque handles + ints) ---- */
 typedef struct _nvrtcProgram *nvrtcProgram;
 typedef int (*nvrtcCreateProgram_t)(nvrtcProgram *, const char *, const char *, int, const char *const *, const char *const *);
 typedef int (*nvrtcCompileProgram_t)(nvrtcProgram, int, const char *const *);
@@ -56,7 +58,7 @@ typedef int (*cuModuleLoadData_t)(CUmodule *, const void *);
 typedef int (*cuModuleGetFunction_t)(CUfunction *, CUmodule, const char *);
 typedef int (*cuFuncSetAttribute_t)(CUfunction, int, int);
 typedef int (*cuOccupancy_t)(int *, CUfunction, int, size_t);
-typedef int (*cuLaunchKernel_t)(CUfunction, unsigned, unsigned, unsigned, unsigned, unsigned, unsigned, unsigned, void *, void **, void **);
+typedef int (*cuLaunchKernelEx_t)(const CUlaunchConfig *, CUfunction, void **, void **);
 typedef int (*cuGetErrorString_t)(int, const char **);
 #define CG_CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES 8
 
@@ -66,7 +68,7 @@ static struct
 	nvrtcCreateProgram_t create; nvrtcCompileProgram_t compile; nvrtcGetSize_t cubin_size, log_size;
 	nvrtcGetData_t cubin, log; nvrtcDestroyProgram_t destroy;
 	cuModuleLoadData_t load; cuModuleGetFunction_t getfn; cuFuncSetAttribute_t setattr; cuOccupancy_t occupancy;
-	cuLaunchKernel_t launch; cuGetErrorString_t errstr;
+	cuLaunchKernelEx_t launch; cuGetErrorString_t errstr;
 } g_api;
 
 static bool load_rtc()
@@ -98,7 +100,7 @@ static bool load_drv()
 	g_api.getfn = (cuModuleGetFunction_t) dlsym(h, "cuModuleGetFunction");
 	g_api.setattr = (cuFuncSetAttribute_t) dlsym(h, "cuFuncSetAttribute");
 	g_api.occupancy = (cuOccupancy_t) dlsym(h, "cuOccupancyMaxActiveBlocksPerMultiprocessor");
-	g_api.launch = (cuLaunchKernel_t) dlsym(h, "cuLaunchKernel");
+	g_api.launch = (cuLaunchKernelEx_t) dlsym(h, "cuLaunchKernelEx");
 	g_api.errstr = (cuGetErrorString_t) dlsym(h, "cuGetErrorString");
 	g_api.have_drv = g_api.load && g_api.getfn && g_api.setattr && g_api.occupancy && g_api.launch;
 	return g_api.have_drv;
@@ -921,15 +923,18 @@ static void gen_row(std::string &s, const KPlan &plan, const JitShape &sh, int u
 	addf(s, "%s}\n%s}\n\t\t\t\t\t}\n", B, T);
 }
 
+/* the generated kernel's signature and the opening brace of its body */
+#define JIT_ENTRY "cg_jit_scan(const __grid_constant__ KPlan P)\n{\n"
+
 static std::string gen_source(const KPlan &plan, const JitShape &sh)
 {
 	std::string s;
 	s.reserve(32768);
 	gen_prelude(s, plan);
 	if (sh.min_blocks > 0)
-		addf(s, "extern \"C\" __global__ void __launch_bounds__(%d, %d) cg_jit_scan(const __grid_constant__ KPlan P)\n{\n", JIT_THREADS, sh.min_blocks);
+		addf(s, "extern \"C\" __global__ void __launch_bounds__(%d, %d) %s", JIT_THREADS, sh.min_blocks, JIT_ENTRY);
 	else
-		addf(s, "extern \"C\" __global__ void __launch_bounds__(%d) cg_jit_scan(const __grid_constant__ KPlan P)\n{\n", JIT_THREADS);
+		addf(s, "extern \"C\" __global__ void __launch_bounds__(%d) %s", JIT_THREADS, JIT_ENTRY);
 	s += "\tconst uint32_t tid = threadIdx.x;\n\tuint32_t removed = 0;\n\tunsigned long long scanned = 0;\n\tuint64_t g_rows = 0;\n";
 	if (sh.kind == JK_GLOBAL)
 		for (int a = 0; a < plan.naggs; a++)
@@ -1165,9 +1170,15 @@ static std::map<std::string, JitKernel> g_cache;
 static std::mutex g_cache_mutex;
 static unsigned long long g_jit_compiles = 0, g_jit_launches = 0;
 
-static int compile_source(const std::string &src, std::string *cubin)
+/* compiles a plan's generated source as it is launched: the kernel's first statement lets the next scan launch of a
+ * chain start as soon as every CTA of this one runs (cg_chain_scan, cg_host.cpp) */
+static int compile_source(const std::string &plan_src, std::string *cubin)
 {
 	if (!load_rtc()) return cg_set_error(CG_EUNSUPPORTED, "libnvrtc is not available");
+	const size_t body = plan_src.find(JIT_ENTRY);
+	if (body == std::string::npos) return cg_set_error(CG_EINVAL, "generated source without the kernel entry");
+	const size_t at = body + strlen(JIT_ENTRY);
+	const std::string src = plan_src.substr(0, at) + "\tasm volatile(\"griddepcontrol.launch_dependents;\" ::: \"memory\");\n" + plan_src.substr(at);
 	nvrtcProgram prog = nullptr;
 	if (g_api.create(&prog, src.c_str(), "cg_jit_scan.cu", 0, nullptr, nullptr) != 0)
 		return cg_set_error(CG_ECUDA, "nvrtcCreateProgram failed");
@@ -1286,12 +1297,27 @@ int cg_launch_scan_jit(CgContext *ctx, const KPlan &plan, uint32_t nullable, cud
 		}
 		uint32_t grid = (uint32_t) std::min<uint64_t>(grid_full, (uint64_t) piece.nselected * (uint64_t) piece.slices);
 		void *args[] = {&piece};
-		int e = g_api.launch(k->fn, grid, 1, 1, JIT_THREADS, 1, 1, (unsigned) smem, (void *) stream, args, nullptr);
+		bool overlap;
+		int rc = cg_chain_scan(ctx, stream, true, &overlap);
+		if (rc) return rc;
+		CUlaunchAttribute attr;
+		memset(&attr, 0, sizeof attr);
+		attr.id = CU_LAUNCH_ATTRIBUTE_PROGRAMMATIC_STREAM_SERIALIZATION;
+		attr.value.programmaticStreamSerializationAllowed = 1;
+		CUlaunchConfig cfg;
+		memset(&cfg, 0, sizeof cfg);
+		cfg.gridDimX = grid; cfg.gridDimY = 1; cfg.gridDimZ = 1;
+		cfg.blockDimX = JIT_THREADS; cfg.blockDimY = 1; cfg.blockDimZ = 1;
+		cfg.sharedMemBytes = (unsigned) smem;
+		cfg.hStream = (CUstream) stream;
+		cfg.attrs = &attr;
+		cfg.numAttrs = overlap ? 1 : 0;
+		int e = g_api.launch(&cfg, k->fn, args, nullptr);
 		if (e != 0)
 		{
 			const char *msg = nullptr;
 			if (g_api.errstr) g_api.errstr(e, &msg);
-			return cg_set_error(CG_ECUDA, "cuLaunchKernel of the plan-specialised kernel failed: %s", msg ? msg : "?");
+			return cg_set_error(CG_ECUDA, "cuLaunchKernelEx of the plan-specialised kernel failed: %s", msg ? msg : "?");
 		}
 		g_cg_launches++;
 		g_jit_launches++;

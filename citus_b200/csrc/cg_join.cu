@@ -144,6 +144,7 @@ extern "C" int cg_join_count_sum(const int64_t *d_build_keys, const uint8_t *d_b
 {
 	CgContext *ctx = cg_ctx();
 	if (!ctx) return CG_EINVAL;
+	if (int rc0 = cg_chain_end(ctx, ctx->compute)) return rc0;
 	if (nbuild < 0 || nprobe < 0 || !joined_rows || !sum_hi || !sum_lo) return cg_set_error(CG_EINVAL, "bad argument");
 	if ((nbuild > 0 && (!d_build_keys || !d_build_payload)) || (nprobe > 0 && (!d_probe_keys || !d_probe_payload)))
 		return cg_set_error(CG_EINVAL, "NULL column");
@@ -335,6 +336,7 @@ extern "C" int cg_join_rows(const int64_t *d_build_keys, const uint8_t *d_build_
 {
 	CgContext *ctx = cg_ctx();
 	if (!ctx) return CG_EINVAL;
+	if (int rc0 = cg_chain_end(ctx, ctx->compute)) return rc0;
 	if (nbuild < 0 || nprobe < 0 || capacity < 0 || !nrows) return cg_set_error(CG_EINVAL, "bad argument");
 	if ((nbuild > 0 && (!d_build_keys || !d_build_payload)) || (nprobe > 0 && (!d_probe_keys || !d_probe_payload)))
 		return cg_set_error(CG_EINVAL, "NULL column");

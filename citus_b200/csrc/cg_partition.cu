@@ -504,6 +504,7 @@ int cg_partition_index_async(const int64_t *d_keys, const uint8_t *d_nulls, int6
 {
 	CgContext *ctx = cg_ctx();
 	if (!ctx) return CG_EINVAL;
+	if (int rc0 = cg_chain_end(ctx, ctx->compute)) return rc0;
 	return partition_index_enqueue(ctx, d_keys, d_nulls, n, key_len, by_hash, mins, maxs, P, d_index, d_counts,
 								   (unsigned long long *) (d_counts + P));
 }
@@ -514,6 +515,7 @@ extern "C" int cg_partition_index(const int64_t *d_keys, const uint8_t *d_nulls,
 {
 	CgContext *ctx = cg_ctx();
 	if (!ctx) return CG_EINVAL;
+	if (int rc0 = cg_chain_end(ctx, ctx->compute)) return rc0;
 	CgAsyncBuf err_buf;
 	CG_CUDA(err_buf.alloc(sizeof(unsigned long long), ctx->compute));
 	unsigned long long *d_err = err_buf.as<unsigned long long>();
@@ -737,6 +739,7 @@ int cg_partition_scatter_async(const int32_t *d_index, int64_t n, int32_t P, con
 {
 	CgContext *ctx = cg_ctx();
 	if (!ctx) return CG_EINVAL;
+	if (int rc0 = cg_chain_end(ctx, ctx->compute)) return rc0;
 	return partition_scatter_enqueue(ctx, d_index, n, P, h_order, d_cols, ncols, d_out, nullptr);
 }
 
@@ -750,6 +753,7 @@ int cg_partition_route_scatter_async(const int64_t *d_keys, const uint8_t *d_nul
 {
 	CgContext *ctx = cg_ctx();
 	if (!ctx) return CG_EINVAL;
+	if (int rc0 = cg_chain_end(ctx, ctx->compute)) return rc0;
 	if (P <= 0 || P > CGP_MAX_P) return cg_set_error(CG_EINVAL, "bad partition count %d", P);
 	if (key_len != 4 && key_len != 8) return cg_set_error(CG_EINVAL, "key_len must be 4 or 8");
 	if (ncols < 1 || ncols > 8 || n < 0 || !d_counts || !mins || !maxs || !h_order) return cg_set_error(CG_EINVAL, "bad argument");
@@ -841,6 +845,7 @@ extern "C" int cg_partition_scatter_ordered(const int32_t *d_index, int64_t n, i
 {
 	CgContext *ctx = cg_ctx();
 	if (!ctx) return CG_EINVAL;
+	if (int rc0 = cg_chain_end(ctx, ctx->compute)) return rc0;
 	if (!h_offsets) return cg_set_error(CG_EINVAL, "NULL offsets");
 	return partition_scatter_enqueue(ctx, d_index, n, P, h_order, d_cols, ncols, d_out, h_offsets);
 }
@@ -933,6 +938,7 @@ extern "C" int cg_partition_copy_bytes(const int32_t *d_index, int64_t n, int32_
 {
 	CgContext *ctx = cg_ctx();
 	if (!ctx) return CG_EINVAL;
+	if (int rc0 = cg_chain_end(ctx, ctx->compute)) return rc0;
 	if (P < 1 || P > CGP_MAX_P) return cg_set_error(CG_EINVAL, "partition count %d out of range", P);
 	if (ncols < 1 || ncols > CGP_MAX_COLS) return cg_set_error(CG_EUNSUPPORTED, "1..%d columns", CGP_MAX_COLS);
 	if (n < 0 || !d_cols || !col_len || !rows_written || !bytes_written) return cg_set_error(CG_EINVAL, "bad argument");
@@ -1135,6 +1141,7 @@ extern "C" int cg_partition_copy_serialize(const int32_t *d_index, int64_t n, in
 {
 	CgContext *ctx = cg_ctx();
 	if (!ctx) return CG_EINVAL;
+	if (int rc0 = cg_chain_end(ctx, ctx->compute)) return rc0;
 	if (P < 1 || P > CGP_MAX_P) return cg_set_error(CG_EINVAL, "partition count %d out of range", P);
 	if (ncols < 1 || ncols > CGP_MAX_COLS) return cg_set_error(CG_EUNSUPPORTED, "1..%d columns", CGP_MAX_COLS);
 	if (n < 0 || !d_cols || !col_len || !file_offsets) return cg_set_error(CG_EINVAL, "bad argument");

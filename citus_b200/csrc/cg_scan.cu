@@ -258,6 +258,9 @@ static int launch_variant(CgContext *ctx, const KPlan &plan, cudaStream_t stream
 	uint32_t grid = (uint32_t) (ctx->sm_count * occ);
 	if (grid > plan.nselected) grid = plan.nselected;
 	if (grid == 0) return CG_OK;
+	bool overlap;
+	int rc = cg_chain_scan(ctx, stream, false, &overlap);     /* does not trigger its dependents early: ends a chain */
+	if (rc) return rc;
 	cg_scan_kernel<NCC, NAC, MODE, ALL8, U><<<grid, CG_THREADS, 0, stream>>>(plan);
 	CG_CUDA(cudaGetLastError()); g_cg_launches++;
 	return CG_OK;
@@ -329,8 +332,9 @@ cg_rank_kernel(const uint8_t *arena, const DevChunkCol *chunkcols, uint64_t firs
 int cg_launch_rank(CgContext *ctx, const uint8_t *arena, const DevChunkCol *chunkcols, uint64_t first,
 				   uint64_t count, cudaStream_t stream)
 {
-	(void) ctx;
 	if (count == 0) return CG_OK;
+	int rc = cg_chain_end(ctx, stream);
+	if (rc) return rc;
 	uint64_t blocks = (count + 7) / 8;
 	cg_rank_kernel<<<(unsigned) blocks, 256, 0, stream>>>(arena, chunkcols, first, count);
 	CG_CUDA(cudaGetLastError()); g_cg_launches++;
@@ -524,6 +528,8 @@ void cg_realign_set_tma(int on) { g_realign_tma = on ? 1 : 0; }
 int cg_launch_realign(const uint8_t *raw, uint8_t *arena, const RealignItem *items, uint64_t nitems, cudaStream_t stream)
 {
 	if (nitems == 0) return CG_OK;
+	int rc = cg_chain_end(cg_ctx(), stream);
+	if (rc) return rc;
 	if (g_realign_tma < 0) { const char *e = getenv("CG_REALIGN_TMA"); g_realign_tma = e ? (atoi(e) != 0) : 1; }
 	if (g_realign_tma) cg_realign_tma_kernel<<<(unsigned) nitems, RT_THREADS, 0, stream>>>(raw, arena, items);
 	else cg_realign_kernel<<<(unsigned) nitems, 128, 0, stream>>>(raw, arena, items);
@@ -574,6 +580,8 @@ __global__ void cg_table_init_kernel(const __grid_constant__ TableView T)
 
 int cg_launch_table_init(CgPartial *p, cudaStream_t stream)
 {
+	int rc = cg_chain_end(cg_ctx(), stream);
+	if (rc) return rc;
 	TableView v = view_of(p);
 	uint64_t total = v.entries * (uint64_t) v.stride;
 	/* a direct-indexed table whose wide words were never written since the last initialisation (packed words only) is
@@ -666,6 +674,8 @@ __global__ void cg_export_kernel(const __grid_constant__ TableView T, uint64_t o
 int cg_launch_export(CgPartial *p, uint64_t out_capacity, int64_t *d_keys, uint8_t *d_nulls, uint64_t *d_words,
 					 unsigned long long *d_count, cudaStream_t stream)
 {
+	int rc = cg_chain_end(cg_ctx(), stream);
+	if (rc) return rc;
 	TableView v = view_of(p);
 	CG_CUDA(cudaMemsetAsync(d_count, 0, 2 * sizeof(unsigned long long), stream));
 	unsigned blocks = (unsigned) ((v.entries + 255) / 256);
@@ -717,6 +727,8 @@ __global__ void cg_export_packed_kernel(const __grid_constant__ TableView T, con
 int cg_launch_export_packed(CgPartial *p, uint64_t out_capacity, int64_t *d_keys, uint8_t *d_nulls, uint64_t *d_words,
 							unsigned long long *d_count, cudaStream_t stream)
 {
+	int rc = cg_chain_end(cg_ctx(), stream);
+	if (rc) return rc;
 	TableView v = view_of(p);
 	CG_CUDA(cudaMemsetAsync(d_count, 0, 2 * sizeof(unsigned long long), stream));
 	unsigned blocks = (unsigned) ((v.entries + 255) / 256);
@@ -770,6 +782,8 @@ int cg_launch_merge(CgPartial *p, const int64_t *d_keys, const uint8_t *d_nulls,
 					int64_t nrows, cudaStream_t stream)
 {
 	if (nrows <= 0) return CG_OK;
+	int rc = cg_chain_end(cg_ctx(), stream);
+	if (rc) return rc;
 	KPlan plan;
 	memset(&plan, 0, sizeof plan);
 	plan.mode = p->mode; plan.nwords = p->nwords; plan.stride = p->stride; plan.table = p->d_table; plan.hkeys = p->d_hkeys;

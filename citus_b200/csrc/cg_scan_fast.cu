@@ -255,6 +255,8 @@ cg_scan_fast_kernel(const __grid_constant__ FPlan P)
 	constexpr int NCA = NC > 0 ? NC : 1;
 	constexpr int KEYPOS = NQ;
 	constexpr int SUMPOS = NQ + (MODE != CG_MODE_GLOBAL ? 1 : 0);
+	/* the next scan launch of a chain may start as soon as every CTA of this one runs (cg_chain_scan, cg_host.cpp) */
+	asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 	FastAcc<NS> acc;
 	acc.rows = 0;
 #pragma unroll
@@ -404,6 +406,8 @@ cg_drain_kernel(uint64_t *packed, uint64_t *table, uint64_t entries, int stride,
 int cg_launch_drain(CgPartial *p, cudaStream_t stream)
 {
 	if (!p->d_packed || !p->packed_dirty) return CG_OK;
+	int rc = cg_chain_end(cg_ctx(), stream);
+	if (rc) return rc;
 	unsigned blocks = (unsigned) ((p->entries + 255) / 256);
 	if (blocks > (unsigned) cg_ctx()->sm_count * 8) blocks = (unsigned) cg_ctx()->sm_count * 8;
 	cg_drain_kernel<<<blocks, 256, 0, stream>>>(p->d_packed, p->d_table, p->entries, p->stride, p->pack_word, p->pack_shift, p->d_stats);
@@ -435,8 +439,20 @@ static int launch_fast_variant(CgContext *ctx, const FPlan &plan, cudaStream_t s
 	const uint64_t units = (uint64_t) plan.nselected * (uint64_t) launch.slices;
 	if (grid > units) grid = (uint32_t) units;
 	if (grid == 0) return CG_OK;
-	cg_scan_fast_kernel<NQ, MODE, NS, PACK, U><<<grid, CGF_THREADS, 0, stream>>>(launch);
-	CG_CUDA(cudaGetLastError()); g_cg_launches++;
+	bool overlap;
+	int rc = cg_chain_scan(ctx, stream, true, &overlap);
+	if (rc) return rc;
+	cudaLaunchAttribute attr;
+	attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+	attr.val.programmaticStreamSerializationAllowed = 1;
+	cudaLaunchConfig_t cfg = {};
+	cfg.gridDim = dim3(grid);
+	cfg.blockDim = dim3(CGF_THREADS);
+	cfg.stream = stream;
+	cfg.attrs = &attr;
+	cfg.numAttrs = overlap ? 1 : 0;
+	CG_CUDA(cudaLaunchKernelEx(&cfg, cg_scan_fast_kernel<NQ, MODE, NS, PACK, U>, launch));
+	g_cg_launches++;
 	return CG_OK;
 }
 

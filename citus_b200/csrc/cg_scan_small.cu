@@ -172,6 +172,9 @@ static int launch_small_variant(CgContext *ctx, const KPlan &plan, size_t smem, 
 	uint32_t grid = (uint32_t) (ctx->sm_count * occ);
 	if (grid > plan.nselected) grid = plan.nselected;
 	if (grid == 0) return CG_OK;
+	bool overlap;
+	int rc = cg_chain_scan(ctx, stream, false, &overlap);     /* does not trigger its dependents early: ends a chain */
+	if (rc) return rc;
 	cg_scan_small_kernel<NCC, ALL8><<<grid, CGS_THREADS, smem, stream>>>(plan);
 	CG_CUDA(cudaGetLastError()); g_cg_launches++;
 	return CG_OK;

@@ -22,6 +22,7 @@ extern "C" int cg_partial_merge_values(CgPartial *p, int64_t nrows, const int64_
 {
 	CgContext *ctx = cg_ctx();
 	if (!ctx || !p) return CG_EINVAL;
+	if (int rc0 = cg_chain_end(ctx, ctx->compute)) return rc0;
 	if (nrows < 0) return cg_set_error(CG_EINVAL, "negative row count");
 	if (nrows == 0) return CG_OK;
 	const int na = p->desc.naggs, nw = p->nwords;
@@ -172,6 +173,7 @@ extern "C" int cg_agg_column(int32_t attlen, int32_t is_float, const void *value
 {
 	CgContext *ctx = cg_ctx();
 	if (!ctx) return CG_EINVAL;
+	if (int rc0 = cg_chain_end(ctx, ctx->compute)) return rc0;
 	if (n < 0 || (n > 0 && !values)) return cg_set_error(CG_EINVAL, "bad argument");
 	if (attlen != 1 && attlen != 2 && attlen != 4 && attlen != 8) return cg_set_error(CG_EUNSUPPORTED, "attlen %d", attlen);
 	if (is_float && attlen != 4 && attlen != 8) return cg_set_error(CG_EINVAL, "float with attlen %d", attlen);

@@ -131,8 +131,9 @@ cg_varlena_decode_kernel(uint8_t *arena, const VarlenaItem *items, uint64_t nite
 int cg_launch_varlena_decode(CgContext *ctx, uint8_t *arena, const VarlenaItem *items, uint64_t nitems, unsigned long long *err,
 							 unsigned long long flag, cudaStream_t stream)
 {
-	(void) ctx;
 	if (nitems == 0) return CG_OK;
+	int rc = cg_chain_end(ctx, stream);
+	if (rc) return rc;
 	const unsigned blocks = (unsigned) ((nitems + CGV_WARPS - 1) / CGV_WARPS);
 	cg_varlena_decode_kernel<<<blocks, CGV_WARPS * 32, 0, stream>>>(arena, items, nitems, err, flag);
 	CG_CUDA(cudaGetLastError()); g_cg_launches++;

@@ -47,9 +47,14 @@ int cg_synchronize(void);                 /* waits for the library's streams */
  * cudaStreamLegacy).  Lets a host that already has a stream -- e.g. the one its NCCL
  * collectives are ordered on -- keep everything in one queue. */
 int cg_set_stream(void *cuda_stream);
-/* Per-launch device timing of the fused scan kernels: between begin and collect every scan
- * launch is bracketed by CUDA events on the launching stream (no host synchronisation);
- * collect waits for them and returns the launch count and the summed / maximum duration. */
+/* Device timing of the fused scan kernels.  Consecutive scan launches on the library's stream --
+ * the shards of one query -- form a chain whose launches overlap (programmatic dependent launch of
+ * the fast and the generated scan kernels); any other work the library enqueues on that stream
+ * ends the chain.  Between begin and collect, a CUDA event is recorded on the stream before the
+ * first launch of every chain and one where the chain ends (no event between two launches of a
+ * chain, no host synchronisation).  collect ends the open chain, waits for the events and returns
+ * the number of scan kernel launches, the summed busy time of the chains and the longest chain
+ * (ms); total / launches is the average time per launch. */
 int cg_profile_begin(void);
 int cg_profile_collect(int32_t *launches, double *total_ms, double *max_ms);
 /* number of CUDA kernels this library has launched so far (all kernels, all entry points) */
