@@ -21,12 +21,15 @@ CG_TYPE_INT, CG_TYPE_FLOAT = 0, 1
 CG_OP = {"<": 0, "<=": 1, "=": 2, ">=": 3, ">": 4, "<>": 5, "in": 6, "not in": 7, "is null": 8, "is not null": 9}
 CG_AGG_COUNT_STAR, CG_AGG_COUNT, CG_AGG_SUM, CG_AGG_MIN, CG_AGG_MAX = range(5)
 CG_AGG_BIT_AND, CG_AGG_BIT_OR, CG_AGG_BOOL_AND, CG_AGG_BOOL_OR = range(5, 9)
+CG_AGG_VARIANCE = 9
+CG_VAR_POP, CG_VAR_SAMP, CG_STDDEV_POP, CG_STDDEV_SAMP = range(4)
 CG_WORD_ADD, CG_WORD_MIN, CG_WORD_MAX, CG_WORD_FADD, CG_WORD_FMIN, CG_WORD_FMAX = range(6)
 CG_WORD_AND, CG_WORD_OR = 6, 7
 CG_GEN_UNIFORM, CG_GEN_SEQUENCE = 0, 1
 CG_MAX_QUALS, CG_MAX_AGGS, CG_MAX_GROUP_COLS = 8, 8, 4
 CG_MAX_QEXPR, CG_QX_AND, CG_QX_OR = 16, -1, -2
 CG_MAX_FILTER_QUALS = 8
+CG_MAX_WORDS = 32
 CG_MAX_IN_LISTS, CG_MAX_IN_VALUES, CG_IN_REFUTE_MAX = 8, 1024, 100
 
 
@@ -146,6 +149,7 @@ SYMBOLS = [
     ("cg_scan_relation", C.c_int, [C.POINTER(CgRelation), C.POINTER(CgScanDesc), _P, C.POINTER(CgScanStats)]),
     ("cg_partial_ngroups", C.c_int, [_P, C.POINTER(C.c_int64)]),
     ("cg_partial_fetch", C.c_int, [_P, C.c_int64, _P, _P, _P, _P, _P, _P, _P, C.POINTER(C.c_int64)]),
+    ("cg_partial_fetch_ex", C.c_int, [_P, C.c_int64, _P, _P, _P, _P, _P, _P, _P, _P, C.POINTER(C.c_int64)]),
     ("cg_partial_layout", C.c_int, [_P, C.POINTER(C.c_int32), _P, C.POINTER(C.c_int32), C.POINTER(C.c_int64)]),
     ("cg_partial_export_device", C.c_int, [_P, C.c_int64, _P, _P, _P, C.POINTER(C.c_int64)]),
     ("cg_partial_merge_rows", C.c_int, [_P, _P, _P, _P, C.c_int64]),
@@ -162,6 +166,8 @@ SYMBOLS = [
                                          C.POINTER(C.c_int64)]),
     ("cg_numeric_out", C.c_int, [C.c_int64, C.c_uint64, C.c_int32, C.c_char_p, C.c_size_t]),
     ("cg_numeric_div_out", C.c_int, [C.c_int64, C.c_uint64, C.c_int32, C.c_int64, C.c_char_p, C.c_size_t]),
+    ("cg_numeric_var_out", C.c_int, [C.c_int32, C.c_int64, C.c_int64, C.c_uint64, _P, C.c_int32, C.c_char_p, C.c_size_t,
+                                     C.POINTER(C.c_int32)]),
     ("cg_gen_relation", C.c_int, [C.POINTER(CgGenColumn), C.c_int32, C.c_uint64, C.c_uint64, C.c_uint64,
                                   C.c_uint64, C.c_uint32, C.c_int32, C.POINTER(_P)]),
     ("cg_write_relation", C.c_int, [C.POINTER(CgColumnDesc), C.c_int32, _P, _P, C.c_uint64, C.c_uint64,

@@ -239,6 +239,12 @@ def bool_or(tree, filter=None):
     return Agg(capi.CG_AGG_BOOL_OR, filter=filter, arg=tree)
 
 
+def variance(col, filter=None):
+    """the state of var_pop / var_samp / variance / stddev_pop / stddev_samp / stddev over an integer column: fetch()
+    gives N in count, sum(x) in sum and sum(x^2) in sumsq; numeric_var_out() makes the SQL value"""
+    return Agg(capi.CG_AGG_VARIANCE, [(col, 0, 1)], filter=filter)
+
+
 def flatten_where(where):
     """WHERE as a nested tuple tree -- ("and" | "or", arm, arm, ...) over atoms (column, op, constant), (column, "in" |
     "not in", (value, ...)) and (column, "is null" | "is not null"); a plain list of atoms is their AND -- to (atoms, postfix
@@ -515,11 +521,12 @@ class GpuColumnarAgg:
             if not bufs or bufs[0].shape[0] < cap:
                 bufs = (np.zeros(cap, np.int64), np.zeros(cap, np.uint8), np.zeros(cap * na, np.int64),
                         np.zeros(cap * na, np.uint64), np.zeros(cap * na, np.int64), np.zeros(cap * na, np.int64),
-                        np.zeros(cap * na, np.float64))
-            keys, kn, hi, lo, cnt, mm, fs = bufs
+                        np.zeros(cap * na, np.float64), np.zeros(cap * na * 3, np.uint64))
+            keys, kn, hi, lo, cnt, mm, fs, sq = bufs
             got = C.c_int64()
-            rc = lib().cg_partial_fetch(self.h, keys.shape[0], keys.ctypes.data, kn.ctypes.data, hi.ctypes.data, lo.ctypes.data,
-                                        cnt.ctypes.data, mm.ctypes.data, fs.ctypes.data, C.byref(got))
+            rc = lib().cg_partial_fetch_ex(self.h, keys.shape[0], keys.ctypes.data, kn.ctypes.data, hi.ctypes.data,
+                                           lo.ctypes.data, cnt.ctypes.data, mm.ctypes.data, fs.ctypes.data, sq.ctypes.data,
+                                           C.byref(got))
             if rc != 0 and reuse and got.value > keys.shape[0]:      # cached buffers too small for this result: grow once
                 cap, bufs = got.value, None
                 continue
@@ -530,7 +537,8 @@ class GpuColumnarAgg:
         n = got.value
         return dict(n=n, keys=keys[:n], key_nulls=kn[:n], sum_hi=hi[:n * na].reshape(n, na),
                     sum_lo=lo[:n * na].reshape(n, na), count=cnt[:n * na].reshape(n, na),
-                    minmax=mm[:n * na].reshape(n, na), fsum=fs[:n * na].reshape(n, na))
+                    minmax=mm[:n * na].reshape(n, na), fsum=fs[:n * na].reshape(n, na),
+                    sumsq=sq[:n * na * 3].reshape(n, na, 3))
 
     def groups(self):
         """same shape as oracle.Result.groups(): key (None = NULL group) -> per-aggregate dicts.  A composite partial's
@@ -542,8 +550,11 @@ class GpuColumnarAgg:
             per = []
             for a in range(self.naggs):
                 s = (int(f["sum_hi"][i, a]) << 64) + int(f["sum_lo"][i, a])
-                per.append(dict(sum=s, count=int(f["count"][i, a]), minmax=int(f["minmax"][i, a]),
-                                fsum=float(f["fsum"][i, a])))
+                d = dict(sum=s, count=int(f["count"][i, a]), minmax=int(f["minmax"][i, a]), fsum=float(f["fsum"][i, a]))
+                if self.desc.aggs[a].kind == capi.CG_AGG_VARIANCE:
+                    q = f["sumsq"][i, a]
+                    d["sumsq"] = int(q[0]) | (int(q[1]) << 64) | (int(q[2]) << 128)
+                per.append(d)
             if keys is not None:
                 out[keys[i]] = per
             else:
@@ -671,3 +682,13 @@ def partition_scatter(d_index_ptr, n, P, d_col_ptrs, d_out_ptrs, order=None):
         check(lib().cg_partition_scatter_ordered(d_index_ptr, n, P, order.ctypes.data, cols, len(d_col_ptrs), outs,
                                                  offs.ctypes.data))
     return offs
+
+
+def numeric_var_out(final: int, n: int, s: int, q: int, scale: int, buflen: int = 1100):
+    """PostgreSQL's text of var_pop / var_samp / stddev_pop / stddev_samp (final = capi.CG_VAR_* / CG_STDDEV_*) from the
+    exact state N = n, sum(x) = s, sum(x^2) = q in units of 10^-scale; None for SQL NULL"""
+    buf = C.create_string_buffer(buflen)
+    isnull = C.c_int32()
+    qs = np.array([(q >> (64 * i)) & ((1 << 64) - 1) for i in range(3)], np.uint64)
+    check(lib().cg_numeric_var_out(final, n, s >> 64, s & ((1 << 64) - 1), qs.ctypes.data, scale, buf, buflen, C.byref(isnull)))
+    return None if isnull.value else buf.value.decode()

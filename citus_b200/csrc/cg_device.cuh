@@ -452,6 +452,12 @@ __device__ __forceinline__ uint64_t dense_slot_of_packed(const KPlan &P, int64_t
 	return ~0ull;
 }
 
+/* the sum(x^2) callback of the kernels built without CG_AGG_VARIANCE (it is never called) */
+struct NoSquares
+{
+	__device__ __forceinline__ void operator()(int, const KAgg &, uint64_t, uint64_t) const {}
+};
+
 /*
  * K4: the transition terms of a row that passed WHERE and has a group.  For each aggregate a < min(naggs, NA), in
  * order, term(a, g, noinput, w0, w1) is called when the row is no input of a -- an argument is NULL, its FILTER is
@@ -459,9 +465,12 @@ __device__ __forceinline__ uint64_t dense_slot_of_packed(const KPlan &P, int64_t
  * counted -- and otherwise when a has a value word: w0 = that word's operand, w1 = the high limb of a two-limb sum
  * (count(x) is rows - no-input rows).  A term goes to its accumulator before the next one is computed, so that the
  * 64-register general kernel never holds more than one.
+ * VAR: the plan may hold CG_AGG_VARIANCE aggregates.  Their term is sum's (w0, w1 of x), and before it
+ * sq(a, g, lo, hi) receives x^2 = hi:lo (unsigned 128 bits, from |x|).  Without VAR the kind is not compiled in, so the
+ * kernels of the other plans are what they were.
  */
-template <int NCC, int NA, class Term>
-__device__ __forceinline__ void row_terms(const KPlan &P, const int64_t (&v)[NCC], uint32_t nullmask, Term term)
+template <int NCC, int NA, bool VAR = false, class Term, class Sq = NoSquares>
+__device__ __forceinline__ void row_terms(const KPlan &P, const int64_t (&v)[NCC], uint32_t nullmask, Term term, Sq sq = Sq())
 {
 	uint32_t argtrue;
 	const uint32_t rejected = eval_filters<NCC>(P, v, nullmask, &argtrue);
@@ -501,6 +510,14 @@ __device__ __forceinline__ void row_terms(const KPlan &P, const int64_t (&v)[NCC
 				}
 				else { w0 = (uint64_t) (uint32_t) it; w1 = (uint64_t) (it >> 32); }
 			}
+			else if (VAR && g.kind == CG_AGG_VARIANCE)
+			{
+				if (g.bound > 0 && (it > g.bound || it < -g.bound)) atomicOr(P.stats + 2, CG_ERRFLAG_SUM_BOUND);
+				if (g.nlimbs == 1) w0 = (uint64_t) it;
+				else { w0 = (uint64_t) (uint32_t) it; w1 = (uint64_t) (it >> 32); }
+				const uint64_t u = it < 0 ? 0ull - (uint64_t) it : (uint64_t) it;
+				sq(a, g, u * u, __umul64hi(u, u));
+			}
 			else if (g.barg) /* BOOL_AND / BOOL_OR: TRUE = all ones */
 				w0 = ((argtrue >> a) & 1u) ? ~0ull : 0ull;
 			else /* MIN / MAX, BIT_AND / BIT_OR (the sign-extended column value) */
@@ -512,20 +529,55 @@ __device__ __forceinline__ void row_terms(const KPlan &P, const int64_t (&v)[NCC
 
 /* an exact integer sum kept as two words (low 32 bits, high part) */
 __host__ __device__ __forceinline__ bool two_limbs(const KAgg &g) { return g.kind == CG_AGG_SUM && !g.is_float && g.nlimbs == 2; }
+/* the same, for kernels built with VAR: a variance aggregate's sum(x) may be two limbs too */
+template <bool VAR>
+__host__ __device__ __forceinline__ bool two_sum_limbs(const KAgg &g)
+{
+	return VAR ? (cg_kind_sums(g.kind) && !g.is_float && g.nlimbs == 2) : two_limbs(g);
+}
+
+/* the 32-bit limb l of x^2 = hi:lo */
+__device__ __forceinline__ uint64_t square_limb(uint64_t lo, uint64_t hi, int l)
+{
+	const uint64_t w = l < 2 ? lo : hi;
+	return (l & 1) ? (w >> 32) : (w & 0xffffffffull);
+}
+
+/* x^2 = hi:lo into the sum(x^2) words q[0 .. qlimbs) of a table entry (a zero limb adds nothing) */
+__device__ __forceinline__ void squares_apply_global(uint64_t *q, int qlimbs, uint64_t lo, uint64_t hi)
+{
+	if (qlimbs == 1)
+	{
+		if (lo) atomicAdd((unsigned long long *) q, (unsigned long long) lo);
+		return;
+	}
+#pragma unroll
+	for (int l = 0; l < 4; l++)
+		if (l < qlimbs)
+		{
+			const uint64_t x = square_limb(lo, hi, l);
+			if (x) atomicAdd((unsigned long long *) q + l, (unsigned long long) x);
+		}
+}
 
 /* one row into an entry of the global group table (word 0 = rows in the group) */
-template <int NCC, int NA>
+template <int NCC, int NA, bool VAR = false>
 __device__ __forceinline__ void global_accumulate(const KPlan &P, uint64_t *entry, const int64_t (&v)[NCC], uint32_t nullmask)
 {
 	atomicAdd((unsigned long long *) entry, 1ull);
-	row_terms<NCC, NA>(P, v, nullmask, [&](int, const KAgg &g, bool noinput, uint64_t w0, uint64_t w1) {
+	auto term = [&](int, const KAgg &g, bool noinput, uint64_t w0, uint64_t w1) {
 		if (noinput) atomicAdd((unsigned long long *) entry + g.nullword, 1ull);
 		else
 		{
 			word_apply_global(entry + g.word0, P.wordop[g.word0], w0);
-			if (two_limbs(g)) atomicAdd((unsigned long long *) entry + g.word0 + 1, (unsigned long long) w1);
+			if (two_sum_limbs<VAR>(g)) atomicAdd((unsigned long long *) entry + g.word0 + 1, (unsigned long long) w1);
 		}
-	});
+	};
+	if constexpr (VAR)
+		row_terms<NCC, NA, true>(P, v, nullmask, term,
+								 [&](int, const KAgg &g, uint64_t lo, uint64_t hi) { squares_apply_global(entry + g.qword, g.qlimbs, lo, hi); });
+	else
+		row_terms<NCC, NA>(P, v, nullmask, term);
 }
 
 #endif

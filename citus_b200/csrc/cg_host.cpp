@@ -522,7 +522,7 @@ extern "C" int cg_relation_bounds(const CgRelation *rel, const CgScanDesc *desc,
 		{
 			const CgAggSpec &s = desc->aggs[a];
 			term_abs_bound[a] = 0;
-			if (s.kind != CG_AGG_SUM || s.is_float) continue;
+			if (!cg_kind_sums(s.kind) || s.is_float) continue;
 			__int128 bound = 1;
 			bool ok = true;
 			for (int f = 0; f < s.nfactors && ok; f++)
@@ -1819,6 +1819,27 @@ extern "C" int cg_partial_fetch(CgPartial *p, int64_t capacity, int64_t *keys, u
 								int64_t *sum_hi, uint64_t *sum_lo, int64_t *count, int64_t *minmax,
 								double *fsum, int64_t *ngroups)
 {
+	return cg_partial_fetch_ex(p, capacity, keys, key_nulls, sum_hi, sum_lo, count, minmax, fsum, nullptr, ngroups);
+}
+
+/* sum(x^2) of a variance aggregate from its limb words, as a 192-bit little-endian integer */
+static void squares_of_words(const KAgg &k, const uint64_t *w, uint64_t *q)
+{
+	typedef unsigned __int128 u128;
+	const uint64_t *l = w + k.qword;
+	u128 lo = l[0], hi = 0;
+	if (k.qlimbs >= 2) lo += (u128) l[1] << 32;
+	if (k.qlimbs == 4) hi = (u128) l[2] + ((u128) l[3] << 32);
+	const u128 mid = hi + (lo >> 64);
+	q[0] = (uint64_t) lo;
+	q[1] = (uint64_t) mid;
+	q[2] = (uint64_t) (mid >> 64);
+}
+
+extern "C" int cg_partial_fetch_ex(CgPartial *p, int64_t capacity, int64_t *keys, uint8_t *key_nulls,
+								   int64_t *sum_hi, uint64_t *sum_lo, int64_t *count, int64_t *minmax,
+								   double *fsum, uint64_t *sumsq, int64_t *ngroups)
+{
 	CgContext *ctx = cg_ctx();
 	if (!ctx || !p) return CG_EINVAL;
 	if (capacity < 0) return cg_set_error(CG_EINVAL, "negative capacity");
@@ -1852,10 +1873,12 @@ extern "C" int cg_partial_fetch(CgPartial *p, int64_t capacity, int64_t *keys, u
 	CG_CUDA(cudaMemcpyAsync((void *) hw, p->d_out_words, wbytes, cudaMemcpyDeviceToHost, ctx->compute));
 	CG_CUDA(cudaStreamSynchronize(ctx->compute));
 	const int na = p->desc.naggs;
-	/* a two-limb sum's low word grows by < 2^32 per row of the group (scanned, or merged with its carry folded):
-	 * it is exact while the group has fewer than 2^32 rows */
+	/* a two-limb sum's low word, and every limb word of a variance aggregate's sum(x^2) below its top one, grows by
+	 * < 2^32 per row of the group (scanned, or merged with its carry folded): it is exact while the group has fewer than
+	 * 2^32 rows */
 	for (int a = 0; a < na; a++)
-		if (p->aggs[a].kind == CG_AGG_SUM && !p->aggs[a].is_float && p->aggs[a].nlimbs == 2)
+		if ((cg_kind_sums(p->aggs[a].kind) && !p->aggs[a].is_float && p->aggs[a].nlimbs == 2) ||
+			(p->aggs[a].kind == CG_AGG_VARIANCE && p->aggs[a].qlimbs > 1))
 		{
 			for (unsigned long long i = 0; i < n; i++)
 				if (hw[i * p->nwords] >> 32)
@@ -1881,6 +1904,7 @@ extern "C" int cg_partial_fetch(CgPartial *p, int64_t capacity, int64_t *keys, u
 				case CG_AGG_COUNT_STAR: cnt = k.filt ? rows - (int64_t) w[k.nullword] : rows; break;
 				case CG_AGG_COUNT: cnt = rows - (int64_t) w[k.nullword]; break;
 				case CG_AGG_SUM:
+				case CG_AGG_VARIANCE:
 					cnt = rows - (int64_t) w[k.nullword];
 					if (k.is_float) memcpy(&fs, &w[k.word0], 8);
 					else
@@ -1912,6 +1936,12 @@ extern "C" int cg_partial_fetch(CgPartial *p, int64_t capacity, int64_t *keys, u
 			if (count) count[o] = cnt;
 			if (minmax) minmax[o] = mm;
 			if (fsum) fsum[o] = fs;
+			if (sumsq)
+			{
+				uint64_t *q = sumsq + o * 3;
+				if (k.kind == CG_AGG_VARIANCE) squares_of_words(k, w, q);
+				else q[0] = q[1] = q[2] = 0;
+			}
 		}
 	}
 	return CG_OK;

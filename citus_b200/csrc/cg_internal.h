@@ -158,7 +158,7 @@ struct CgShard
  *  Kernel plan (passed by value as a __grid_constant__ parameter).
  * ------------------------------------------------------------------------------ */
 #define CG_KMAX_COLS 8
-#define CG_KMAX_WORDS 32
+#define CG_KMAX_WORDS CG_MAX_WORDS
 
 enum { CG_MODE_GLOBAL = 0, CG_MODE_DENSE = 1, CG_MODE_HASH = 2 };
 
@@ -180,9 +180,15 @@ struct KAgg
 						 * filter not TRUE); count(*) then gets a nullword of its own (count = rows - it) */
 	int8_t barg;        /* bool_and / bool_or: the argument is the predicate tree argexpr[a] over the filter pool;
 						 * nullword counts the rows that gave no input (argument UNKNOWN, or FILTER not TRUE) */
+	/* CG_AGG_VARIANCE: word0 (and nlimbs, bound) hold sum(x) as a sum's words do; sum(x^2) is qlimbs words from qword on:
+	 * 1 = the whole sum, 2 = (x^2 low 32 bits, x^2 >> 32), 4 = the four 32-bit limbs of the unsigned 128-bit x^2.  0 for
+	 * the other kinds.  These two bytes sit in what was padding before a[], so no offset moves (the generated kernels of
+	 * plans without the kind restate the struct without them, cg_jit.cpp) */
+	int8_t qlimbs;
+	int8_t qword;
 	int64_t a[3];
 	int64_t b[3];
-	int64_t bound;      /* nlimbs == 1: every |term| must be <= bound */
+	int64_t bound;      /* nlimbs == 1 (and CG_AGG_VARIANCE with a term bound): every |term| must be <= bound */
 	int64_t tbound;     /* integer SUM: the caller-proven bound on |term| whatever nlimbs is (0 = unknown) */
 };
 
@@ -315,6 +321,14 @@ static inline bool cg_desc_uses_pool(const CgScanDesc *d)
 
 static inline bool cg_kind_is_bool(int kind) { return kind == CG_AGG_BOOL_AND || kind == CG_AGG_BOOL_OR; }
 static inline bool cg_kind_is_bit(int kind) { return kind == CG_AGG_BIT_AND || kind == CG_AGG_BIT_OR; }
+/* an integer aggregate whose sum(x) words follow sum's form (word0, nlimbs, bound) */
+static inline __host__ __device__ bool cg_kind_sums(int kind) { return kind == CG_AGG_SUM || kind == CG_AGG_VARIANCE; }
+static inline __host__ __device__ bool cg_plan_has_variance(const KAgg *aggs, int naggs)
+{
+	for (int a = 0; a < naggs; a++)
+		if (aggs[a].kind == CG_AGG_VARIANCE) return true;
+	return false;
+}
 
 /* plan of the specialised kernel (cg_scan_fast.cu): column roles in fixed order
  * [range quals..., group key, summed columns...] */

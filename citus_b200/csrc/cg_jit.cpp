@@ -141,6 +141,7 @@ struct JitShape
 	int64_t bias[CG_MAX_AGGS];
 	int rows_partner = -1;            /* aggregate in the high half of cell 0 (whose low half counts the rows), -1 = none */
 	int ncell[CG_MAX_AGGS];           /* SMALL: cell of a filtered aggregate's no-input counter, -1 = none */
+	int qcell[CG_MAX_AGGS];           /* SMALL: first of the qlimbs cells of a variance aggregate's sum(x^2), -1 = none */
 	long long lane_rows_cap = (1ll << 22);
 	int min_blocks = 0;               /* __launch_bounds__ second argument, 0 = none */
 	size_t smem = 0;
@@ -161,7 +162,17 @@ static void addf(std::string &s, const char *fmt, ...)
 }
 
 static bool agg_has_value(const KAgg &g) { return g.kind != CG_AGG_COUNT_STAR && g.kind != CG_AGG_COUNT; }
-static bool agg_two_limbs(const KAgg &g) { return g.kind == CG_AGG_SUM && !g.is_float && g.nlimbs == 2; }
+static bool agg_two_limbs(const KAgg &g) { return (g.kind == CG_AGG_SUM || g.kind == CG_AGG_VARIANCE) && !g.is_float && g.nlimbs == 2; }
+static bool agg_is_var(const KAgg &g) { return g.kind == CG_AGG_VARIANCE; }
+
+/* sum(x^2) limb l of a variance aggregate a as an expression over x^2 = qh<a>:ql<a> */
+static std::string square_limb_expr(int a, int qlimbs, int l)
+{
+	char b[96];
+	if (qlimbs == 1) snprintf(b, sizeof b, "ql%d", a);
+	else snprintf(b, sizeof b, "(q%c%d %s)", l < 2 ? 'l' : 'h', a, (l & 1) ? ">> 32" : "& 0xffffffffull");
+	return b;
+}
 
 static std::string agg_null_expr(const KAgg &g, const JitShape &sh);
 static std::string agg_noinput_expr(const KPlan &plan, int a, const JitShape &sh);
@@ -179,7 +190,10 @@ static void choose_shape(const KPlan &plan, uint32_t nullable, JitShape *sh)
 		if (r && (atoi(r) == 2 || atoi(r) == 4)) sh->R = atoi(r);
 		if (u && atoi(u) >= 1 && atoi(u) <= 4) sh->U = atoi(u);
 	}
-	for (int a = 0; a < CG_MAX_AGGS; a++) { sh->hot0[a] = -1; sh->lane1[a] = false; sh->half[a] = -1; sh->bias[a] = 0; sh->ncell[a] = -1; }
+	for (int a = 0; a < CG_MAX_AGGS; a++)
+	{
+		sh->hot0[a] = -1; sh->lane1[a] = false; sh->half[a] = -1; sh->bias[a] = 0; sh->ncell[a] = -1; sh->qcell[a] = -1;
+	}
 	if (plan.mode == CG_MODE_DENSE)
 	{
 		static int narrow_on = -1;
@@ -215,7 +229,7 @@ static void choose_shape(const KPlan &plan, uint32_t nullable, JitShape *sh)
 			const KAgg &g = plan.aggs[a];
 			if (!agg_has_value(g) || taken[a]) continue;
 			sh->hot0[a] = nhot;
-			if (g.kind == CG_AGG_SUM && !g.is_float)
+			if ((g.kind == CG_AGG_SUM || agg_is_var(g)) && !g.is_float)
 			{
 				/* one cell if the lane's running sum cannot overflow: the table's own single-word
 				 * guarantee, or the caller's term bound times the per-lane row cap */
@@ -226,6 +240,9 @@ static void choose_shape(const KPlan &plan, uint32_t nullable, JitShape *sh)
 			}
 			else
 				nhot += 1;
+			/* sum(x^2): a cell per limb word (a lane's limb grows by < 2^32 per row; the one-word form is bounded by the table's
+			 * own guarantee) */
+			if (agg_is_var(g)) { sh->qcell[a] = nhot; nhot += g.qlimbs; }
 		}
 		/* rejected rows are common, not rare like NULL inputs: a filtered aggregate's no-input counter gets a cell too, and
 		 * so does the counter of a bool_and / bool_or, whose UNKNOWN rows are as common as its atoms' NULLs */
@@ -345,8 +362,10 @@ static void gen_prelude(std::string &s, const KPlan &plan)
 		"typedef unsigned short uint16_t; typedef short int16_t; typedef unsigned char uint8_t; typedef signed char int8_t;\n"
 		"struct DevChunkCol { uint64_t values_off; uint64_t exists_off; uint64_t rank_off; uint32_t value_count; uint32_t row_count; };\n";
 	if (sets) s += "struct KSet { uint16_t off; uint16_t len; uint8_t steps; uint8_t nnull; uint8_t pad[2]; };\n";
-	s += args ? "struct KAgg { int8_t kind; int8_t nfactors; int8_t is_float; int8_t nlimbs; int8_t pcol[3]; int8_t word0; int8_t nullword; int8_t ovchk; int8_t filt; int8_t barg;\n"
-			  : "struct KAgg { int8_t kind; int8_t nfactors; int8_t is_float; int8_t nlimbs; int8_t pcol[3]; int8_t word0; int8_t nullword; int8_t ovchk; int8_t filt; int8_t pad;\n";
+	s += args ? "struct KAgg { int8_t kind; int8_t nfactors; int8_t is_float; int8_t nlimbs; int8_t pcol[3]; int8_t word0; int8_t nullword; int8_t ovchk; int8_t filt; int8_t barg;"
+			  : "struct KAgg { int8_t kind; int8_t nfactors; int8_t is_float; int8_t nlimbs; int8_t pcol[3]; int8_t word0; int8_t nullword; int8_t ovchk; int8_t filt; int8_t pad;";
+	/* the sum(x^2) fields sit in KAgg's padding: plans without a variance aggregate restate the struct without them */
+	s += cg_plan_has_variance(plan.aggs, plan.naggs) ? " int8_t qlimbs; int8_t qword;\n" : "\n";
 	s += "  int64_t a[3]; int64_t b[3]; int64_t bound; int64_t tbound; };\n";
 	addf(s,
 		 "struct KPlan { const uint8_t *arena; const DevChunkCol *chunkcols; const uint32_t *selected; uint32_t nselected; int32_t nstaged;\n"
@@ -638,6 +657,15 @@ static void gen_table_updates(std::string &s, const KPlan &plan, const JitShape 
 		if ((g.kind == CG_AGG_COUNT_STAR && an[a].empty()) || (with_packed && a == sh.pack_agg)) continue;
 		if (!an[a].empty()) addf(s, "%sif (an%d) red_add(e + %d, 1ull);\n", C, a, g.nullword);
 		if (!agg_has_value(g)) continue;
+		if (agg_is_var(g))
+		{
+			/* sum(x^2): one reduction per limb, none for a zero limb above the first */
+			std::string q = an[a].empty() ? "{" : ("if (!an" + std::to_string(a) + ") {");
+			for (int l = 0; l < g.qlimbs; l++)
+				q += (l ? " if (" + square_limb_expr(a, g.qlimbs, l) + ") " : std::string(" ")) + "red_add(e + " + std::to_string(g.qword + l) +
+					 ", " + square_limb_expr(a, g.qlimbs, l) + ");";
+			addf(s, "%s%s }\n", C, q.c_str());
+		}
 		char p[32];
 		snprintf(p, sizeof p, "e + %d", g.word0);
 		std::string guard = an[a].empty() ? "" : ("if (!an" + std::to_string(a) + ") ");
@@ -824,13 +852,18 @@ static void gen_row(std::string &s, const KPlan &plan, const JitShape &sh, int u
 			if (g.ovchk)
 				addf(s, "%sif (%sov%d) raise_flag(P.stats, %lluull);\n", C, an[a].empty() ? "" : ("!an" + std::to_string(a) + " && ").c_str(),
 					 a, (unsigned long long) CG_ERRFLAG_TERM_OVERFLOW);
-			if (g.kind == CG_AGG_SUM && g.nlimbs == 1)
+			if ((g.kind == CG_AGG_SUM && g.nlimbs == 1) || (agg_is_var(g) && g.bound > 0))
 				addf(s, "%sif (%s(it%d > P.aggs[%d].bound || it%d < -P.aggs[%d].bound)) raise_flag(P.stats, %lluull);\n", C,
 					 an[a].empty() ? "" : ("!an" + std::to_string(a) + " && ").c_str(), a, a, a, a, (unsigned long long) CG_ERRFLAG_SUM_BOUND);
+			if (agg_is_var(g))
+				/* x^2 = qh:ql from |x| (x = INT64_MIN gives 2^126) */
+				addf(s, "%sconst uint64_t qa%d = it%d < 0 ? 0ull - (uint64_t) it%d : (uint64_t) it%d;\n"
+						"%sconst uint64_t ql%d = qa%d * qa%d, qh%d = __umul64hi(qa%d, qa%d);\n",
+					 C, a, a, a, a, C, a, a, a, a, a, a);
 		}
 		/* the word-0 value the aggregate contributes */
 		char buf[128];
-		if (g.kind == CG_AGG_SUM)
+		if (g.kind == CG_AGG_SUM || agg_is_var(g))
 		{
 			if (g.is_float) snprintf(buf, sizeof buf, "(uint64_t) __double_as_longlong(ft%d)", a);
 			else if (g.nlimbs == 1) snprintf(buf, sizeof buf, "(uint64_t) it%d", a);
@@ -856,6 +889,12 @@ static void gen_row(std::string &s, const KPlan &plan, const JitShape &sh, int u
 					 op_combine(plan.wordop[g.word0], acc, w0v[a]).c_str(), a, a);
 			else
 				addf(s, "%s%s%s = %s;\n", C, guard.c_str(), acc, op_combine(plan.wordop[g.word0], acc, w0v[a]).c_str());
+			if (agg_is_var(g))
+			{
+				std::string q = guard + "{";
+				for (int l = 0; l < g.qlimbs; l++) q += " g_q" + std::to_string(a) + "_" + std::to_string(l) + " += " + square_limb_expr(a, g.qlimbs, l) + ";";
+				addf(s, "%s%s }\n", C, q.c_str());
+			}
 		}
 	}
 	else if (sh.kind == JK_SMALL)
@@ -901,7 +940,7 @@ static void gen_row(std::string &s, const KPlan &plan, const JitShape &sh, int u
 			char cell[48];
 			snprintf(cell, sizeof cell, "e[%d]", sh.hot0[a] * JIT_THREADS);
 			std::string guard = an[a].empty() ? "" : ("if (!an" + std::to_string(a) + ") ");
-			if (g.kind == CG_AGG_SUM && !g.is_float)
+			if ((g.kind == CG_AGG_SUM || agg_is_var(g)) && !g.is_float)
 			{
 				if (sh.lane1[a]) addf(s, "%s%s%s += (uint64_t) it%d;\n", D, guard.c_str(), cell, a);
 				else
@@ -910,6 +949,13 @@ static void gen_row(std::string &s, const KPlan &plan, const JitShape &sh, int u
 			}
 			else
 				addf(s, "%s%s%s = %s;\n", D, guard.c_str(), cell, op_combine(plan.wordop[g.word0], cell, w0v[a]).c_str());
+			if (agg_is_var(g))
+			{
+				std::string q = guard + "{";
+				for (int l = 0; l < g.qlimbs; l++)
+					q += " e[" + std::to_string((sh.qcell[a] + l) * JIT_THREADS) + "] += " + square_limb_expr(a, g.qlimbs, l) + ";";
+				addf(s, "%s%s }\n", D, q.c_str());
+			}
 		}
 		for (int k = 0; k < sh.nhot; k++)
 			if (!cellexpr[k].empty()) addf(s, "%se[%d] += %s;\n", D, k * JIT_THREADS, cellexpr[k].c_str());
@@ -943,6 +989,7 @@ static std::string gen_source(const KPlan &plan, const JitShape &sh)
 			if (!agg_noinput_expr(plan, a, sh).empty()) addf(s, "\tuint64_t g_n%d = 0;\n", a);
 			if (!agg_has_value(g)) continue;
 			addf(s, "\tuint64_t g_a%d_0 = %s, g_a%d_1 = 0;\n", a, op_identity(plan.wordop[g.word0]), a);
+			for (int l = 0; agg_is_var(g) && l < g.qlimbs; l++) addf(s, "\tuint64_t g_q%d_%d = 0;\n", a, l);
 		}
 	if (sh.kind == JK_SMALL || sh.nullable)
 		s += "\textern __shared__ uint64_t s_acc[];\n";
@@ -1074,6 +1121,8 @@ static std::string gen_source(const KPlan &plan, const JitShape &sh)
 			addf(s, "\t  if ((tid & 31) == 0 && x != %s) { %s }\n", op_identity(op), op_apply_global(op, p, "x").c_str());
 			if (agg_two_limbs(g))
 				addf(s, "\t  uint64_t x1 = wsum(g_a%d_1); if ((tid & 31) == 0 && x1) red_add(P.table + %d, x1);\n", a, g.word0 + 1);
+			for (int l = 0; agg_is_var(g) && l < g.qlimbs; l++)
+				addf(s, "\t  { uint64_t q = wsum(g_q%d_%d); if ((tid & 31) == 0 && q) red_add(P.table + %d, q); }\n", a, l, g.qword + l);
 			s += "\t}\n";
 		}
 	}
@@ -1124,7 +1173,10 @@ static std::string gen_source(const KPlan &plan, const JitShape &sh)
 			int op = plan.wordop[g.word0];
 			char p[32];
 			snprintf(p, sizeof p, "ge + %d", g.word0);
-			if (g.kind == CG_AGG_SUM && !g.is_float)
+			for (int l = 0; agg_is_var(g) && l < g.qlimbs; l++)
+				addf(s, "\t\t\tcase %d: { uint64_t x = 0; for (uint32_t k = 0; k < %d; k++) x += col[(k + tid) %% %d]; if (x) red_add(ge + %d, x); break; }\n",
+					 sh.qcell[a] + l, JIT_THREADS, JIT_THREADS, g.qword + l);
+			if ((g.kind == CG_AGG_SUM || agg_is_var(g)) && !g.is_float)
 			{
 				if (sh.lane1[a] && g.nlimbs == 2)
 					/* exact 64-bit lane sums -> the table's (low 32 unsigned, high signed) limbs */

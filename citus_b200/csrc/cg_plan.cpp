@@ -150,9 +150,24 @@ static int validate_desc(const CgScanDesc *d, const CgColumnDesc *columns, int n
 	for (int a = 0; a < d->naggs; a++)
 	{
 		const CgAggSpec &s = d->aggs[a];
-		if (s.kind < CG_AGG_COUNT_STAR || s.kind > CG_AGG_BOOL_OR) return cg_set_error(CG_EINVAL, "aggregate %d: bad kind", a);
+		if (s.kind < CG_AGG_COUNT_STAR || s.kind > CG_AGG_VARIANCE) return cg_set_error(CG_EINVAL, "aggregate %d: bad kind", a);
 		if (s.nfactors < 0 || s.nfactors > 3) return cg_set_error(CG_EINVAL, "aggregate %d: nfactors", a);
-		if (s.kind > CG_AGG_MAX && s.term_abs_bound != 0) return cg_set_error(CG_EINVAL, "aggregate %d: term_abs_bound on bit / bool kind", a);
+		if (s.kind > CG_AGG_MAX && s.kind != CG_AGG_VARIANCE && s.term_abs_bound != 0)
+			return cg_set_error(CG_EINVAL, "aggregate %d: term_abs_bound on bit / bool kind", a);
+		if (s.kind == CG_AGG_VARIANCE)
+		{
+			/* the exact integer state of numeric_stddev_internal: a float argument has no such state */
+			if (s.nfactors < 1) return cg_set_error(CG_EINVAL, "aggregate %d needs an argument", a);
+			for (int f = 0; f < s.nfactors; f++)
+			{
+				if (s.column[f] < 0 || s.column[f] >= natts) return cg_set_error(CG_EINVAL, "aggregate %d: column out of range", a);
+				if (cg_type_class(columns[s.column[f]]) == CG_TYPE_BPCHAR1)
+					return cg_set_error(CG_EINVAL, "aggregate %d: variance over a char(1) column", a);
+				if (s.is_float || cg_type_class(columns[s.column[f]]) == CG_TYPE_FLOAT)
+					return cg_set_error(CG_EUNSUPPORTED, "aggregate %d: variance / stddev of a float argument", a);
+			}
+			continue;
+		}
 		if (cg_kind_is_bool(s.kind))
 		{
 			/* the argument is a predicate tree, not factors */
@@ -284,6 +299,12 @@ extern "C" int cg_group_key_decode(const CgScanDesc *desc, int64_t n, const int6
  *   bit_and/or    1 AND/OR word (identity ~0 / 0) over the sign-extended values + NULL-input count
  *   bool_and/or   1 AND/OR word whose bit 0 is the result (a TRUE input contributes ~0, a FALSE one 0, so TRUE is the
  *                 identity of bool_and and FALSE that of bool_or) + a count of the rows that gave no input (UNKNOWN)
+ *   variance      sum(x) in sum's one-word or two-limb form under sum's rule; then sum(x^2) in ADD words:
+ *                   1 word    when B^2 * max_rows < 2^63 (B = term_abs_bound)
+ *                   2 limbs   (x^2 low 32 bits, x^2 >> 32) when B < 2^32
+ *                   4 limbs   the four 32-bit limbs of the unsigned 128-bit x^2 (x = INT64_MIN gives 2^126)
+ *                 + NULL-input count: 3 to 7 words.  Every limb word grows by < 2^32 per row (the merge kernel's carry
+ *                 chain keeps it so for merged rows: limb l's carry goes to limb l + 1)
  * Counting the NULL inputs instead of the non-NULL ones keeps NULL-free data (the common
  * case) at one atomic per aggregate and row, while "no non-NULL input => SQL NULL" and
  * count(x) stay exact: non-NULL inputs = rows in group - NULL inputs.
@@ -296,6 +317,11 @@ static int layout_partial(CgPartial *p, const CgColumnDesc *columns)
 	const CgScanDesc &d = p->desc;
 	int nw = 1;
 	memset(p->wordop, CG_WORD_ADD, sizeof p->wordop);
+	/* appends one word; past CG_KMAX_WORDS it only counts (the aggregate list is refused below, nothing is written) */
+	auto push = [&](int op) {
+		if (nw < CG_KMAX_WORDS) p->wordop[nw] = (uint8_t) op;
+		nw++;
+	};
 	for (int a = 0; a < d.naggs; a++)
 	{
 		const CgAggSpec &s = d.aggs[a];
@@ -306,10 +332,10 @@ static int layout_partial(CgPartial *p, const CgColumnDesc *columns)
 		k.is_float = (int8_t) (s.is_float != 0);
 		for (int f = 0; f < 3; f++) { k.a[f] = s.a[f]; k.b[f] = s.b[f]; }
 		k.nlimbs = 1;
-		k.tbound = (s.kind == CG_AGG_SUM && !s.is_float && s.term_abs_bound > 0) ? s.term_abs_bound : 0;
+		k.tbound = (cg_kind_sums(s.kind) && !s.is_float && s.term_abs_bound > 0) ? s.term_abs_bound : 0;
 		/* an integer argument other than a bare column can leave int64 ([PG] int8mul / int8pl raise "bigint out of
 		 * range", numeric is exact): unless the caller proved a bound, the kernels check every factor and product */
-		k.ovchk = (int8_t) (!s.is_float && (s.kind == CG_AGG_SUM || s.kind == CG_AGG_MIN || s.kind == CG_AGG_MAX) &&
+		k.ovchk = (int8_t) (!s.is_float && (cg_kind_sums(s.kind) || s.kind == CG_AGG_MIN || s.kind == CG_AGG_MAX) &&
 							k.tbound == 0 && !(s.nfactors == 1 && s.a[0] == 0 && s.b[0] == 1));
 		k.filt = (int8_t) (d.nfilter_expr[a] > 0);
 		k.barg = (int8_t) cg_kind_is_bool(s.kind);
@@ -320,22 +346,39 @@ static int layout_partial(CgPartial *p, const CgColumnDesc *columns)
 			case CG_AGG_BOOL_AND:
 			case CG_AGG_BOOL_OR:
 				k.word0 = (int8_t) nw;
-				p->wordop[nw++] = (s.kind == CG_AGG_BIT_AND || s.kind == CG_AGG_BOOL_AND) ? CG_WORD_AND : CG_WORD_OR;
-				k.nullword = (int8_t) nw; p->wordop[nw++] = CG_WORD_ADD;
+				push((s.kind == CG_AGG_BIT_AND || s.kind == CG_AGG_BOOL_AND) ? CG_WORD_AND : CG_WORD_OR);
+				k.nullword = (int8_t) nw; push(CG_WORD_ADD);
 				break;
 			case CG_AGG_COUNT_STAR:
 				k.word0 = 0;
-				if (k.filt) { k.nullword = (int8_t) nw; p->wordop[nw++] = CG_WORD_ADD; }
+				if (k.filt) { k.nullword = (int8_t) nw; push(CG_WORD_ADD); }
 				break;
 			case CG_AGG_COUNT:
-				k.word0 = (int8_t) nw; k.nullword = (int8_t) nw; p->wordop[nw++] = CG_WORD_ADD;
+				k.word0 = (int8_t) nw; k.nullword = (int8_t) nw; push(CG_WORD_ADD);
 				break;
+			case CG_AGG_VARIANCE:
+			{
+				/* sum(x): sum's words under sum's rule */
+				k.word0 = (int8_t) nw;
+				push(CG_WORD_ADD);
+				const __int128 B = s.term_abs_bound, R = p->max_rows;
+				if (B > 0 && R > 0 && B * R < ((__int128) 1 << 63)) { k.nlimbs = 1; k.bound = s.term_abs_bound; }
+				else { k.nlimbs = 2; push(CG_WORD_ADD); if (B > 0) k.bound = s.term_abs_bound; }
+				/* sum(x^2): every limb word grows by < 2^32 per row, so 2^32 rows per group never wrap one */
+				k.qword = (int8_t) nw;
+				if (B > 0 && R > 0 && B < ((__int128) 1 << 32) && (B * B) * R < ((__int128) 1 << 63)) k.qlimbs = 1;
+				else if (B > 0 && B < ((__int128) 1 << 32)) k.qlimbs = 2;
+				else k.qlimbs = 4;
+				for (int l = 0; l < k.qlimbs; l++) push(CG_WORD_ADD);
+				k.nullword = (int8_t) nw; push(CG_WORD_ADD);
+				break;
+			}
 			case CG_AGG_SUM:
 				k.word0 = (int8_t) nw;
-				if (s.is_float) p->wordop[nw++] = CG_WORD_FADD;
+				if (s.is_float) push(CG_WORD_FADD);
 				else
 				{
-					p->wordop[nw++] = CG_WORD_ADD;
+					push(CG_WORD_ADD);
 					bool one = false;
 					if (s.term_abs_bound > 0 && p->max_rows > 0)
 					{
@@ -343,15 +386,15 @@ static int layout_partial(CgPartial *p, const CgColumnDesc *columns)
 						one = worst < ((__int128) 1 << 63);
 					}
 					if (one) { k.nlimbs = 1; k.bound = s.term_abs_bound; }
-					else { k.nlimbs = 2; p->wordop[nw++] = CG_WORD_ADD; }
+					else { k.nlimbs = 2; push(CG_WORD_ADD); }
 				}
-				k.nullword = (int8_t) nw; p->wordop[nw++] = CG_WORD_ADD;
+				k.nullword = (int8_t) nw; push(CG_WORD_ADD);
 				break;
 			default:
 				k.word0 = (int8_t) nw;
-				if (s.kind == CG_AGG_MIN) p->wordop[nw++] = s.is_float ? CG_WORD_FMIN : CG_WORD_MIN;
-				else p->wordop[nw++] = s.is_float ? CG_WORD_FMAX : CG_WORD_MAX;
-				k.nullword = (int8_t) nw; p->wordop[nw++] = CG_WORD_ADD;
+				if (s.kind == CG_AGG_MIN) push(s.is_float ? CG_WORD_FMIN : CG_WORD_MIN);
+				else push(s.is_float ? CG_WORD_FMAX : CG_WORD_MAX);
+				k.nullword = (int8_t) nw; push(CG_WORD_ADD);
 				break;
 		}
 		if (nw > CG_KMAX_WORDS) return cg_set_error(CG_EUNSUPPORTED, "too many accumulator words (%d)", nw);

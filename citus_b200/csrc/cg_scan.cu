@@ -67,16 +67,17 @@ __device__ __forceinline__ uint64_t *find_entry(const KPlan &P, int64_t key, boo
 }
 
 /* per-thread accumulators of the plain-aggregate mode */
-template <int NAC>
+template <int NAC, bool VAR>
 struct ThreadAcc
 {
 	uint64_t w[NAC][3];     /* [agg][word0, word0+1, NULL-input count] */
 	uint64_t rows;
+	uint64_t q[NAC][VAR ? 4 : 1];   /* VAR: [agg][sum(x^2) word qword + l] */
 };
 
-template <int NCC, int NAC, int MODE>
+template <int NCC, int NAC, int MODE, bool VAR>
 __device__ __forceinline__ void process_row(const KPlan &P, const int64_t (&v)[NCC], uint32_t nullmask,
-											ThreadAcc<NAC> &acc, uint32_t &removed)
+											ThreadAcc<NAC, VAR> &acc, uint32_t &removed)
 {
 	/* K3: WHERE tree, three-valued: an atom on a NULL input is not TRUE */
 	if (!eval_where<NCC>(P, v, nullmask))
@@ -90,18 +91,31 @@ __device__ __forceinline__ void process_row(const KPlan &P, const int64_t (&v)[N
 		bool key_null;
 		if (!group_key<NCC>(P, v, nullmask, key, key_null)) return;
 		uint64_t *entry = find_entry<MODE>(P, key, key_null);
-		if (entry != nullptr) global_accumulate<NCC, NAC>(P, entry, v, nullmask);
+		if (entry != nullptr) global_accumulate<NCC, NAC, VAR>(P, entry, v, nullmask);
 		return;
 	}
 	acc.rows++;
-	row_terms<NCC, NAC>(P, v, nullmask, [&](int a, const KAgg &g, bool noinput, uint64_t w0, uint64_t w1) {
+	auto term = [&](int a, const KAgg &g, bool noinput, uint64_t w0, uint64_t w1) {
 		if (noinput) acc.w[a][2]++;
 		else
 		{
 			acc.w[a][0] = word_combine(P.wordop[g.word0], acc.w[a][0], w0);
-			if (two_limbs(g)) acc.w[a][1] += w1;
+			if (two_sum_limbs<VAR>(g)) acc.w[a][1] += w1;
 		}
-	});
+	};
+	if constexpr (VAR)
+		row_terms<NCC, NAC, true>(P, v, nullmask, term, [&](int a, const KAgg &g, uint64_t lo, uint64_t hi) {
+			/* a thread's limb sums grow by < 2^32 per row; the one-word form is bounded by the table's own guarantee */
+			if (g.qlimbs == 1) acc.q[a][0] += lo;
+			else
+			{
+#pragma unroll
+				for (int l = 0; l < 4; l++)
+					if (l < g.qlimbs) acc.q[a][l] += square_limb(lo, hi, l);
+			}
+		});
+	else
+		row_terms<NCC, NAC>(P, v, nullmask, term);
 }
 
 /*
@@ -112,11 +126,11 @@ __device__ __forceinline__ void process_row(const KPlan &P, const int64_t (&v)[N
  *   NAC  capacity of the per-thread aggregate accumulators (plain aggregate mode)
  *   ALL8 every plan column is 8 bytes wide (skips the width switch)
  */
-template <int NCC, int NAC, int MODE, bool ALL8, int U>
+template <int NCC, int NAC, int MODE, bool ALL8, int U, bool VAR = false>
 __global__ void __launch_bounds__(CG_THREADS, 4)
 cg_scan_kernel(const __grid_constant__ KPlan P)
 {
-	ThreadAcc<NAC> acc;
+	ThreadAcc<NAC, VAR> acc;
 	acc.rows = 0;
 #pragma unroll
 	for (int a = 0; a < NAC; a++)
@@ -124,6 +138,11 @@ cg_scan_kernel(const __grid_constant__ KPlan P)
 		acc.w[a][0] = (a < P.naggs && P.aggs[a].kind != CG_AGG_COUNT_STAR) ? word_identity(P.wordop[P.aggs[a].word0]) : 0;
 		acc.w[a][1] = 0;
 		acc.w[a][2] = 0;
+		if constexpr (VAR)
+		{
+#pragma unroll
+			for (int l = 0; l < 4; l++) acc.q[a][l] = 0;
+		}
 	}
 	uint32_t removed = 0;
 	unsigned long long scanned = 0;
@@ -183,8 +202,8 @@ cg_scan_kernel(const __grid_constant__ KPlan P)
 					uint32_t r = base + (u * CG_THREADS + tid) * 2;
 					if (r < rows)
 					{
-						process_row<NCC, NAC, MODE>(P, v0[u], 0u, acc, removed);
-						if (r + 1 < rows) process_row<NCC, NAC, MODE>(P, v1[u], 0u, acc, removed);
+						process_row<NCC, NAC, MODE, VAR>(P, v0[u], 0u, acc, removed);
+						if (r + 1 < rows) process_row<NCC, NAC, MODE, VAR>(P, v1[u], 0u, acc, removed);
 					}
 				}
 			}
@@ -206,8 +225,8 @@ cg_scan_kernel(const __grid_constant__ KPlan P)
 						else
 							load_pair(vptr[c], r, len, P.isfloat[c], v0[c], v1[c]);
 					}
-				process_row<NCC, NAC, MODE>(P, v0, n0, acc, removed);
-				if (r + 1 < rows) process_row<NCC, NAC, MODE>(P, v1, n1, acc, removed);
+				process_row<NCC, NAC, MODE, VAR>(P, v0, n0, acc, removed);
+				if (r + 1 < rows) process_row<NCC, NAC, MODE, VAR>(P, v1, n1, acc, removed);
 			}
 		}
 	}
@@ -240,8 +259,20 @@ cg_scan_kernel(const __grid_constant__ KPlan P)
 					if (g.kind != CG_AGG_COUNT && g.kind != CG_AGG_COUNT_STAR)
 					{
 						if (x0 != word_identity(P.wordop[g.word0])) word_apply_global(P.table + g.word0, P.wordop[g.word0], x0);
-						if (two_limbs(g) && x1)
+						if (two_sum_limbs<VAR>(g) && x1)
 							atomicAdd((unsigned long long *) P.table + g.word0 + 1, (unsigned long long) x1);
+					}
+				}
+				if constexpr (VAR)
+				{
+					if (g.kind == CG_AGG_VARIANCE)
+					{
+#pragma unroll
+						for (int l = 0; l < 4; l++)
+						{
+							const uint64_t x = warp_reduce_word(acc.q[a][l], CG_WORD_ADD);
+							if ((tid & 31) == 0 && l < g.qlimbs && x) atomicAdd((unsigned long long *) P.table + g.qword + l, (unsigned long long) x);
+						}
 					}
 				}
 			}
@@ -249,11 +280,11 @@ cg_scan_kernel(const __grid_constant__ KPlan P)
 	}
 }
 
-template <int NCC, int NAC, int MODE, bool ALL8, int U>
+template <int NCC, int NAC, int MODE, bool ALL8, int U, bool VAR = false>
 static int launch_variant(CgContext *ctx, const KPlan &plan, cudaStream_t stream)
 {
 	int occ = 0;
-	CG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, cg_scan_kernel<NCC, NAC, MODE, ALL8, U>, CG_THREADS, 0));
+	CG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, cg_scan_kernel<NCC, NAC, MODE, ALL8, U, VAR>, CG_THREADS, 0));
 	if (occ < 1) occ = 1;
 	uint32_t grid = (uint32_t) (ctx->sm_count * occ);
 	if (grid > plan.nselected) grid = plan.nselected;
@@ -261,7 +292,7 @@ static int launch_variant(CgContext *ctx, const KPlan &plan, cudaStream_t stream
 	bool overlap;
 	int rc = cg_chain_scan(ctx, stream, false, &overlap);     /* does not trigger its dependents early: ends a chain */
 	if (rc) return rc;
-	cg_scan_kernel<NCC, NAC, MODE, ALL8, U><<<grid, CG_THREADS, 0, stream>>>(plan);
+	cg_scan_kernel<NCC, NAC, MODE, ALL8, U, VAR><<<grid, CG_THREADS, 0, stream>>>(plan);
 	CG_CUDA(cudaGetLastError()); g_cg_launches++;
 	return CG_OK;
 }
@@ -291,6 +322,14 @@ static int launch_mode(CgContext *ctx, const KPlan &plan, bool all8, cudaStream_
 
 int cg_launch_scan(CgContext *ctx, const KPlan &plan, bool all8, cudaStream_t stream)
 {
+	/* plans with a variance aggregate: one instantiation per table kind, any column width (the others keep theirs) */
+	if (cg_plan_has_variance(plan.aggs, plan.naggs))
+		switch (plan.mode)
+		{
+			case CG_MODE_GLOBAL: return launch_variant<CG_KMAX_COLS, CG_MAX_AGGS, CG_MODE_GLOBAL, false, 1, true>(ctx, plan, stream);
+			case CG_MODE_DENSE: return launch_variant<CG_KMAX_COLS, CG_MAX_AGGS, CG_MODE_DENSE, false, 1, true>(ctx, plan, stream);
+			default: return launch_variant<CG_KMAX_COLS, CG_MAX_AGGS, CG_MODE_HASH, false, 1, true>(ctx, plan, stream);
+		}
 	if (plan.ncols <= 2) return launch_mode<2>(ctx, plan, all8, stream);
 	if (plan.ncols <= 4) return launch_mode<4>(ctx, plan, all8, stream);
 	return launch_mode<CG_KMAX_COLS>(ctx, plan, all8, stream);
@@ -746,10 +785,21 @@ __global__ void cg_merge_kernel(const __grid_constant__ KPlan P, const int64_t *
 								const uint64_t *words, int64_t nrows)
 {
 	/* low words of two-limb sums: a row's low word may hold up to 64 bits of summed low halves; its carry
-	 * (bits 32..63) moves to the high word, so the table's low word grows by < 2^32 per merged row */
-	uint32_t lo_words = 0;
+	 * (bits 32..63) moves to the high word, so the table's low word grows by < 2^32 per merged row.  The limbs of a
+	 * variance aggregate's sum(x^2) chain: limb l takes the carry of limb l - 1 and gives its own (bits 32.. of the
+	 * sum, 65 bits wide when that sum wrapped) to limb l + 1 */
+	uint32_t gives = 0, takes = 0;
 	for (int a = 0; a < P.naggs; a++)
-		if (two_limbs(P.aggs[a])) lo_words |= 1u << P.aggs[a].word0;
+	{
+		const KAgg &g = P.aggs[a];
+		if (two_sum_limbs<true>(g)) { gives |= 1u << g.word0; takes |= 1u << (g.word0 + 1); }
+		if (g.kind == CG_AGG_VARIANCE && g.qlimbs > 1)
+			for (int l = 0; l < g.qlimbs; l++)
+			{
+				if (l + 1 < g.qlimbs) gives |= 1u << (g.qword + l);
+				if (l > 0) takes |= 1u << (g.qword + l);
+			}
+	}
 	for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < nrows; i += (int64_t) gridDim.x * blockDim.x)
 	{
 		uint64_t *entry;
@@ -771,8 +821,9 @@ __global__ void cg_merge_kernel(const __grid_constant__ KPlan P, const int64_t *
 		for (int w = 0; w < P.nwords; w++)
 		{
 			uint64_t val = words[i * (int64_t) P.nwords + w];
-			if ((lo_words >> w) & 1u) { carry = val >> 32; val &= 0xffffffffull; }
-			else if (w > 0 && ((lo_words >> (w - 1)) & 1u)) val += carry;
+			uint64_t wrapped = 0;
+			if ((takes >> w) & 1u) { val += carry; wrapped = val < carry; }
+			if ((gives >> w) & 1u) { carry = (val >> 32) | (wrapped << 32); val &= 0xffffffffull; }
 			if (val != word_identity(P.wordop[w])) word_apply_global(entry + w, P.wordop[w], val);
 		}
 	}

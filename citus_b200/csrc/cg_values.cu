@@ -23,6 +23,9 @@ extern "C" int cg_partial_merge_values(CgPartial *p, int64_t nrows, const int64_
 	CgContext *ctx = cg_ctx();
 	if (!ctx || !p) return CG_EINVAL;
 	if (int rc0 = cg_chain_end(ctx, ctx->compute)) return rc0;
+	for (int a = 0; a < p->desc.naggs; a++)
+		if (p->aggs[a].kind == CG_AGG_VARIANCE)
+			return cg_set_error(CG_EUNSUPPORTED, "aggregate %d: a variance state has no sum(x^2) among the host rows (merge its words with cg_partial_merge_rows)", a);
 	if (nrows < 0) return cg_set_error(CG_EINVAL, "negative row count");
 	if (nrows == 0) return CG_OK;
 	const int na = p->desc.naggs, nw = p->nwords;

@@ -216,14 +216,21 @@ typedef struct CgInList
 } CgInList;
 
 enum { CG_AGG_COUNT_STAR = 0, CG_AGG_COUNT = 1, CG_AGG_SUM = 2, CG_AGG_MIN = 3, CG_AGG_MAX = 4,
-	   CG_AGG_BIT_AND = 5, CG_AGG_BIT_OR = 6, CG_AGG_BOOL_AND = 7, CG_AGG_BOOL_OR = 8 };
+	   CG_AGG_BIT_AND = 5, CG_AGG_BIT_OR = 6, CG_AGG_BOOL_AND = 7, CG_AGG_BOOL_OR = 8, CG_AGG_VARIANCE = 9 };
 
 /* aggregate argument = product over factors of (a + b * column); covers sum(x),
  * sum(x*y), sum(x*(1-d)), sum(x*(1-d)*(1+t)) on scaled-integer decimals (TPC-H Q1/Q6).
  * bit_and / bit_or (CG_AGG_BIT_*): the argument is one bare integer column (nfactors 1, a 0, b 1, is_float 0); the
  * result is in the column's type, the words hold it sign-extended to 64 bits.  bool_and / bool_or / every
  * (CG_AGG_BOOL_*): nfactors 0, the argument is the predicate tree arg_expr[a] of CgScanDesc.  None of the four takes
- * a term_abs_bound. */
+ * a term_abs_bound.
+ * CG_AGG_VARIANCE: the state of var_pop / var_samp / variance / stddev_pop / stddev_samp / stddev over an integer
+ * argument (the term sum takes: int1/2/4/8, numeric(p, s) as value * 10^s), which PostgreSQL keeps as the exact integers
+ * N, sum(x) and sum(x^2).  The argument follows sum's rules: the same int64 overflow check, the same optional
+ * term_abs_bound (a row over it fails the scan with CG_EINVAL; cg_relation_bounds fills it), FILTER, WHERE and every key
+ * form.  A float argument is CG_EUNSUPPORTED (float8_accum's result cannot be matched bit for bit in any order).  All
+ * six SQL names share this state: the name only picks the final function, cg_numeric_var_out, on the host.
+ * cg_partial_fetch_ex returns N in count, sum(x) in sum_hi:sum_lo and sum(x^2) in sumsq. */
 typedef struct CgAggSpec
 {
 	int32_t kind;        /* CG_AGG_* */
@@ -409,12 +416,22 @@ int cg_partial_ngroups(CgPartial *p, int64_t *ngroups);
 int cg_partial_fetch(CgPartial *p, int64_t capacity, int64_t *keys, uint8_t *key_nulls,
 					 int64_t *sum_hi, uint64_t *sum_lo, int64_t *count, int64_t *minmax,
 					 double *fsum, int64_t *ngroups);
+/* cg_partial_fetch plus sumsq [capacity * naggs * 3]: for a CG_AGG_VARIANCE aggregate, sum(x^2) of the group as an
+ * unsigned 192-bit little-endian integer in the argument's scaled units (x^2 <= 2^126, at most 2^32 rows per group), in
+ * the same group order as the other arrays (0 for the other kinds).  One call, because the order of the groups is not
+ * the same from one call to the next.  cg_partial_fetch is this call with sumsq = NULL.  A group of 2^32 rows or more
+ * in a partial with a limb-word sum is CG_EUNSUPPORTED. */
+int cg_partial_fetch_ex(CgPartial *p, int64_t capacity, int64_t *keys, uint8_t *key_nulls,
+						int64_t *sum_hi, uint64_t *sum_lo, int64_t *count, int64_t *minmax,
+						double *fsum, uint64_t *sumsq, int64_t *ngroups);
 
 /* The inverse of cg_partial_fetch: partial-aggregate ROWS held on the host (group key + per aggregate the 128-bit
  * sum, count, min / max, float sum; arrays [nrows * naggs] laid out like cg_partial_fetch's) are folded into p by the
  * combine kernel.  What the coordinator does with the per-shard result rows it receives (adaptive_executor.c:3964-4189
  * ReceiveResults -> TupleDestination) in place of a CPU HashAggregate over them.  Arrays an aggregate list does not
- * need may be NULL.  count[] of a sum / min / max is its number of non-NULL inputs (0 = the partial was SQL NULL). */
+ * need may be NULL.  count[] of a sum / min / max is its number of non-NULL inputs (0 = the partial was SQL NULL).
+ * A partial with a CG_AGG_VARIANCE aggregate is CG_EUNSUPPORTED: the rows carry no sum(x^2) (merge the words with
+ * cg_partial_merge_rows instead). */
 int cg_partial_merge_values(CgPartial *p, int64_t nrows, const int64_t *keys, const uint8_t *key_nulls, const int64_t *sum_hi,
 							const uint64_t *sum_lo, const int64_t *count, const int64_t *minmax, const double *fsum);
 /* count / exact sum / min / max of one host column (attlen 1, 2, 4, 8; float4 is widened to float8 for min / max; a float
@@ -428,6 +445,10 @@ int cg_agg_column(int32_t attlen, int32_t is_float, const void *values, const ui
  * with one commutative op (add / min / max / float add), so partials of different
  * shards or GPUs are merged word by word -- by this library (cg_partial_merge_rows)
  * or by ncclReduce on the dense layout. */
+/* at most CG_MAX_WORDS words per group: word 0 (rows) and per aggregate count(*) 0 (1 with a FILTER), count(x) 1,
+ * sum 2 or 3, min / max / bit_* / bool_* 2, variance 3 to 7 (7 without a term_abs_bound); cg_partial_create refuses a
+ * longer aggregate list with CG_EUNSUPPORTED */
+#define CG_MAX_WORDS 32
 int cg_partial_layout(const CgPartial *p, int32_t *nwords, int32_t *word_ops /* [nwords] CG_WORD_* */,
 					  int32_t *is_dense, int64_t *capacity);
 /* CG_WORD_AND / CG_WORD_OR: bitwise, identities ~0 and 0 (bit_and / bit_or values; bool_and / bool_or keep the truth
@@ -598,6 +619,17 @@ int cg_selected_chunk_mask(const CgRelation *rel, int32_t stripe_index, const Cg
  * master-side sum(sum)/sum(count), multi_logical_optimizer.c:1807-1830).  buf >= 64 bytes. */
 int cg_numeric_out(int64_t hi, uint64_t lo, int32_t scale, char *buf, size_t buflen);
 int cg_numeric_div_out(int64_t hi, uint64_t lo, int32_t scale, int64_t count, char *buf, size_t buflen);
+/* The final functions of a CG_AGG_VARIANCE state, as PostgreSQL's numeric_stddev_internal computes them from
+ * N = n, S = sum_hi:sum_lo and Q = sumsq[0..3) (192-bit little-endian), all in units of 10^-scale (scale 0..30):
+ *   NULL (*is_null = 1, buf = "") when N = 0, or N <= 1 for the sample forms;
+ *   num = N * Q - S^2 at display scale 2 * scale; num <= 0 gives the text "0";
+ *   otherwise den = N * (N - 1) (samp) or N^2 (pop), rscale = select_div_scale(num, den) (16 significant digits counted
+ *   in base-10000 digits, at least 2 * scale, within [0, 1000]), the variance = num / den rounded half away from zero at
+ *   rscale, and the standard deviation = the square root of that rounded variance, rounded half away from zero at
+ *   rscale.  The text has exactly rscale fraction digits.  A buffer too small for it is CG_EINVAL. */
+enum { CG_VAR_POP = 0, CG_VAR_SAMP = 1, CG_STDDEV_POP = 2, CG_STDDEV_SAMP = 3 };
+int cg_numeric_var_out(int32_t final, int64_t n, int64_t sum_hi, uint64_t sum_lo, const uint64_t *sumsq /* [3] */, int32_t scale,
+					   char *buf, size_t buflen, int32_t *is_null);
 
 /* ---------------------------------------------------------------------------------- *
  *  Synthetic shard writer (bench / test tooling; the on-disk encoding of

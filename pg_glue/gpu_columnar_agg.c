@@ -54,7 +54,8 @@ PG_MODULE_MAGIC;
 void _PG_init(void);
 
 /* what one output column of the node is made of */
-typedef enum GpuOutKind { GPU_OUT_KEY, GPU_OUT_COUNT, GPU_OUT_SUM_NUMERIC, GPU_OUT_SUM_INT8, GPU_OUT_SUM_FLOAT8, GPU_OUT_MINMAX } GpuOutKind;
+typedef enum GpuOutKind { GPU_OUT_KEY, GPU_OUT_COUNT, GPU_OUT_SUM_NUMERIC, GPU_OUT_SUM_INT8, GPU_OUT_SUM_FLOAT8, GPU_OUT_MINMAX,
+						  GPU_OUT_VARIANCE } GpuOutKind;
 
 typedef struct GpuOutColumn
 {
@@ -62,6 +63,7 @@ typedef struct GpuOutColumn
 	int32 index;         /* group column number / aggregate number in the CgScanDesc */
 	Oid type;            /* result type */
 	int32 scale;         /* numeric display scale of a sum over scaled integers (0 for plain int8) */
+	int32 final;         /* GPU_OUT_VARIANCE: CG_VAR_POP / CG_VAR_SAMP / CG_STDDEV_POP / CG_STDDEV_SAMP */
 } GpuOutColumn;
 
 /* the plan-time product: travels in CustomScan.custom_private as one bytea Const (so that copyObject works) */
@@ -88,6 +90,7 @@ typedef struct GpuColumnarAggState
 	int64 *count;
 	int64 *minmax;
 	double *fsum;
+	uint64 *sumsq;       /* [cells * 3]: sum(x^2) of the variance aggregates */
 	/* composite key: the decoded key columns of every group, [group][column] */
 	int64 *key_values;
 	uint8 *key_value_nulls;
@@ -341,6 +344,23 @@ translate_where(Node *node, TupleDesc tupdesc, CgScanDesc *desc, CgQual *atoms, 
 	return true;
 }
 
+/* the most accumulator words the library can lay out for the aggregate list (include/citus_gpu.h, CG_MAX_WORDS): word 0
+ * plus per aggregate its widest form, whatever the term bounds turn out to be */
+static int
+worst_case_words(const CgScanDesc *desc)
+{
+	int words = 1;
+	for (int a = 0; a < desc->naggs; a++)
+		switch (desc->aggs[a].kind)
+		{
+			case CG_AGG_COUNT_STAR: case CG_AGG_COUNT: words += 1; break;
+			case CG_AGG_SUM: words += 3; break;
+			case CG_AGG_VARIANCE: words += 7; break;
+			default: words += 2; break;
+		}
+	return words;
+}
+
 /* the worker half of the aggregate split names plain built-ins (planner/multi_logical_optimizer.c:3160-3484) */
 static bool
 translate_aggref(Aggref *agg, TupleDesc tupdesc, CgScanDesc *desc, GpuOutColumn *out)
@@ -412,6 +432,19 @@ translate_aggref(Aggref *agg, TupleDesc tupdesc, CgScanDesc *desc, GpuOutColumn 
 		/* any_value(x): any non-NULL input -- the minimum is one */
 		spec->kind = name[1] == 'a' ? CG_AGG_MAX : CG_AGG_MIN;
 		out->kind = GPU_OUT_MINMAX; out->type = var->vartype;
+	}
+	else if (strcmp(name, "var_pop") == 0 || strcmp(name, "var_samp") == 0 || strcmp(name, "variance") == 0 ||
+			 strcmp(name, "stddev_pop") == 0 || strcmp(name, "stddev_samp") == 0 || strcmp(name, "stddev") == 0)
+	{
+		/* over int2 / int4 / int8 PostgreSQL keeps N, sum(x) and sum(x^2) as exact integers and the result is numeric: one
+		 * state for all six names, the name picks the final function (cg_numeric_var_out).  A float argument keeps the
+		 * reference's executor (float8_accum cannot be matched bit for bit) */
+		if (var->vartype != INT2OID && var->vartype != INT4OID && var->vartype != INT8OID)
+			return false;
+		const bool pop = strcmp(name, "var_pop") == 0 || strcmp(name, "stddev_pop") == 0;
+		spec->kind = CG_AGG_VARIANCE;
+		out->kind = GPU_OUT_VARIANCE; out->type = NUMERICOID;
+		out->final = strncmp(name, "var", 3) == 0 ? (pop ? CG_VAR_POP : CG_VAR_SAMP) : (pop ? CG_STDDEV_POP : CG_STDDEV_SAMP);
 	}
 	else if (strcmp(name, "bit_and") == 0 || strcmp(name, "bit_or") == 0)
 	{
@@ -502,7 +535,9 @@ translate_query(PlannerInfo *root, RelOptInfo *input_rel, GpuAggPlan *plan)
 		plan->nout++;
 	}
 	table_close(rel, AccessShareLock);
-	return ok && plan->desc.naggs > 0;
+	/* the library refuses an aggregate list whose words pass CG_MAX_WORDS, and only at run time, when the bounds are known:
+	 * a list that could pass it keeps the reference executor */
+	return ok && plan->desc.naggs > 0 && worst_case_words(&plan->desc) <= CG_MAX_WORDS;
 }
 
 /* ------------------------------------------------------------------------------------ *
@@ -769,8 +804,9 @@ run_scan(GpuColumnarAggState *state)
 	state->sum_hi = palloc(sizeof(int64) * cells); state->sum_lo = palloc(sizeof(uint64) * cells);
 	state->count = palloc(sizeof(int64) * cells); state->minmax = palloc(sizeof(int64) * cells);
 	state->fsum = palloc(sizeof(double) * cells);
-	gpu_check(cg_partial_fetch(state->partial, Max(n, 1), state->keys, state->key_nulls, state->sum_hi, state->sum_lo, state->count,
-							   state->minmax, state->fsum, &state->ngroups));
+	state->sumsq = palloc(sizeof(uint64) * 3 * cells);
+	gpu_check(cg_partial_fetch_ex(state->partial, Max(n, 1), state->keys, state->key_nulls, state->sum_hi, state->sum_lo, state->count,
+								  state->minmax, state->fsum, state->sumsq, &state->ngroups));
 	if (desc->composite_key)
 	{
 		/* the key arrays hold composite codes: the key columns come from the library's decoder */
@@ -859,6 +895,17 @@ GpuColumnarAgg_Exec(CustomScanState *node)
 				if (state->count[cell] == 0) { slot->tts_isnull[i] = true; break; }
 				slot->tts_values[i] = i64_to_datum(state->minmax[cell], out->type);
 				break;
+			case GPU_OUT_VARIANCE:
+			{
+				/* numeric_stddev_internal's text: up to 1000 fraction digits */
+				char buf[1200];
+				int32 isnull = 0;
+				gpu_check(cg_numeric_var_out(out->final, state->count[cell], state->sum_hi[cell], state->sum_lo[cell], &state->sumsq[cell * 3],
+											 out->scale, buf, sizeof buf, &isnull));
+				if (isnull) { slot->tts_isnull[i] = true; break; }
+				slot->tts_values[i] = DirectFunctionCall3(numeric_in, CStringGetDatum(buf), ObjectIdGetDatum(InvalidOid), Int32GetDatum(-1));
+				break;
+			}
 		}
 	}
 	return ExecStoreVirtualTuple(slot);
