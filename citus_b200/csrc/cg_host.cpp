@@ -938,6 +938,7 @@ extern "C" int cg_shard_stage(const CgRelation *rel, const int32_t *columns, int
 	}
 	cudaFree(d_decode); cudaFree(d_varlena);
 	if (rc) { cg_shard_free(sh); return rc; }
+	cg_shard_build_narrow(ctx, sh);
 	*out = sh;
 	return CG_OK;
 }
@@ -948,10 +949,12 @@ extern "C" void cg_shard_free(CgShard *sh)
 	cudaFree(sh->d_arena);
 	cudaFree(sh->d_chunkcols);
 	cudaFree(sh->d_selected);
+	cudaFree(sh->d_narrow);
+	cudaFree(sh->d_packcols);
 	delete sh;
 }
 
-extern "C" uint64_t cg_shard_device_bytes(const CgShard *sh) { return sh ? sh->arena_bytes : 0; }
+extern "C" uint64_t cg_shard_device_bytes(const CgShard *sh) { return sh ? sh->arena_bytes + sh->narrow_bytes : 0; }
 extern "C" uint64_t cg_shard_rows(const CgShard *sh) { return sh ? sh->rows : 0; }
 
 /* ------------------------------------------------------------------------------ *
@@ -1162,6 +1165,25 @@ static int upload_sets(CgContext *ctx, CgPartial *p, const std::vector<uint64_t>
 	return CG_OK;
 }
 
+/* the fast kernel reads the narrow images when its plan has at most three columns (the shapes whose narrow instances fit
+ * 64 registers without spilling, cg_scan_fast.cu) and every one of them has images in this shard */
+static void set_narrow(const CgShard *sh, FPlan *f)
+{
+	const int nc = f->nquals + (f->mode != CG_MODE_GLOBAL ? 1 : 0) + f->nsums;
+	bool all = nc > 0 && nc <= 3 && !sh->slot_narrow.empty();
+	for (int c = 0; all && c < nc; c++) all = sh->slot_narrow[f->slot[c]] != 0;
+	f->narrow = all ? 1 : 0;
+	f->narrow_base = all ? sh->d_narrow : nullptr;
+	f->packcols = all ? sh->d_packcols : nullptr;
+}
+
+/* bytes of a chunk column's narrow stream (what the fast kernel reads of it) */
+static uint64_t narrow_stream_bytes(const CgShard *sh, uint64_t cg, int slot)
+{
+	const DevPackCol &pc = sh->h_packcols[cg * sh->staged.size() + slot];
+	return pc.width == CG_NARROW_NONE ? 0 : cg_narrow_words(sh->cg_rows[cg], pc.width) * 8;
+}
+
 extern "C" int cg_scan_shard(const CgShard *sh, const CgScanDesc *desc, CgPartial *into, CgScanStats *stats)
 {
 	CgContext *ctx = cg_ctx();
@@ -1237,9 +1259,6 @@ extern "C" int cg_scan_shard(const CgShard *sh, const CgScanDesc *desc, CgPartia
 	const std::vector<uint32_t> &selected = sh->h_selected;
 	int64_t filtered = sh->sel_filtered;
 	uint64_t bytes = 0;
-	if (stats)
-		for (uint32_t cg : selected)
-			for (int c = 0; c < plan.ncols; c++) bytes += sh->algorithmic_bytes_per_cg_col(cg, plan.slot[c]);
 	unsigned long long before[3];
 	rc = stats_begin(ctx, into, stats, before);
 	if (rc) return rc;
@@ -1255,7 +1274,16 @@ extern "C" int cg_scan_shard(const CgShard *sh, const CgScanDesc *desc, CgPartia
 		plan.max_cg_rows = sh->sel_max_cg_rows;
 		FPlan fplan;
 		const FPlan *fast = fast_eligible(desc, plan, all8, &fplan) ? &fplan : nullptr;
-		if (stats) CG_CUDA(cudaEventRecord(ctx->ev_a, ctx->compute));     /* stats_begin has ended the chain */
+		if (fast) set_narrow(sh, &fplan);
+		if (stats)
+		{
+			/* the bytes the kernels read: the narrow streams where the fast kernel reads them, the plain columns elsewhere */
+			for (size_t i = 0; i < selected.size(); i++)
+				for (int c = 0; c < plan.ncols; c++)
+					bytes += (fast && fast->narrow && i < sh->sel_nfast) ? narrow_stream_bytes(sh, selected[i], plan.slot[c])
+																		 : sh->algorithmic_bytes_per_cg_col(selected[i], plan.slot[c]);
+			CG_CUDA(cudaEventRecord(ctx->ev_a, ctx->compute));     /* stats_begin has ended the chain */
+		}
 		/* the chunk groups without NULLs in the plan columns come first in the selection; when no specialised kernel
 		 * takes them they join the rest */
 		KPlan rest = plan;

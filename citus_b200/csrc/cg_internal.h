@@ -113,6 +113,29 @@ struct DevChunkCol
 	uint32_t row_count;
 };
 
+/*
+ * Narrow image of an 8-byte integer chunk column (cg_narrow.cu), built at staging next to the plain arena for the
+ * ahead-of-time fast kernel: value = base + field in wrapping uint64, field r at bits [r * width, r * width + width) of
+ * a bit stream of 64-bit little-endian words.  Rows [64 k, 64 k + 64) take exactly the words [k * width, k * width +
+ * width), so a warp's 64 consecutive rows are one contiguous run of at most 256 bytes; the stream holds
+ * ceil(rows / 64) * width words, 16-byte aligned.  width = CG_NARROW_NONE: no image (NULLs in the chunk column, or the
+ * column has no image in this shard).
+ */
+#define CG_NARROW_NONE 255u
+#define CG_NARROW_MAX_WIDTH 32u
+struct DevPackCol
+{
+	uint64_t off;           /* byte offset of the bit stream in CgShard.d_narrow */
+	int64_t base;           /* minimum of the chunk column */
+	uint32_t width;         /* bits per row, 0 .. CG_NARROW_MAX_WIDTH, or CG_NARROW_NONE */
+	uint32_t pad;
+};
+/* words of a chunk column's bit stream */
+static inline __host__ __device__ uint64_t cg_narrow_words(uint32_t rows, uint32_t width)
+{
+	return (uint64_t) ((rows + 63u) / 64u) * width;
+}
+
 struct CgShard
 {
 	int natts = 0;
@@ -147,6 +170,12 @@ struct CgShard
 	uint32_t sel_nfast = 0;
 	uint32_t sel_max_cg_rows = 0;
 	uint64_t sel_rows_fast = 0, sel_rows_total = 0;   /* rows of the first part / of the whole selection */
+	/* narrow images (cg_narrow.cu): a staged column has them in every NULL-free chunk group or in none */
+	uint8_t *d_narrow = nullptr;
+	uint64_t narrow_bytes = 0;
+	DevPackCol *d_packcols = nullptr;        /* [nchunkgroups][nstaged] */
+	std::vector<DevPackCol> h_packcols;
+	std::vector<uint8_t> slot_narrow;        /* per staged slot: 1 = the column has images */
 	uint64_t algorithmic_bytes_per_cg_col(uint64_t cg, int slot) const
 	{
 		const DevChunkCol &c = h_chunkcols[cg * staged.size() + slot];
@@ -360,6 +389,11 @@ struct FPlan
 	int32_t slices;               /* see KPlan */
 	uint32_t slice_rows;
 	uint32_t max_cg_rows;
+	/* nonzero: every column the plan reads has narrow images in this shard, and the kernel reads those instead of the
+	 * arena (set by cg_scan_shard; the chunk groups the fast kernel takes are NULL-free, so all of them have images) */
+	int32_t narrow;
+	const uint8_t *narrow_base;
+	const DevPackCol *packcols;
 };
 /* how many row ranges a chunk group is cut into so that `nselected` chunk groups give a launch of `grid_full` CTAs at least two
  * units per CTA; step = rows one CTA iteration covers (slice boundaries stay multiples of it) */
@@ -559,6 +593,8 @@ uint64_t cg_key_codec_id(const CgScanDesc *desc);
 int cg_partial_shape(CgPartial *p, const CgScanDesc *desc, const CgColumnDesc *columns, int32_t natts,
 					 int64_t key_min, int64_t key_max, int64_t max_rows);
 bool cg_build_fast_plan(const CgScanDesc *desc, const KPlan &plan, bool all8, FPlan *fast);
+/* narrow images of a freshly staged shard (cg_narrow.cu); best effort: when they cannot be built the shard stays as staged */
+void cg_shard_build_narrow(CgContext *ctx, CgShard *sh);
 /* set_codes (may be NULL): receives the codes plan->qset / fset index (KPlan.sets is left NULL for the caller to point at
  * their device copy) */
 int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts,

@@ -32,6 +32,14 @@ __device__ __forceinline__ void ldg16(const void *p, uint64_t &a, uint64_t &b, u
 	asm("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.u64 {%0, %1}, [%2], %3;" : "=l"(a), "=l"(b) : "l"(p), "l"(policy));
 }
 
+/* one 64-bit word of a narrow image (DevPackCol): same streaming path and hint as ldg16 */
+__device__ __forceinline__ uint64_t ldg8(const void *p, uint64_t policy)
+{
+	uint64_t a;
+	asm("ld.global.nc.L1::no_allocate.L2::cache_hint.u64 %0, [%1], %2;" : "=l"(a) : "l"(p), "l"(policy));
+	return a;
+}
+
 /* group-table update: fire-and-forget reduction at the L2 atomic unit */
 __device__ __forceinline__ void red_add_u64(uint64_t *p, uint64_t v)
 {
@@ -247,8 +255,16 @@ __device__ __forceinline__ uint64_t warp_sum(uint64_t x)
 	return x;
 }
 
-template <int NQ, int MODE, int NS, bool PACK, int U>
-__global__ void __launch_bounds__(CGF_THREADS)
+/*
+ * NARROW: the columns come from the shard's narrow images instead of the arena.  Rows [64 k, 64 k + 64) of a chunk column
+ * are the `width` words [k * width, (k + 1) * width) of its bit stream, and a warp's 64 consecutive rows are one such
+ * block (every warp starts at a multiple of 64 rows): lane i loads word i, and each lane takes the (at most two) words its
+ * two rows' fields lie in from the lanes that loaded them.  Narrow plans have at most three columns (cg_host.cpp
+ * set_narrow); their instances are held to 64 registers (four CTAs per SM, as the plain C2 instance), which they meet
+ * without spilling.
+ */
+template <int NQ, int MODE, int NS, bool PACK, int U, bool NARROW>
+__global__ void __launch_bounds__(CGF_THREADS, NARROW ? 4 : 0)
 cg_scan_fast_kernel(const __grid_constant__ FPlan P)
 {
 	constexpr int NC = NQ + (MODE != CG_MODE_GLOBAL ? 1 : 0) + NS;
@@ -264,6 +280,7 @@ cg_scan_fast_kernel(const __grid_constant__ FPlan P)
 	uint32_t removed = 0;
 	unsigned long long scanned = 0;
 	const uint32_t tid = threadIdx.x;
+	const uint32_t lane = tid & 31u;
 	const uint64_t pol_stream = policy_evict_first();
 	/* hash tables with single-word sums: lane-paired updates (decided per launch, uniform) */
 	const bool paired = (MODE == CG_MODE_HASH) && !PACK && NS > 0 && (P.flags & CG_FAST_PAIRED);
@@ -279,8 +296,22 @@ cg_scan_fast_kernel(const __grid_constant__ FPlan P)
 		const uint32_t row0 = sl * P.slice_rows;
 		const uint32_t rows = min(chunk_rows, row0 + P.slice_rows);       /* this unit covers rows [row0, rows) */
 		const uint8_t *vp[NCA];
+		/* narrow: the stream's first word (an index into P.narrow_base, which stays in the parameter bank), base, width */
+		uint32_t nword[NCA], nwidth[NCA];
+		int64_t nbase[NCA];
 #pragma unroll
-		for (int c = 0; c < NC; c++) vp[c] = P.arena + __ldg(&cc[P.slot[c]].values_off);
+		for (int c = 0; c < NC; c++)
+		{
+			if (NARROW)
+			{
+				const DevPackCol *pc = P.packcols + (uint64_t) P.selected[ci] * (uint64_t) P.nstaged + P.slot[c];
+				nword[c] = (uint32_t) (__ldg(&pc->off) / 8);
+				nbase[c] = __ldg(&pc->base);
+				nwidth[c] = __ldg(&pc->width);
+			}
+			else
+				vp[c] = P.arena + __ldg(&cc[P.slot[c]].values_off);
+		}
 		scanned += (tid == 0 && sl == 0) ? chunk_rows : 0;
 		if (NC == 0)
 		{
@@ -291,11 +322,23 @@ cg_scan_fast_kernel(const __grid_constant__ FPlan P)
 		for (uint32_t base = row0; base < rows; base += CGF_THREADS * 2 * U)
 		{
 			int64_t v0[U][NCA], v1[U][NCA];
+			uint64_t raw[U][NCA];
 #pragma unroll
 			for (int u = 0; u < U; u++)
 			{
 				uint32_t r = base + (u * CGF_THREADS + tid) * 2;
-				if (r < rows)
+				if (NARROW)
+				{
+					const uint32_t r0 = base + (u * CGF_THREADS + (tid & ~31u)) * 2;     /* the warp's first row */
+#pragma unroll
+					for (int c = 0; c < NC; c++)
+					{
+						raw[u][c] = 0;
+						if (r0 < rows && lane < nwidth[c])
+							raw[u][c] = ldg8((const uint64_t *) P.narrow_base + nword[c] + (r0 / 64u) * nwidth[c] + lane, pol_stream);
+					}
+				}
+				else if (r < rows)
 				{
 #pragma unroll
 					for (int c = 0; c < NC; c++)
@@ -310,6 +353,27 @@ cg_scan_fast_kernel(const __grid_constant__ FPlan P)
 			for (int u = 0; u < U; u++)
 			{
 				uint32_t r = base + (u * CGF_THREADS + tid) * 2;
+				if (NARROW && base + (u * CGF_THREADS + (tid & ~31u)) * 2 < rows)
+				{
+					/* warp-uniform: the fields of rows r, r + 1 lie in bits [2 lane w, 2 lane w + 2 w) of the block, at most
+					 * 64 bits (w <= 32) across words lo and lo + 1 (lo + 1 = 32 only when it is not needed) */
+#pragma unroll
+					for (int c = 0; c < NC; c++)
+					{
+						/* re-read per row block (a register move the compiler cannot hoist): the shift amounts derived from
+						 * it are cheap to recompute, and hoisting them for every column would cost the registers of a
+						 * fourth CTA per SM */
+						uint32_t w;
+						asm volatile("mov.b32 %0, %1;" : "=r"(w) : "r"(nwidth[c]));
+						const uint32_t b0 = 2u * lane * w, lo = b0 >> 6, sh = b0 & 63u;
+						const uint64_t a = __shfl_sync(0xffffffffu, raw[u][c], (int) lo);
+						const uint64_t b = __shfl_sync(0xffffffffu, raw[u][c], (int) ((lo + 1) & 31u));
+						const uint64_t x = (a >> sh) | ((b << 1) << (63u - sh));
+						const uint64_t mask = (1ull << w) - 1ull;
+						v0[u][c] = (int64_t) ((uint64_t) nbase[c] + (x & mask));
+						v1[u][c] = (int64_t) ((uint64_t) nbase[c] + ((x >> w) & mask));
+					}
+				}
 				if (MODE == CG_MODE_HASH && paired)
 				{
 					/* warp-converged: lanes past the end of the chunk group take part with pass = false */
@@ -420,15 +484,23 @@ int cg_launch_drain(CgPartial *p, cudaStream_t stream)
 	return CG_OK;
 }
 
-template <int NQ, int MODE, int NS, bool PACK>
+template <int NQ, int MODE, int NS, bool PACK, bool NARROW>
 static int launch_fast_variant(CgContext *ctx, const FPlan &plan, cudaStream_t stream)
 {
 	constexpr int NC = NQ + (MODE != CG_MODE_GLOBAL ? 1 : 0) + NS;
-	constexpr int U = NC <= 3 ? 2 : 1;
+	/* narrow plans never have more than three columns (set_narrow): no narrow instance for the wider shapes */
+	if constexpr (NARROW && NC > 3)
+		return launch_fast_variant<NQ, MODE, NS, PACK, false>(ctx, plan, stream);
+	else
+	{
+	/* two row pairs per lane and iteration, as the plain instances, where they fit 64 registers without spilling (up to two
+	 * columns): a lone launch of few, short work units then waits on as few dependent load rounds as the plain kernel.  A
+	 * three-column plan (C2) takes one row pair: the registers of a second would cost the fourth CTA per SM */
+	constexpr int U = NARROW ? (NC <= 2 ? 2 : 1) : (NC <= 3 ? 2 : 1);
 	static int occ = 0;
 	if (occ == 0)
 	{
-		CG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, cg_scan_fast_kernel<NQ, MODE, NS, PACK, U>, CGF_THREADS, 0));
+		CG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, cg_scan_fast_kernel<NQ, MODE, NS, PACK, U, NARROW>, CGF_THREADS, 0));
 		if (occ < 1) occ = 1;
 	}
 	uint32_t grid = (uint32_t) (ctx->sm_count * occ);
@@ -451,12 +523,13 @@ static int launch_fast_variant(CgContext *ctx, const FPlan &plan, cudaStream_t s
 	cfg.stream = stream;
 	cfg.attrs = &attr;
 	cfg.numAttrs = overlap ? 1 : 0;
-	CG_CUDA(cudaLaunchKernelEx(&cfg, cg_scan_fast_kernel<NQ, MODE, NS, PACK, U>, launch));
+	CG_CUDA(cudaLaunchKernelEx(&cfg, cg_scan_fast_kernel<NQ, MODE, NS, PACK, U, NARROW>, launch));
 	g_cg_launches++;
 	return CG_OK;
+	}
 }
 
-template <int NQ, int MODE>
+template <int NQ, int MODE, bool NARROW>
 static int launch_fast_ns(CgContext *ctx, const FPlan &plan, cudaStream_t stream)
 {
 	if (MODE != CG_MODE_GLOBAL && plan.packed)
@@ -464,37 +537,44 @@ static int launch_fast_ns(CgContext *ctx, const FPlan &plan, cudaStream_t stream
 		constexpr int PM = MODE == CG_MODE_GLOBAL ? CG_MODE_DENSE : MODE;
 		switch (plan.nsums)
 		{
-			case 1: return launch_fast_variant<NQ, PM, 1, true>(ctx, plan, stream);
-			case 2: return launch_fast_variant<NQ, PM, 2, true>(ctx, plan, stream);
-			default: return launch_fast_variant<NQ, PM, 3, true>(ctx, plan, stream);
+			case 1: return launch_fast_variant<NQ, PM, 1, true, NARROW>(ctx, plan, stream);
+			case 2: return launch_fast_variant<NQ, PM, 2, true, NARROW>(ctx, plan, stream);
+			default: return launch_fast_variant<NQ, PM, 3, true, NARROW>(ctx, plan, stream);
 		}
 	}
 	switch (plan.nsums)
 	{
-		case 0: return launch_fast_variant<NQ, MODE, 0, false>(ctx, plan, stream);
-		case 1: return launch_fast_variant<NQ, MODE, 1, false>(ctx, plan, stream);
-		case 2: return launch_fast_variant<NQ, MODE, 2, false>(ctx, plan, stream);
-		default: return launch_fast_variant<NQ, MODE, 3, false>(ctx, plan, stream);
+		case 0: return launch_fast_variant<NQ, MODE, 0, false, NARROW>(ctx, plan, stream);
+		case 1: return launch_fast_variant<NQ, MODE, 1, false, NARROW>(ctx, plan, stream);
+		case 2: return launch_fast_variant<NQ, MODE, 2, false, NARROW>(ctx, plan, stream);
+		default: return launch_fast_variant<NQ, MODE, 3, false, NARROW>(ctx, plan, stream);
 	}
 }
 
-template <int NQ>
+template <int NQ, bool NARROW>
 static int launch_fast_mode(CgContext *ctx, const FPlan &plan, cudaStream_t stream)
 {
 	switch (plan.mode)
 	{
-		case CG_MODE_GLOBAL: return launch_fast_ns<NQ, CG_MODE_GLOBAL>(ctx, plan, stream);
-		case CG_MODE_DENSE: return launch_fast_ns<NQ, CG_MODE_DENSE>(ctx, plan, stream);
-		default: return launch_fast_ns<NQ, CG_MODE_HASH>(ctx, plan, stream);
+		case CG_MODE_GLOBAL: return launch_fast_ns<NQ, CG_MODE_GLOBAL, NARROW>(ctx, plan, stream);
+		case CG_MODE_DENSE: return launch_fast_ns<NQ, CG_MODE_DENSE, NARROW>(ctx, plan, stream);
+		default: return launch_fast_ns<NQ, CG_MODE_HASH, NARROW>(ctx, plan, stream);
 	}
 }
 
 int cg_launch_scan_fast(CgContext *ctx, const FPlan &plan, cudaStream_t stream)
 {
+	if (plan.narrow)
+		switch (plan.nquals)
+		{
+			case 0: return launch_fast_mode<0, true>(ctx, plan, stream);
+			case 1: return launch_fast_mode<1, true>(ctx, plan, stream);
+			default: return launch_fast_mode<2, true>(ctx, plan, stream);
+		}
 	switch (plan.nquals)
 	{
-		case 0: return launch_fast_mode<0>(ctx, plan, stream);
-		case 1: return launch_fast_mode<1>(ctx, plan, stream);
-		default: return launch_fast_mode<2>(ctx, plan, stream);
+		case 0: return launch_fast_mode<0, false>(ctx, plan, stream);
+		case 1: return launch_fast_mode<1, false>(ctx, plan, stream);
+		default: return launch_fast_mode<2, false>(ctx, plan, stream);
 	}
 }

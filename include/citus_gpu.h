@@ -359,8 +359,27 @@ typedef struct CgShard CgShard;
  * is resident.  Compressed value streams (lz4, pglz, zstd) are decoded on the GPU behind the copies. */
 int cg_shard_stage(const CgRelation *rel, const int32_t *columns, int32_t ncolumns, CgShard **out);
 void cg_shard_free(CgShard *shard);
-uint64_t cg_shard_device_bytes(const CgShard *shard);
+uint64_t cg_shard_device_bytes(const CgShard *shard);   /* the arena and the narrow images */
 uint64_t cg_shard_rows(const CgShard *shard);
+
+/* Narrow images.  Besides the plain arena, cg_shard_stage keeps every staged 8-byte integer column whose NULL-free chunk
+ * columns each span at most 2^32 values (max - min < 2^32) in a second, bit-packed form: per chunk column base = min and
+ * width = bits(max - min), 0 .. 32, and row r at bits [r * width, r * width + width) of a bit stream.  The ahead-of-time
+ * fast kernel reads those images when every column of its plan has them; everything else reads the arena.  The images
+ * are best effort: when their memory cannot be had (with a fixed headroom left free) the shard is staged without them.
+ * cg_shard_narrow_bytes = bytes of the images (0: none); cg_shard_narrow_column = 1 when attribute att has them. */
+uint64_t cg_shard_narrow_bytes(const CgShard *shard);
+int32_t cg_shard_narrow_column(const CgShard *shard, int32_t att);
+
+/* The layout cg_shard_stage gives the narrow images of ncg chunk groups x ncols staged columns, arrays [ncg][ncols]:
+ * candidate[c] = column c may have images (8-byte integer); rows[g] = rows of chunk group g; nullfree[g][c] = the chunk
+ * column has no NULLs; mins / maxs = its exact minimum / maximum (read only where nullfree).  A candidate column gets
+ * images (col_narrow[c] = 1) when every NULL-free chunk column of it spans max - min < 2^32.  Out, per chunk column:
+ * widths (255 = no image), bases, byte offsets of the 16-byte aligned bit streams (ceil(rows / 64) * width words each);
+ * *total_bytes = bytes of all streams. */
+int cg_narrow_plan(int64_t ncg, int32_t ncols, const uint8_t *candidate, const uint32_t *rows, const uint8_t *nullfree,
+				   const int64_t *mins, const int64_t *maxs, uint8_t *col_narrow, uint8_t *widths, int64_t *bases, uint64_t *offs,
+				   uint64_t *total_bytes);
 
 /* ---------------------------------------------------------------------------------- *
  *  Partial aggregate state: the device-resident group table a worker task accumulates
