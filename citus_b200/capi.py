@@ -140,6 +140,8 @@ SYMBOLS = [
     ("cg_shard_rows", C.c_uint64, [_P]),
     ("cg_shard_narrow_bytes", C.c_uint64, [_P]),
     ("cg_shard_narrow_column", C.c_int32, [_P, C.c_int32]),
+    ("cg_shard_narrow_image", C.c_int, [_P, C.c_int64, C.c_int32, C.POINTER(C.c_int64), C.POINTER(C.c_uint32), _P, C.c_uint64,
+                                        C.POINTER(C.c_uint64)]),
     ("cg_narrow_plan", C.c_int, [C.c_int64, C.c_int32, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.POINTER(C.c_uint64)]),
     ("cg_partial_create", C.c_int, [C.POINTER(CgScanDesc), C.POINTER(CgColumnDesc), C.c_int32, C.c_int64,
                                     C.c_int64, C.c_int64, C.POINTER(_P)]),

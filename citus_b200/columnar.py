@@ -32,7 +32,7 @@ def init(device: int = 0):
 
 
 def set_option(name: str, value: int):
-    """cg_set_option: "jit" 0/1/2, "force_general" 0/1"""
+    """cg_set_option: "jit" 0/1/2, "force_general" 0/1, "narrow_images" 0/1, ... (include/citus_gpu.h)"""
     check(lib().cg_set_option(name.encode(), value))
 
 
@@ -454,6 +454,16 @@ class Shard:
     @property
     def rows(self):
         return lib().cg_shard_rows(self.h)
+
+    def narrow_image(self, cg: int, att: int):
+        """(base, width, words: uint64 array) of the narrow image of attribute att in chunk group cg; width 255 = none"""
+        base, width, n = C.c_int64(), C.c_uint32(), C.c_uint64()
+        check(lib().cg_shard_narrow_image(self.h, cg, att, C.byref(base), C.byref(width), None, 0, C.byref(n)))
+        words = np.zeros(n.value // 8, np.uint64)
+        if n.value:
+            check(lib().cg_shard_narrow_image(self.h, cg, att, C.byref(base), C.byref(width), words.ctypes.data, n.value,
+                                              C.byref(n)))
+        return base.value, width.value, words
 
 
 class GpuColumnarAgg:

@@ -822,6 +822,9 @@ static int stream_to_device(CgContext *ctx, const CgRelation *rel, const StagePl
 	return CG_OK;
 }
 
+/* cg_set_option("narrow_images"): 0 = cg_shard_stage builds no narrow images, so every scan reads the plain arena */
+static int g_narrow_images = 1;
+
 extern "C" int cg_shard_stage(const CgRelation *rel, const int32_t *columns, int32_t ncolumns, CgShard **out)
 {
 	CgContext *ctx = cg_ctx();
@@ -938,7 +941,7 @@ extern "C" int cg_shard_stage(const CgRelation *rel, const int32_t *columns, int
 	}
 	cudaFree(d_decode); cudaFree(d_varlena);
 	if (rc) { cg_shard_free(sh); return rc; }
-	cg_shard_build_narrow(ctx, sh);
+	if (g_narrow_images) cg_shard_build_narrow(ctx, sh);
 	*out = sh;
 	return CG_OK;
 }
@@ -972,12 +975,14 @@ static bool cg_force_general(void)
  * applies (default), 2 = always; "force_general" 1 = the interpretive kernels for everything; "lz4_lanes" 1 / 0 = LZ4 value
  * streams are decoded a lane per stream / eight lanes per stream, 2 or < 0 = by launch size (default); "zstd_coop" 0 = Zstandard
  * frames are decoded by one lane, 1 or < 0 = by the whole warp (default); "peer_window" 0 = the
- * combine and the repartition exchange stay on NCCL instead of the IPC-mapped peer window (set it on every rank) */
+ * combine and the repartition exchange stay on NCCL instead of the IPC-mapped peer window (set it on every rank); "narrow_images"
+ * 0 = shards staged from then on get no narrow images (1 = default) */
 extern "C" int cg_set_option(const char *name, int64_t value)
 {
 	if (!name) return cg_set_error(CG_EINVAL, "NULL option name");
 	if (strcmp(name, "jit") == 0) { cg_jit_set_level((int) value); return CG_OK; }
 	if (strcmp(name, "force_general") == 0) { g_force_general = value ? 1 : 0; return CG_OK; }
+	if (strcmp(name, "narrow_images") == 0) { g_narrow_images = value ? 1 : 0; return CG_OK; }
 	if (strcmp(name, "realign_tma") == 0) { cg_realign_set_tma((int) value); return CG_OK; }
 	if (strcmp(name, "lz4_lanes") == 0) { cg_decompress_set_lz4_lanes((int) value); return CG_OK; }
 	if (strcmp(name, "lz4_lane_warps") == 0) { cg_decompress_set_lz4_lane_warps((int) value); return CG_OK; }

@@ -139,6 +139,37 @@ extern "C" int32_t cg_shard_narrow_column(const CgShard *sh, int32_t att)
 	return sh->slot_narrow[sh->slot_of_att[att]];
 }
 
+extern "C" int cg_shard_narrow_image(const CgShard *sh, int64_t cg, int32_t att, int64_t *base, uint32_t *width, void *host_buf,
+									 uint64_t capacity, uint64_t *nbytes)
+{
+	if (!sh || !base || !width || !nbytes || cg < 0 || (uint64_t) cg >= sh->nchunkgroups || att < 0 || att >= sh->natts ||
+		sh->slot_of_att[att] < 0)
+		return cg_set_error(CG_EINVAL, "cg_shard_narrow_image: bad arguments");
+	*base = 0;
+	*width = CG_NARROW_NONE;
+	*nbytes = 0;
+	if (sh->h_packcols.empty()) return CG_OK;
+	const DevPackCol &pc = sh->h_packcols[(uint64_t) cg * sh->staged.size() + sh->slot_of_att[att]];
+	if (pc.width == CG_NARROW_NONE) return CG_OK;
+	const uint64_t n = cg_narrow_words(sh->cg_rows[cg], pc.width) * 8;
+	if (host_buf && capacity < n)
+		return cg_set_error(CG_EINVAL, "cg_shard_narrow_image: the image takes %llu bytes", (unsigned long long) n);
+	if (host_buf && n > 0)
+	{
+		/* the images are written once, at staging, and only read after it: no scan in flight can change them */
+		CgContext *ctx = cg_ctx();
+		if (!ctx) return CG_EINVAL;
+		int rc = cg_chain_end(ctx, ctx->compute);
+		if (rc) return rc;
+		CG_CUDA(cudaMemcpyAsync(host_buf, sh->d_narrow + pc.off, n, cudaMemcpyDeviceToHost, ctx->compute));
+		CG_CUDA(cudaStreamSynchronize(ctx->compute));
+	}
+	*base = pc.base;
+	*width = pc.width;
+	*nbytes = n;
+	return CG_OK;
+}
+
 /* frees what a failed build allocated and clears the CUDA error it left, so that the shard stays exactly as staged */
 static void narrow_abandon(CgShard *sh, NarrowItem *d_items, int64_t *d_mm)
 {

@@ -74,6 +74,8 @@ uint64_t cg_jit_compiles(void);
  *   "zstd_coop" 0 | 1 (< 0 = default = 1)       Zstandard frames: one lane decodes a frame | the warp cooperates on it
  *   "peer_window" 0 | 1                         exchange steps over NCCL | over the IPC-mapped peer window; the same
  *                                               value on every rank
+ *   "narrow_images" 0 | 1 (default 1)           shards staged from then on get no narrow images | get them where they
+ *                                               fit (a shard without them is what a failed image build leaves)
  * An unknown name is CG_EINVAL. */
 int cg_set_option(const char *name, int64_t value);
 struct CgScanDesc;
@@ -370,6 +372,11 @@ uint64_t cg_shard_rows(const CgShard *shard);
  * cg_shard_narrow_bytes = bytes of the images (0: none); cg_shard_narrow_column = 1 when attribute att has them. */
 uint64_t cg_shard_narrow_bytes(const CgShard *shard);
 int32_t cg_shard_narrow_column(const CgShard *shard, int32_t att);
+/* One chunk column's image, read back: *base, *width and its bit stream (ceil(rows / 64) * width words, *nbytes bytes) into
+ * host_buf, which must hold them; host_buf = NULL only reports them.  *width = 255 and *nbytes = 0 when the chunk column has
+ * no image.  CG_EINVAL: chunk group or attribute out of range, the attribute is not staged, or capacity is too small. */
+int cg_shard_narrow_image(const CgShard *shard, int64_t cg, int32_t att, int64_t *base, uint32_t *width, void *host_buf,
+						  uint64_t capacity, uint64_t *nbytes);
 
 /* The layout cg_shard_stage gives the narrow images of ncg chunk groups x ncols staged columns, arrays [ncg][ncols]:
  * candidate[c] = column c may have images (8-byte integer); rows[g] = rows of chunk group g; nullfree[g][c] = the chunk
