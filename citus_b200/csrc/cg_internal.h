@@ -549,12 +549,10 @@ void cg_jit_set_level(int level);     /* CG_JIT: 0 = off, 1 = where no specialis
 int cg_launch_scan_jit(CgContext *ctx, const KPlan &plan, uint32_t nullable, cudaStream_t stream, bool *launched, bool *used_packed,
 					   bool *packed_only = nullptr);
 
-/* cg_partition.cu: the same without host synchronisation (counts stay on the device; d_counts has P + 1 words,
- * the last one counts rows whose hash fell in no interval) */
-int cg_partition_index_async(const int64_t *d_keys, const uint8_t *d_nulls, int64_t n, int32_t key_len, int32_t by_hash,
-							 const int32_t *mins, const int32_t *maxs, int32_t P, int32_t *d_index, int64_t *d_counts);
-int cg_partition_scatter_async(const int32_t *d_index, int64_t n, int32_t P, const int32_t *h_order, const int64_t *const *d_cols,
-							   int32_t ncols, int64_t *const *d_out);
+/* cg_partition.cu: per-partition exclusive scan of per-block counts on ctx->compute, with all SMs.  d_block[b * P + p]
+ * becomes the sum of d_block[b' * P + p] over b' < b, d_tot[p] the sum over all nblocks (> 0) blocks; scratch holds the
+ * chunk sums until it is returned to the pool in stream order. */
+int partition_scan_blocks(CgContext *ctx, unsigned long long *d_block, unsigned long long *d_tot, int64_t nblocks, int P, CgAsyncBuf *scratch);
 
 /* Scatter straight into the receive buffers of other ranks (peer-mapped memory).  Output positions are
  * destination-major: positions [pos_begin[d], pos_begin[d + 1]) belong to rank d, whose buffer holds column c at

@@ -47,6 +47,42 @@ __device__ __forceinline__ unsigned long long join_home(long long key, int shift
 	return ((unsigned long long) key * 0x9E3779B97F4A7C15ull) >> shift;
 }
 
+/*
+ * The slot of `key` in an open-addressing table of cap key slots (a power of two), for every key but the EMPTY sentinel,
+ * whose slot is cap; ~0 when the key is absent (FIND) or the table is full (CLAIM).  CLAIM claims an empty slot with a
+ * CAS and reads the keys through L2 (__ldcg: other threads are claiming slots); FIND stops at an empty slot and reads the
+ * keys of a table an earlier kernel built through the read-only path (__ldg).
+ */
+enum JoinFind { CLAIM, FIND };
+
+template <JoinFind MODE>
+__device__ __forceinline__ unsigned long long join_find(long long *table, unsigned long long cap, int shift, long long key)
+{
+	unsigned long long h = join_home(key, shift), slot = ~0ull;
+	for (unsigned long long probes = 0; probes <= cap; probes++)
+	{
+		long long cur = MODE == CLAIM ? (long long) __ldcg((unsigned long long *) table + h) : (long long) __ldg((const unsigned long long *) table + h);
+		if (cur == key) { slot = h; break; }
+		if (cur == CGJ_EMPTY)
+		{
+			if (MODE == FIND) break;
+			long long old = (long long) atomicCAS((unsigned long long *) table + h, (unsigned long long) CGJ_EMPTY, (unsigned long long) key);
+			if (old == CGJ_EMPTY || old == key) { slot = h; break; }
+		}
+		h = (h + 1) & (cap - 1);
+	}
+	return slot;
+}
+
+/* load factor <= 1/2: cap = the smallest power of two >= 2 * nbuild, at least 1024; shift = 64 - log2(cap) */
+static void join_table_size(int64_t nbuild, unsigned long long *cap, int *shift)
+{
+	*cap = 1024;
+	while (*cap < 2ull * (uint64_t) nbuild) *cap <<= 1;
+	*shift = 64;
+	for (unsigned long long c = *cap; c > 1; c >>= 1) (*shift)--;
+}
+
 __global__ void __launch_bounds__(CGJ_THREADS)
 cg_join_build_kernel(JoinTable T, const long long *keys, const uint8_t *nulls, const long long *payload, long long n)
 {
@@ -57,19 +93,7 @@ cg_join_build_kernel(JoinTable T, const long long *keys, const uint8_t *nulls, c
 		unsigned long long slot = T.cap;
 		if (key != CGJ_EMPTY)
 		{
-			unsigned long long h = join_home(key, T.shift);
-			slot = ~0ull;
-			for (unsigned long long probes = 0; probes <= T.cap; probes++)
-			{
-				long long cur = (long long) __ldcg((unsigned long long *) T.keys + h);
-				if (cur == key) { slot = h; break; }
-				if (cur == CGJ_EMPTY)
-				{
-					long long old = (long long) atomicCAS((unsigned long long *) T.keys + h, (unsigned long long) CGJ_EMPTY, (unsigned long long) key);
-					if (old == CGJ_EMPTY || old == key) { slot = h; break; }
-				}
-				h = (h + 1) & (T.cap - 1);
-			}
+			slot = join_find<CLAIM>(T.keys, T.cap, T.shift, key);
 			if (slot == ~0ull) { atomicAdd(T.errors, 1ull); continue; }
 		}
 		const long long x = payload[r];
@@ -101,15 +125,7 @@ cg_join_probe_kernel(JoinTable T, const long long *keys, const uint8_t *nulls, c
 		unsigned long long slot = T.cap;
 		if (key != CGJ_EMPTY)
 		{
-			unsigned long long h = join_home(key, T.shift);
-			slot = ~0ull;
-			for (unsigned long long probes = 0; probes <= T.cap; probes++)
-			{
-				long long cur = (long long) __ldg((const unsigned long long *) T.keys + h);
-				if (cur == key) { slot = h; break; }
-				if (cur == CGJ_EMPTY) break;
-				h = (h + 1) & (T.cap - 1);
-			}
+			slot = join_find<FIND>(T.keys, T.cap, T.shift, key);
 			if (slot == ~0ull) continue;
 		}
 		const ulonglong2 v01 = __ldg((const ulonglong2 *) (T.vals + slot * 4));
@@ -151,10 +167,7 @@ extern "C" int cg_join_count_sum(const int64_t *d_build_keys, const uint8_t *d_b
 	*joined_rows = 0; *sum_hi = 0; *sum_lo = 0;
 	if (nbuild == 0 || nprobe == 0) return CG_OK;
 	JoinTable T;
-	T.cap = 1024;
-	while (T.cap < 2ull * (uint64_t) nbuild) T.cap <<= 1;
-	T.shift = 64;
-	for (unsigned long long c = T.cap; c > 1; c >>= 1) T.shift--;
+	join_table_size(nbuild, &T.cap, &T.shift);
 	const size_t key_bytes = (T.cap + 1) * sizeof(long long), val_bytes = (T.cap + 1) * 4 * sizeof(unsigned long long);
 	uint8_t *d_mem = nullptr;
 	if (cudaMallocAsync((void **) &d_mem, key_bytes + 64 + val_bytes + 64, ctx->compute) != cudaSuccess)
@@ -210,25 +223,6 @@ struct JoinRowsTable
 	unsigned long long *errors;
 };
 
-__device__ __forceinline__ unsigned long long join_rows_find(const JoinRowsTable &T, long long key, bool insert)
-{
-	if (key == CGJ_EMPTY) return T.cap;
-	unsigned long long h = join_home(key, T.shift);
-	for (unsigned long long probes = 0; probes <= T.cap; probes++)
-	{
-		long long cur = (long long) __ldcg((unsigned long long *) T.keys + h);
-		if (cur == key) return h;
-		if (cur == CGJ_EMPTY)
-		{
-			if (!insert) return ~0ull;
-			long long old = (long long) atomicCAS((unsigned long long *) T.keys + h, (unsigned long long) CGJ_EMPTY, (unsigned long long) key);
-			if (old == CGJ_EMPTY || old == key) return h;
-		}
-		h = (h + 1) & (T.cap - 1);
-	}
-	return ~0ull;
-}
-
 __global__ void cg_join_rows_init_kernel(JoinRowsTable T)
 {
 	for (unsigned long long i = (unsigned long long) blockIdx.x * blockDim.x + threadIdx.x; i <= T.cap; i += (unsigned long long) gridDim.x * blockDim.x)
@@ -243,14 +237,15 @@ cg_join_rows_build_kernel(JoinRowsTable T, const long long *keys, const uint8_t 
 	for (long long r = (long long) blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (long long) gridDim.x * blockDim.x)
 	{
 		if (nulls && nulls[r]) continue;
-		unsigned long long slot = join_rows_find(T, keys[r], true);
+		const long long key = keys[r];
+		const unsigned long long slot = key == CGJ_EMPTY ? T.cap : join_find<CLAIM>(T.keys, T.cap, T.shift, key);
 		if (slot == ~0ull) { atomicAdd(T.errors, 1ull); continue; }
 		atomicAdd(T.count + slot, 1u);
 		T.next[r] = (long long) atomicExch((unsigned long long *) T.head + slot, (unsigned long long) r);
 	}
 }
 
-/* matches[r] = rows probe row r joins; block sums for the scan */
+/* matches[r] = rows probe row r joins; block sums for the scan (partition_scan_blocks with one partition) */
 __global__ void __launch_bounds__(CGJ_THREADS)
 cg_join_rows_count_kernel(JoinRowsTable T, const long long *keys, const uint8_t *nulls, long long n, unsigned int *matches,
 						  unsigned long long *block_sums)
@@ -260,7 +255,8 @@ cg_join_rows_count_kernel(JoinRowsTable T, const long long *keys, const uint8_t 
 	unsigned int m = 0;
 	if (r < n && !(nulls && nulls[r]))
 	{
-		unsigned long long slot = join_rows_find(T, keys[r], false);
+		const long long key = keys[r];
+		const unsigned long long slot = key == CGJ_EMPTY ? T.cap : join_find<FIND>(T.keys, T.cap, T.shift, key);
 		if (slot != ~0ull) m = T.count[slot];
 	}
 	if (r < n) matches[r] = m;
@@ -273,29 +269,6 @@ cg_join_rows_count_kernel(JoinRowsTable T, const long long *keys, const uint8_t 
 		for (int i = 0; i < CGJ_THREADS / 32; i++) t += s_sum[i];
 		block_sums[blockIdx.x] = t;
 	}
-}
-
-/* exclusive scan of the block sums by one block (nblocks is n / 256: up to ~1 M entries, a few hundred microseconds) */
-__global__ void __launch_bounds__(1024)
-cg_join_rows_scan_kernel(unsigned long long *block_sums, long long nblocks, unsigned long long *total)
-{
-	__shared__ unsigned long long s[1024];
-	const long long per = (nblocks + 1023) / 1024;
-	const long long b0 = (long long) threadIdx.x * per, b1 = b0 + per < nblocks ? b0 + per : nblocks;
-	unsigned long long local = 0;
-	for (long long b = b0; b < b1; b++) local += block_sums[b];
-	s[threadIdx.x] = local;
-	__syncthreads();
-	for (int off = 1; off < 1024; off <<= 1)
-	{
-		unsigned long long v = threadIdx.x >= (unsigned) off ? s[threadIdx.x - off] : 0;
-		__syncthreads();
-		s[threadIdx.x] += v;
-		__syncthreads();
-	}
-	unsigned long long run = s[threadIdx.x] - local;
-	for (long long b = b0; b < b1; b++) { unsigned long long c = block_sums[b]; block_sums[b] = run; run += c; }
-	if (threadIdx.x == 1023) *total = s[1023];
 }
 
 __global__ void __launch_bounds__(CGJ_THREADS)
@@ -321,7 +294,7 @@ cg_join_rows_emit_kernel(JoinRowsTable T, const long long *bpay, const long long
 	for (unsigned w = 0; w < warp; w++) pos += s_warp[w];
 	if (m == 0) return;
 	const long long key = keys[r];
-	const unsigned long long slot = join_rows_find(T, key, false);
+	const unsigned long long slot = key == CGJ_EMPTY ? T.cap : join_find<FIND>(T.keys, T.cap, T.shift, key);
 	const long long y = ppay[r];
 	for (long long b = T.head[slot]; b >= 0; b = T.next[b], pos++)
 		if (pos < capacity)
@@ -344,10 +317,7 @@ extern "C" int cg_join_rows(const int64_t *d_build_keys, const uint8_t *d_build_
 	*nrows = 0;
 	if (nbuild == 0 || nprobe == 0) return CG_OK;
 	JoinRowsTable T;
-	T.cap = 1024;
-	while (T.cap < 2ull * (uint64_t) nbuild) T.cap <<= 1;
-	T.shift = 64;
-	for (unsigned long long c = T.cap; c > 1; c >>= 1) T.shift--;
+	join_table_size(nbuild, &T.cap, &T.shift);
 	const long long nblocks = (nprobe + CGJ_THREADS - 1) / CGJ_THREADS;
 	auto a16 = [](size_t x) { return (x + 63) & ~(size_t) 63; };
 	const size_t kb = a16((T.cap + 1) * 8), cb = a16((T.cap + 1) * 4), hb = a16((T.cap + 1) * 8), nb = a16((size_t) nbuild * 8),
@@ -373,8 +343,8 @@ extern "C" int cg_join_rows(const int64_t *d_build_keys, const uint8_t *d_build_
 	cg_join_rows_count_kernel<<<(unsigned) nblocks, CGJ_THREADS, 0, ctx->compute>>>(T, (const long long *) d_probe_keys, d_probe_nulls, (long long) nprobe,
 																				  d_matches, d_block);
 	CG_CUDA(cudaGetLastError()); g_cg_launches++;
-	cg_join_rows_scan_kernel<<<1, 1024, 0, ctx->compute>>>(d_block, nblocks, d_tot);
-	CG_CUDA(cudaGetLastError()); g_cg_launches++;
+	CgAsyncBuf chunk_buf;
+	if (int rc = partition_scan_blocks(ctx, d_block, d_tot, nblocks, 1, &chunk_buf)) return rc;
 	unsigned long long h[2] = {0, 0};
 	CG_CUDA(cudaMemcpyAsync(h, d_tot, sizeof h, cudaMemcpyDeviceToHost, ctx->compute));
 	CG_CUDA(cudaStreamSynchronize(ctx->compute));

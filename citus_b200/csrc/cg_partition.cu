@@ -20,6 +20,7 @@
  * reference goldens through the oracle (tests/test_oracle_golden.py).
  */
 #include <algorithm>
+#include <initializer_list>
 #include <vector>
 
 #include "cg_internal.h"
@@ -53,177 +54,21 @@ __device__ __forceinline__ int32_t hashint8_dev(int64_t v)
 	return (int32_t) hash_bytes_uint32(lo);
 }
 
-struct PartParams
-{
-	const int64_t *keys;
-	const uint8_t *nulls;
-	int64_t n;
-	int32_t key_len;
-	int32_t by_hash;
-	int32_t P;
-	const int32_t *mins;   /* device */
-	const int32_t *maxs;
-	int32_t *index;
-	unsigned long long *counts;        /* [P] */
-	unsigned long long *block_counts;  /* [nblocks][P] (may be NULL) */
-	unsigned long long *errors;
-};
-
-__global__ void __launch_bounds__(CGP_THREADS)
-cg_partition_index_kernel(const __grid_constant__ PartParams A)
-{
-	extern __shared__ unsigned int s_count[];   /* [P] counts, then [P] mins, [P] maxs */
-	int32_t *s_min = (int32_t *) (s_count + A.P);
-	int32_t *s_max = s_min + A.P;
-	for (int p = threadIdx.x; p < A.P; p += CGP_THREADS)
-	{
-		s_count[p] = 0;
-		s_min[p] = A.mins[p];
-		s_max[p] = A.maxs[p];
-	}
-	__syncthreads();
-	int64_t base = (int64_t) blockIdx.x * CGP_ROWS_PER_BLOCK;
-	for (int i = threadIdx.x; i < CGP_ROWS_PER_BLOCK; i += CGP_THREADS)
-	{
-		int64_t r = base + i;
-		if (r >= A.n) break;
-		int idx;
-		if (A.nulls && A.nulls[r]) idx = 0;
-		else
-		{
-			int64_t k = A.keys[r];
-			/* range partitioning compares the key itself: an int8 key outside the int4 interval bounds lies in no
-			 * interval ("could not find shard"), it must not be truncated into one */
-			int64_t searched = A.by_hash ? (int64_t) (A.key_len == 4 ? (int32_t) hash_bytes_uint32((uint32_t) (int32_t) k) : hashint8_dev(k))
-										 : (A.key_len == 4 ? (int64_t) (int32_t) k : k);
-			/* SearchCachedShardInterval */
-			int lower = 0, upper = A.P;
-			idx = -1;
-			while (lower < upper)
-			{
-				int middle = (lower + upper) / 2;
-				if (searched < s_min[middle]) { upper = middle; continue; }
-				if (searched <= s_max[middle]) { idx = middle; break; }
-				lower = middle + 1;
-			}
-			if (idx < 0)
-			{
-				atomicAdd(A.errors, 1ull);   /* "could not find shard for partition column value" */
-				idx = 0;
-			}
-		}
-		A.index[r] = idx;
-		atomicAdd(&s_count[idx], 1u);
-	}
-	__syncthreads();
-	for (int p = threadIdx.x; p < A.P; p += CGP_THREADS)
-	{
-		unsigned int c = s_count[p];
-		if (A.block_counts) A.block_counts[(uint64_t) blockIdx.x * A.P + p] = c;
-		if (c) atomicAdd(A.counts + p, (unsigned long long) c);
-	}
-}
-
-/* exclusive scan over blocks, per partition: block_counts[b][p] -> start offset of block b inside
- * partition p (plus the partition's base).  P threads, sequential over blocks (nblocks ~ n/4096). */
-__global__ void cg_partition_scan_kernel(unsigned long long *block_counts, const unsigned long long *part_base,
-										 int64_t nblocks, int P)
-{
-	int p = blockIdx.x * blockDim.x + threadIdx.x;
-	if (p >= P) return;
-	unsigned long long run = part_base[p];
-	for (int64_t b = 0; b < nblocks; b++)
-	{
-		unsigned long long c = block_counts[b * P + p];
-		block_counts[b * P + p] = run;
-		run += c;
-	}
-}
-
-struct ScatterParams
-{
-	const int32_t *index;
-	int64_t n;
-	int32_t P;
-	int32_t ncols;
-	const unsigned long long *block_offsets;   /* [nblocks][P]: start of the block inside its partition */
-	const unsigned long long *part_base;       /* [P]: start of the partition in the output */
-	const int32_t *order;                      /* [P] output position of partition p, or NULL (identity) */
-	const int64_t *cols[8];
-	int64_t *out[8];
-};
-
 /*
- * Stable scatter.  A block owns 4096 consecutive rows, each of its 8 warps a contiguous
- * segment of 512.  Pass A: every warp histograms its segment into its own row of shared
- * memory (match.any groups the lanes of a step by partition; the group's first lane adds the
- * group size -- the row is warp-private, no atomics).  One barrier, then the per-(warp,
- * partition) start offsets = block offset + counts of the warps before.  Pass B: every warp
- * walks its segment again in input order; a row's destination is its partition's running
- * offset + its rank among the lanes of the same partition in this step.  Output order inside
- * a partition therefore equals input order, like the reference's append-to-file loop
- * (executor/partitioned_intermediate_results.c:493-553), with two block barriers in total.
- */
-__global__ void __launch_bounds__(CGP_THREADS)
-cg_partition_scatter_kernel(const __grid_constant__ ScatterParams A)
-{
-	extern __shared__ unsigned long long s_off[];     /* [warps][P] running destination offsets */
-	constexpr int WARPS = CGP_THREADS / 32;
-	constexpr int SEG = CGP_ROWS_PER_BLOCK / WARPS;
-	const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-	unsigned long long *mine = s_off + warp * A.P;
-	for (int p = lane; p < A.P; p += 32) mine[p] = 0;
-	__syncwarp();
-	const int64_t seg0 = (int64_t) blockIdx.x * CGP_ROWS_PER_BLOCK + (int64_t) warp * SEG;
-	/* pass A: segment histogram */
-	for (int step = 0; step < SEG; step += 32)
-	{
-		int64_t r = seg0 + step + lane;
-		int idx = r < A.n ? A.index[r] : -1;
-		if (idx >= 0 && A.order) idx = A.order[idx];
-		unsigned peers = __match_any_sync(0xffffffffu, idx);
-		if (idx >= 0 && lane == (unsigned) (__ffs(peers) - 1)) mine[idx] += __popc(peers);
-		__syncwarp();
-	}
-	__syncthreads();
-	/* counts -> start offsets: thread (p) walks the warps in order */
-	for (int p = threadIdx.x; p < A.P; p += CGP_THREADS)
-	{
-		unsigned long long run = A.part_base[p] + A.block_offsets[(uint64_t) blockIdx.x * A.P + p];
-		for (int w = 0; w < WARPS; w++)
-		{
-			unsigned long long c = s_off[w * A.P + p];
-			s_off[w * A.P + p] = run;
-			run += c;
-		}
-	}
-	__syncthreads();
-	/* pass B: scatter in input order */
-	for (int step = 0; step < SEG; step += 32)
-	{
-		int64_t r = seg0 + step + lane;
-		int idx = r < A.n ? A.index[r] : -1;
-		if (idx >= 0 && A.order) idx = A.order[idx];
-		unsigned peers = __match_any_sync(0xffffffffu, idx);
-		if (idx >= 0)
-		{
-			unsigned long long dst = mine[idx] + __popc(peers & ((1u << lane) - 1u));
-			for (int c = 0; c < A.ncols; c++) A.out[c][dst] = A.cols[c][r];
-		}
-		__syncwarp();
-		if (idx >= 0 && lane == (unsigned) (__ffs(peers) - 1)) mine[idx] += __popc(peers);
-		__syncwarp();
-	}
-}
-
-/*
- * The scatter the repartition uses.  Same stable order as above, built for instruction count (both kernels of the first
- * version were issue-bound):
+ * Routing and the stable scatter the repartition uses, built for instruction count (the scatter is issue-bound):
  *   routing   hashint4/8, then -- when the intervals are the uniform ones the planner generates
  *             (GenerateSyntheticShardIntervalArray, planner/multi_physical_planner.c:4667-4701) -- the reference's own
  *             shortcut CalculateUniformHashRangeIndex (utils/shardinterval_utils.c:424-452): (hash - INT32_MIN) / increment,
  *             a shift when P is a power of two; the interval search only for arbitrary bounds.  Done ONCE, in the histogram
  *             pass, which leaves a 2-byte partition number per row for the scatter pass.
+ *   order     a block owns 4096 consecutive rows, each of its 8 warps a contiguous segment of 512.  Pass A: every warp
+ *             histograms its segment into its own row of shared memory (match.any groups the lanes of a step by
+ *             partition; the group's first lane adds the group size -- the row is warp-private, no atomics).  One
+ *             barrier, then the per-(warp, partition) start offsets = block offset + counts of the warps before.  Pass B:
+ *             every warp walks its segment again in input order; a row's destination is its partition's running offset +
+ *             its rank among the lanes of the same partition in this step.  Output order inside a partition therefore
+ *             equals input order, like the reference's append-to-file loop
+ *             (executor/partitioned_intermediate_results.c:493-553).
  *   ranks     one match.any per row (pass A); its rank and group size travel to pass B in a register
  *   output    rows are placed in partition order in shared memory and leave as runs (a block's rows of one partition are
  *             contiguous in the output): coalesced stores; the partition of a local position is a 2-byte lookup
@@ -262,8 +107,11 @@ __device__ __forceinline__ int route_row(const RouteParams &R, const int32_t *s_
 		const uint32_t idx = R.uniform_shift >= 0 ? (u >> R.uniform_shift) : (u / R.uniform_inc);
 		return (int) (idx < (uint32_t) P ? idx : (uint32_t) P - 1u);           /* the last interval is widened to INT32_MAX */
 	}
+	/* range partitioning compares the key itself: an int8 key outside the int4 interval bounds lies in no interval ("could
+	 * not find shard"), it must not be truncated into one */
 	const int64_t searched = R.by_hash ? (int64_t) (R.key_len == 4 ? (int32_t) hash_bytes_uint32((uint32_t) (int32_t) k) : hashint8_dev(k))
 									   : (R.key_len == 4 ? (int64_t) (int32_t) k : k);
+	/* SearchCachedShardInterval */
 	int lower = 0, upper = P;
 	while (lower < upper)
 	{
@@ -309,6 +157,39 @@ cg_route_hist_kernel(const RouteParams R, int64_t n, int P, const int32_t *order
 	{
 		const unsigned int c = s_hist[s_ord[p]];
 		block_counts[(uint64_t) blockIdx.x * P + s_ord[p]] = c;
+		if (c) atomicAdd(counts + p, (unsigned long long) c);
+	}
+}
+
+/* routing for caller arrays (cg_partition_index): index[r] = the row's partition, counts[p], errors */
+__global__ void __launch_bounds__(CGP_THREADS)
+cg_partition_index_kernel(const RouteParams R, int64_t n, int P, int32_t *index, unsigned long long *counts, unsigned long long *errors)
+{
+	extern __shared__ unsigned int s_count[];     /* [P] counts, [P] mins, [P] maxs */
+	int32_t *s_min = (int32_t *) (s_count + P), *s_max = s_min + P;
+	for (int p = threadIdx.x; p < P; p += CGP_THREADS)
+	{
+		s_count[p] = 0;
+		if (!R.uniform_inc || !R.by_hash) { s_min[p] = R.mins[p]; s_max[p] = R.maxs[p]; }
+	}
+	__syncthreads();
+	const int64_t base = (int64_t) blockIdx.x * CGP_ROWS_PER_BLOCK;
+	unsigned int nbad = 0;
+	for (int i = threadIdx.x; i < CGP_ROWS_PER_BLOCK; i += CGP_THREADS)
+	{
+		int64_t r = base + i;
+		if (r >= n) break;
+		bool bad = false;
+		const int idx = route_row(R, s_min, s_max, P, r, &bad);
+		index[r] = idx;
+		atomicAdd(&s_count[idx], 1u);
+		nbad += bad ? 1u : 0u;
+	}
+	if (nbad) atomicAdd(errors, (unsigned long long) nbad);
+	__syncthreads();
+	for (int p = threadIdx.x; p < P; p += CGP_THREADS)
+	{
+		const unsigned int c = s_count[p];
 		if (c) atomicAdd(counts + p, (unsigned long long) c);
 	}
 }
@@ -456,57 +337,38 @@ static void detect_uniform(const int32_t *mins, const int32_t *maxs, int P, Rout
 	for (int sft = 0; sft < 32; sft++) if ((1ull << sft) == inc) R->uniform_shift = sft;
 }
 
-static int32_t *g_d_bounds = nullptr;
-static int g_bounds_cap = 0;
-
-static int partition_index_enqueue(CgContext *ctx, const int64_t *d_keys, const uint8_t *d_nulls, int64_t n, int32_t key_len,
-								   int32_t by_hash, const int32_t *mins, const int32_t *maxs, int32_t P, int32_t *d_index,
-								   int64_t *d_counts, unsigned long long *d_err)
+/*
+ * A few kilobytes of host data for the kernels that follow on the compute stream: interval bounds, partition order, the
+ * serializer's file layout.  They go through one pinned bounce buffer -- a pageable source would make the copy
+ * synchronous -- into one device buffer.  The device buffer is reused in stream order, the bounce buffer once the
+ * previous upload's copy has run.  d[i] receives the device address of host[i].
+ */
+struct HostArray
 {
-	if (P <= 0) return cg_set_error(CG_EINVAL, "number of partitions cannot be 0");
-	if (P > CGP_MAX_P) return cg_set_error(CG_EUNSUPPORTED, "more than %d partitions", CGP_MAX_P);
-	if (key_len != 4 && key_len != 8) return cg_set_error(CG_EINVAL, "key_len must be 4 or 8");
-	if (n < 0 || (n > 0 && !d_keys) || !d_index || !d_counts || !mins || !maxs) return cg_set_error(CG_EINVAL, "bad argument");
-	if (g_bounds_cap < 2 * P + 2)
+	const void *data;
+	size_t bytes;
+};
+#define CGP_UPLOAD_BYTES ((3 * sizeof(unsigned long long) + 1) * CGP_MAX_P + 64)
+
+static int upload_small(CgContext *ctx, std::initializer_list<HostArray> host, const void **d)
+{
+	static uint8_t *h_pin = nullptr, *d_buf = nullptr;
+	static cudaEvent_t pin_free = nullptr;
+	if (!h_pin) CG_CUDA(cudaHostAlloc((void **) &h_pin, CGP_UPLOAD_BYTES, cudaHostAllocDefault));
+	if (!d_buf) CG_CUDA(cudaMalloc((void **) &d_buf, CGP_UPLOAD_BYTES));
+	if (!pin_free) CG_CUDA(cudaEventCreateWithFlags(&pin_free, cudaEventDisableTiming));
+	CG_CUDA(cudaEventSynchronize(pin_free));
+	size_t off = 0;
+	for (const HostArray &a : host)
 	{
-		cudaFree(g_d_bounds);
-		CG_CUDA(cudaMalloc(&g_d_bounds, sizeof(int32_t) * (2 * CGP_MAX_P + 2)));
-		g_bounds_cap = 2 * CGP_MAX_P + 2;
+		if (off + a.bytes > CGP_UPLOAD_BYTES) return cg_set_error(CG_EINVAL, "%zu bytes of host arrays exceed the upload buffer", off + a.bytes);
+		memcpy(h_pin + off, a.data, a.bytes);
+		*d++ = d_buf + off;
+		off += (a.bytes + 15) & ~(size_t) 15;
 	}
-	/* the interval bounds go through a pinned bounce buffer: a pageable source would make the copy synchronous */
-	static int32_t *h_bounds = nullptr;
-	if (!h_bounds) CG_CUDA(cudaHostAlloc((void **) &h_bounds, sizeof(int32_t) * 2 * CGP_MAX_P, cudaHostAllocDefault));
-	static cudaEvent_t bounds_free = nullptr;
-	if (!bounds_free) CG_CUDA(cudaEventCreateWithFlags(&bounds_free, cudaEventDisableTiming));
-	CG_CUDA(cudaEventSynchronize(bounds_free));
-	memcpy(h_bounds, mins, sizeof(int32_t) * P);
-	memcpy(h_bounds + CGP_MAX_P, maxs, sizeof(int32_t) * P);
-	CG_CUDA(cudaMemcpyAsync(g_d_bounds, h_bounds, sizeof(int32_t) * P, cudaMemcpyHostToDevice, ctx->compute));
-	CG_CUDA(cudaMemcpyAsync(g_d_bounds + CGP_MAX_P, h_bounds + CGP_MAX_P, sizeof(int32_t) * P, cudaMemcpyHostToDevice, ctx->compute));
-	CG_CUDA(cudaEventRecord(bounds_free, ctx->compute));
-	CG_CUDA(cudaMemsetAsync(d_err, 0, sizeof(unsigned long long), ctx->compute));
-	CG_CUDA(cudaMemsetAsync(d_counts, 0, sizeof(int64_t) * P, ctx->compute));
-	if (n > 0)
-	{
-		PartParams A;
-		A.keys = d_keys; A.nulls = d_nulls; A.n = n; A.key_len = key_len; A.by_hash = by_hash; A.P = P;
-		A.mins = g_d_bounds; A.maxs = g_d_bounds + CGP_MAX_P; A.index = d_index;
-		A.counts = (unsigned long long *) d_counts; A.block_counts = nullptr; A.errors = d_err;
-		int64_t nblocks = (n + CGP_ROWS_PER_BLOCK - 1) / CGP_ROWS_PER_BLOCK;
-		cg_partition_index_kernel<<<(unsigned) nblocks, CGP_THREADS, 3 * P * sizeof(int32_t), ctx->compute>>>(A);
-		CG_CUDA(cudaGetLastError()); g_cg_launches++;
-	}
+	CG_CUDA(cudaMemcpyAsync(d_buf, h_pin, off, cudaMemcpyHostToDevice, ctx->compute));
+	CG_CUDA(cudaEventRecord(pin_free, ctx->compute));
 	return CG_OK;
-}
-
-int cg_partition_index_async(const int64_t *d_keys, const uint8_t *d_nulls, int64_t n, int32_t key_len, int32_t by_hash,
-							 const int32_t *mins, const int32_t *maxs, int32_t P, int32_t *d_index, int64_t *d_counts)
-{
-	CgContext *ctx = cg_ctx();
-	if (!ctx) return CG_EINVAL;
-	if (int rc0 = cg_chain_end(ctx, ctx->compute)) return rc0;
-	return partition_index_enqueue(ctx, d_keys, d_nulls, n, key_len, by_hash, mins, maxs, P, d_index, d_counts,
-								   (unsigned long long *) (d_counts + P));
 }
 
 extern "C" int cg_partition_index(const int64_t *d_keys, const uint8_t *d_nulls, int64_t n, int32_t key_len,
@@ -516,11 +378,27 @@ extern "C" int cg_partition_index(const int64_t *d_keys, const uint8_t *d_nulls,
 	CgContext *ctx = cg_ctx();
 	if (!ctx) return CG_EINVAL;
 	if (int rc0 = cg_chain_end(ctx, ctx->compute)) return rc0;
+	if (P <= 0) return cg_set_error(CG_EINVAL, "number of partitions cannot be 0");
+	if (P > CGP_MAX_P) return cg_set_error(CG_EUNSUPPORTED, "more than %d partitions", CGP_MAX_P);
+	if (key_len != 4 && key_len != 8) return cg_set_error(CG_EINVAL, "key_len must be 4 or 8");
+	if (n < 0 || (n > 0 && !d_keys) || !d_index || !d_counts || !mins || !maxs) return cg_set_error(CG_EINVAL, "bad argument");
 	CgAsyncBuf err_buf;
 	CG_CUDA(err_buf.alloc(sizeof(unsigned long long), ctx->compute));
 	unsigned long long *d_err = err_buf.as<unsigned long long>();
-	int rc = partition_index_enqueue(ctx, d_keys, d_nulls, n, key_len, by_hash, mins, maxs, P, d_index, d_counts, d_err);
-	if (rc) return rc;
+	RouteParams R = {d_keys, d_nulls, key_len, by_hash};
+	const void *d[2];
+	if (int rc = upload_small(ctx, {{mins, sizeof(int32_t) * P}, {maxs, sizeof(int32_t) * P}}, d)) return rc;
+	R.mins = (const int32_t *) d[0]; R.maxs = (const int32_t *) d[1];
+	detect_uniform(mins, maxs, P, &R);
+	CG_CUDA(cudaMemsetAsync(d_err, 0, sizeof(unsigned long long), ctx->compute));
+	CG_CUDA(cudaMemsetAsync(d_counts, 0, sizeof(int64_t) * P, ctx->compute));
+	if (n > 0)
+	{
+		int64_t nblocks = (n + CGP_ROWS_PER_BLOCK - 1) / CGP_ROWS_PER_BLOCK;
+		cg_partition_index_kernel<<<(unsigned) nblocks, CGP_THREADS, 3 * P * sizeof(int32_t), ctx->compute>>>(R, n, P, d_index,
+																											  (unsigned long long *) d_counts, d_err);
+		CG_CUDA(cudaGetLastError()); g_cg_launches++;
+	}
 	unsigned long long err = 0;
 	CG_CUDA(cudaMemcpyAsync(&err, d_err, sizeof err, cudaMemcpyDeviceToHost, ctx->compute));
 	CG_CUDA(cudaStreamSynchronize(ctx->compute));
@@ -528,40 +406,11 @@ extern "C" int cg_partition_index(const int64_t *d_keys, const uint8_t *d_nulls,
 	return CG_OK;
 }
 
-/* per-partition exclusive scan of the block counts (one CTA per partition): every thread sums a
- * contiguous run of blocks, the run sums are scanned in shared memory, then the run is rewritten as
- * offsets; the partition total goes to totals[p] */
-__global__ void __launch_bounds__(1024)
-cg_partition_scan2_kernel(unsigned long long *block_counts, unsigned long long *totals, int64_t nblocks, int P)
-{
-	__shared__ unsigned long long s_sum[1024];
-	const int p = blockIdx.x;
-	const int64_t per = (nblocks + 1023) / 1024;
-	const int64_t b0 = (int64_t) threadIdx.x * per, b1 = b0 + per < nblocks ? b0 + per : nblocks;
-	unsigned long long local = 0;
-	for (int64_t b = b0; b < b1; b++) local += block_counts[b * P + p];
-	s_sum[threadIdx.x] = local;
-	__syncthreads();
-	for (int off = 1; off < 1024; off <<= 1)
-	{
-		unsigned long long v = threadIdx.x >= (unsigned) off ? s_sum[threadIdx.x - off] : 0;
-		__syncthreads();
-		s_sum[threadIdx.x] += v;
-		__syncthreads();
-	}
-	unsigned long long run = s_sum[threadIdx.x] - local;
-	for (int64_t b = b0; b < b1; b++)
-	{
-		unsigned long long c = block_counts[b * P + p];
-		block_counts[b * P + p] = run;
-		run += c;
-	}
-	if (threadIdx.x == 1023) totals[p] = s_sum[1023];
-}
-
 /*
- * The same scan with all SMs: the blocks are cut into chunks of CGP_SCAN_CHUNK; pass 1 sums every (partition, chunk),
- * pass 2 scans the chunk sums of a partition (one warp) and yields its total, pass 3 rewrites every chunk as offsets.
+ * Per-partition exclusive scan of block counts with all SMs (declared in cg_internal.h): block_counts[b][p] becomes the
+ * start of block b inside partition p, totals[p] the partition's total.  The blocks are cut into chunks of CGP_SCAN_CHUNK;
+ * pass 1 sums every (partition, chunk), pass 2 scans the chunk sums of a partition (one thread) and yields its total,
+ * pass 3 rewrites every chunk as offsets.
  */
 #define CGP_SCAN_CHUNK 2048
 __global__ void __launch_bounds__(256)
@@ -621,7 +470,7 @@ cg_partition_scan_apply_kernel(unsigned long long *block_counts, const unsigned 
 	}
 }
 
-static int partition_scan_blocks(CgContext *ctx, unsigned long long *d_block, unsigned long long *d_tot, int64_t nblocks, int P, CgAsyncBuf *scratch)
+int partition_scan_blocks(CgContext *ctx, unsigned long long *d_block, unsigned long long *d_tot, int64_t nblocks, int P, CgAsyncBuf *scratch)
 {
 	const int nchunks = (int) ((nblocks + CGP_SCAN_CHUNK - 1) / CGP_SCAN_CHUNK);
 	CG_CUDA(scratch->alloc(sizeof(unsigned long long) * (size_t) P * (size_t) std::max(nchunks, 1), ctx->compute));
@@ -663,86 +512,6 @@ __global__ void cg_block_count_kernel(const int32_t *index, const int32_t *order
 	for (int p = threadIdx.x; p < P; p += CGP_THREADS) block_counts[(uint64_t) blockIdx.x * P + p] = s_count[p];
 }
 
-/* enqueues histogram -> scan -> scatter on the compute stream; *d_base_out (device, [P + 1], valid until the
- * scratch is returned to the pool in stream order) are the partition offsets in output order */
-static int partition_scatter_enqueue(CgContext *ctx, const int32_t *d_index, int64_t n, int32_t P, const int32_t *h_order,
-									 const int64_t *const *d_cols, int32_t ncols, int64_t *const *d_out, int64_t *h_offsets)
-{
-	if (P <= 0 || P > CGP_MAX_P) return cg_set_error(CG_EINVAL, "bad partition count %d", P);
-	if (ncols < 0 || ncols > 8) return cg_set_error(CG_EUNSUPPORTED, "at most 8 payload columns per call");
-	if (n < 0) return cg_set_error(CG_EINVAL, "negative row count");
-	if (h_order)
-	{
-		std::vector<uint8_t> seen(P, 0);
-		for (int p = 0; p < P; p++)
-		{
-			if (h_order[p] < 0 || h_order[p] >= P || seen[h_order[p]]) return cg_set_error(CG_EINVAL, "order is not a permutation");
-			seen[h_order[p]] = 1;
-		}
-	}
-	int64_t nblocks = (n + CGP_ROWS_PER_BLOCK - 1) / CGP_ROWS_PER_BLOCK;
-	CgAsyncBuf block_buf, tot_buf, order_buf, chunk_buf;
-	int32_t *d_order = nullptr;
-	CG_CUDA(block_buf.alloc(sizeof(unsigned long long) * (size_t) std::max<int64_t>(nblocks, 1) * P, ctx->compute));
-	CG_CUDA(tot_buf.alloc(sizeof(unsigned long long) * (2 * P + 1), ctx->compute));
-	unsigned long long *d_block = block_buf.as<unsigned long long>(), *d_tot = tot_buf.as<unsigned long long>();
-	unsigned long long *d_base = d_tot + P;
-	CG_CUDA(cudaMemsetAsync(d_tot, 0, sizeof(unsigned long long) * (2 * P + 1), ctx->compute));
-	if (h_order)
-	{
-		/* P ints as a kernel-argument-sized copy: through a pinned bounce buffer so that the copy is asynchronous */
-		static int32_t *h_pin = nullptr;
-		static cudaEvent_t pin_free = nullptr;
-		if (!h_pin) CG_CUDA(cudaHostAlloc((void **) &h_pin, sizeof(int32_t) * CGP_MAX_P, cudaHostAllocDefault));
-		if (!pin_free) CG_CUDA(cudaEventCreateWithFlags(&pin_free, cudaEventDisableTiming));
-		CG_CUDA(cudaEventSynchronize(pin_free));
-		memcpy(h_pin, h_order, sizeof(int32_t) * P);
-		CG_CUDA(order_buf.alloc(sizeof(int32_t) * P, ctx->compute));
-		d_order = order_buf.as<int32_t>();
-		CG_CUDA(cudaMemcpyAsync(d_order, h_pin, sizeof(int32_t) * P, cudaMemcpyHostToDevice, ctx->compute));
-		CG_CUDA(cudaEventRecord(pin_free, ctx->compute));
-	}
-	if (n > 0)
-	{
-		cg_block_count_kernel<<<(unsigned) nblocks, CGP_THREADS, P * sizeof(unsigned int), ctx->compute>>>(d_index, d_order, n, P, d_block);
-		CG_CUDA(cudaGetLastError()); g_cg_launches++;
-		int src_ = partition_scan_blocks(ctx, d_block, d_tot, nblocks, P, &chunk_buf);
-		if (src_) return src_;
-		cg_partition_base_kernel<<<1, 32, 0, ctx->compute>>>(d_tot, d_base, P);
-		CG_CUDA(cudaGetLastError()); g_cg_launches++;
-		StagedScatterParams S;
-		memset(&S, 0, sizeof S);
-		S.index = d_index; S.n = n; S.P = P; S.ncols = ncols; S.block_offsets = d_block; S.part_base = d_base; S.order = d_order;
-		for (int c = 0; c < ncols; c++) { S.cols[c] = d_cols[c]; S.out[c] = d_out[c]; }
-		static bool smem_configured = false;
-		if (!smem_configured)
-		{
-			CG_CUDA(cudaFuncSetAttribute(cg_scatter_staged_kernel<int32_t, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) staged_scatter_smem(CGP_MAX_P)));
-			smem_configured = true;
-		}
-		static const CgPeerScatter no_peer = {};
-		cg_scatter_staged_kernel<int32_t, false><<<(unsigned) nblocks, CGP_THREADS, staged_scatter_smem(P), ctx->compute>>>(S, no_peer);
-		CG_CUDA(cudaGetLastError()); g_cg_launches++;
-	}
-	if (h_offsets)
-	{
-		std::vector<unsigned long long> base(P + 1, 0);
-		CG_CUDA(cudaMemcpyAsync(base.data(), d_base, sizeof(unsigned long long) * (P + 1), cudaMemcpyDeviceToHost, ctx->compute));
-		CG_CUDA(cudaStreamSynchronize(ctx->compute));
-		for (int p = 0; p <= P; p++) h_offsets[p] = (int64_t) base[p];
-	}
-	return CG_OK;
-}
-
-int cg_partition_scatter_async(const int32_t *d_index, int64_t n, int32_t P, const int32_t *h_order, const int64_t *const *d_cols,
-							   int32_t ncols, int64_t *const *d_out)
-{
-	CgContext *ctx = cg_ctx();
-	if (!ctx) return CG_EINVAL;
-	if (int rc0 = cg_chain_end(ctx, ctx->compute)) return rc0;
-	return partition_scatter_enqueue(ctx, d_index, n, P, h_order, d_cols, ncols, d_out, nullptr);
-}
-
 /* routing + scatter without an index array (the repartition exchange): d_counts[P] rows per partition and d_counts[P] =
  * rows whose hash lies in no interval are ready on the compute stream after the first kernel; the caller records an
  * event between the two phases through `after_counts` */
@@ -757,39 +526,22 @@ int cg_partition_route_scatter_async(const int64_t *d_keys, const uint8_t *d_nul
 	if (P <= 0 || P > CGP_MAX_P) return cg_set_error(CG_EINVAL, "bad partition count %d", P);
 	if (key_len != 4 && key_len != 8) return cg_set_error(CG_EINVAL, "key_len must be 4 or 8");
 	if (ncols < 1 || ncols > 8 || n < 0 || !d_counts || !mins || !maxs || !h_order) return cg_set_error(CG_EINVAL, "bad argument");
-	if (g_bounds_cap < 2 * P + 2)
-	{
-		cudaFree(g_d_bounds);
-		CG_CUDA(cudaMalloc(&g_d_bounds, sizeof(int32_t) * (2 * CGP_MAX_P + 2)));
-		g_bounds_cap = 2 * CGP_MAX_P + 2;
-	}
-	/* interval bounds + output positions through a pinned bounce buffer (asynchronous copies) */
-	static int32_t *h_pin = nullptr;
-	static cudaEvent_t pin_free = nullptr;
-	if (!h_pin) CG_CUDA(cudaHostAlloc((void **) &h_pin, sizeof(int32_t) * 3 * CGP_MAX_P, cudaHostAllocDefault));
-	if (!pin_free) CG_CUDA(cudaEventCreateWithFlags(&pin_free, cudaEventDisableTiming));
-	CG_CUDA(cudaEventSynchronize(pin_free));
-	memcpy(h_pin, mins, sizeof(int32_t) * P);
-	memcpy(h_pin + CGP_MAX_P, maxs, sizeof(int32_t) * P);
-	memcpy(h_pin + 2 * CGP_MAX_P, h_order, sizeof(int32_t) * P);
 	const int64_t nblocks = (n + CGP_ROWS_PER_BLOCK - 1) / CGP_ROWS_PER_BLOCK;
-	CgAsyncBuf block_buf, tot_buf, order_buf, idx_buf, chunk_buf;
+	CgAsyncBuf block_buf, tot_buf, idx_buf, chunk_buf;
 	CG_CUDA(block_buf.alloc(sizeof(unsigned long long) * (size_t) std::max<int64_t>(nblocks, 1) * P, ctx->compute));
 	CG_CUDA(tot_buf.alloc(sizeof(unsigned long long) * (2 * P + 1), ctx->compute));
-	CG_CUDA(order_buf.alloc(sizeof(int32_t) * P, ctx->compute));
 	CG_CUDA(idx_buf.alloc(sizeof(uint16_t) * (size_t) std::max<int64_t>(n, 1), ctx->compute));
 	unsigned long long *d_block = block_buf.as<unsigned long long>(), *d_tot = tot_buf.as<unsigned long long>(), *d_base = d_tot + P;
-	int32_t *d_order = order_buf.as<int32_t>();
 	uint16_t *d_idx16 = idx_buf.as<uint16_t>();
-	CG_CUDA(cudaMemcpyAsync(g_d_bounds, h_pin, sizeof(int32_t) * P, cudaMemcpyHostToDevice, ctx->compute));
-	CG_CUDA(cudaMemcpyAsync(g_d_bounds + CGP_MAX_P, h_pin + CGP_MAX_P, sizeof(int32_t) * P, cudaMemcpyHostToDevice, ctx->compute));
-	CG_CUDA(cudaMemcpyAsync(d_order, h_pin + 2 * CGP_MAX_P, sizeof(int32_t) * P, cudaMemcpyHostToDevice, ctx->compute));
-	CG_CUDA(cudaEventRecord(pin_free, ctx->compute));
+	RouteParams R = {d_keys, d_nulls, key_len, by_hash};
+	const void *d[3];
+	const size_t pb = sizeof(int32_t) * P;
+	if (int rc = upload_small(ctx, {{mins, pb}, {maxs, pb}, {h_order, pb}}, d)) return rc;
+	R.mins = (const int32_t *) d[0]; R.maxs = (const int32_t *) d[1];
+	const int32_t *d_order = (const int32_t *) d[2];
+	detect_uniform(mins, maxs, P, &R);
 	CG_CUDA(cudaMemsetAsync(d_tot, 0, sizeof(unsigned long long) * (2 * P + 1), ctx->compute));
 	CG_CUDA(cudaMemsetAsync(d_counts, 0, sizeof(int64_t) * (P + 1), ctx->compute));
-	RouteParams R;
-	R.keys = d_keys; R.nulls = d_nulls; R.key_len = key_len; R.by_hash = by_hash; R.mins = g_d_bounds; R.maxs = g_d_bounds + CGP_MAX_P;
-	detect_uniform(mins, maxs, P, &R);
 	if (n > 0)
 	{
 		cg_route_hist_kernel<<<(unsigned) nblocks, CGP_THREADS, 4 * P * sizeof(int32_t), ctx->compute>>>(R, n, P, d_order, d_idx16, d_block,
@@ -847,7 +599,59 @@ extern "C" int cg_partition_scatter_ordered(const int32_t *d_index, int64_t n, i
 	if (!ctx) return CG_EINVAL;
 	if (int rc0 = cg_chain_end(ctx, ctx->compute)) return rc0;
 	if (!h_offsets) return cg_set_error(CG_EINVAL, "NULL offsets");
-	return partition_scatter_enqueue(ctx, d_index, n, P, h_order, d_cols, ncols, d_out, h_offsets);
+	if (P <= 0 || P > CGP_MAX_P) return cg_set_error(CG_EINVAL, "bad partition count %d", P);
+	if (ncols < 0 || ncols > 8) return cg_set_error(CG_EUNSUPPORTED, "at most 8 payload columns per call");
+	if (n < 0) return cg_set_error(CG_EINVAL, "negative row count");
+	if (h_order)
+	{
+		std::vector<uint8_t> seen(P, 0);
+		for (int p = 0; p < P; p++)
+		{
+			if (h_order[p] < 0 || h_order[p] >= P || seen[h_order[p]]) return cg_set_error(CG_EINVAL, "order is not a permutation");
+			seen[h_order[p]] = 1;
+		}
+	}
+	int64_t nblocks = (n + CGP_ROWS_PER_BLOCK - 1) / CGP_ROWS_PER_BLOCK;
+	CgAsyncBuf block_buf, tot_buf, chunk_buf;
+	CG_CUDA(block_buf.alloc(sizeof(unsigned long long) * (size_t) std::max<int64_t>(nblocks, 1) * P, ctx->compute));
+	CG_CUDA(tot_buf.alloc(sizeof(unsigned long long) * (2 * P + 1), ctx->compute));
+	unsigned long long *d_block = block_buf.as<unsigned long long>(), *d_tot = tot_buf.as<unsigned long long>();
+	unsigned long long *d_base = d_tot + P;
+	CG_CUDA(cudaMemsetAsync(d_tot, 0, sizeof(unsigned long long) * (2 * P + 1), ctx->compute));
+	const int32_t *d_order = nullptr;
+	if (h_order)
+	{
+		const void *d;
+		if (int rc = upload_small(ctx, {{h_order, sizeof(int32_t) * P}}, &d)) return rc;
+		d_order = (const int32_t *) d;
+	}
+	if (n > 0)
+	{
+		cg_block_count_kernel<<<(unsigned) nblocks, CGP_THREADS, P * sizeof(unsigned int), ctx->compute>>>(d_index, d_order, n, P, d_block);
+		CG_CUDA(cudaGetLastError()); g_cg_launches++;
+		int src_ = partition_scan_blocks(ctx, d_block, d_tot, nblocks, P, &chunk_buf);
+		if (src_) return src_;
+		cg_partition_base_kernel<<<1, 32, 0, ctx->compute>>>(d_tot, d_base, P);
+		CG_CUDA(cudaGetLastError()); g_cg_launches++;
+		StagedScatterParams S;
+		memset(&S, 0, sizeof S);
+		S.index = d_index; S.n = n; S.P = P; S.ncols = ncols; S.block_offsets = d_block; S.part_base = d_base; S.order = d_order;
+		for (int c = 0; c < ncols; c++) { S.cols[c] = d_cols[c]; S.out[c] = d_out[c]; }
+		static bool smem_configured = false;
+		if (!smem_configured)
+		{
+			CG_CUDA(cudaFuncSetAttribute(cg_scatter_staged_kernel<int32_t, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) staged_scatter_smem(CGP_MAX_P)));
+			smem_configured = true;
+		}
+		static const CgPeerScatter no_peer = {};
+		cg_scatter_staged_kernel<int32_t, false><<<(unsigned) nblocks, CGP_THREADS, staged_scatter_smem(P), ctx->compute>>>(S, no_peer);
+		CG_CUDA(cudaGetLastError()); g_cg_launches++;
+	}
+	std::vector<unsigned long long> base(P + 1, 0);
+	CG_CUDA(cudaMemcpyAsync(base.data(), d_base, sizeof(unsigned long long) * (P + 1), cudaMemcpyDeviceToHost, ctx->compute));
+	CG_CUDA(cudaStreamSynchronize(ctx->compute));
+	for (int p = 0; p <= P; p++) h_offsets[p] = (int64_t) base[p];
+	return CG_OK;
 }
 
 extern "C" int cg_partition_scatter(const int32_t *d_index, int64_t n, int32_t P, const int64_t *const *d_cols,
@@ -870,18 +674,6 @@ extern "C" int cg_partition_scatter(const int32_t *d_index, int64_t n, int32_t P
  *  never starts its receiver: 0 bytes.  The rows themselves stay on the GPU (NCCL instead of
  *  files); only these counters are computed.
  * ------------------------------------------------------------------------------ */
-struct CopyBytesParams
-{
-	const int32_t *index;
-	int64_t n;
-	int32_t P, ncols, binary;
-	const int64_t *cols[CGP_MAX_COLS];
-	const uint8_t *nulls[CGP_MAX_COLS];
-	int32_t len[CGP_MAX_COLS];
-	unsigned long long *bytes;     /* [P] */
-	unsigned long long *rows;      /* [P] */
-};
-
 __constant__ unsigned long long cg_pow10[20] = {1ull, 10ull, 100ull, 1000ull, 10000ull, 100000ull, 1000000ull, 10000000ull, 100000000ull,
 												1000000000ull, 10000000000ull, 100000000000ull, 1000000000000ull, 10000000000000ull,
 												100000000000000ull, 1000000000000000ull, 10000000000000000ull, 100000000000000000ull,
@@ -898,8 +690,47 @@ __device__ __forceinline__ unsigned int decimal_text_len(int64_t v)
 	return digits + (v < 0 ? 1u : 0u);
 }
 
+/* the rows of both COPY entry points (cg_partition_copy_bytes, cg_partition_copy_serialize); row_len and the fields
+ * after it are the serializer's */
+struct CopyParams
+{
+	const int32_t *index;
+	int64_t n;
+	int32_t P, ncols, binary;
+	const int64_t *cols[CGP_MAX_COLS];
+	const uint8_t *nulls[CGP_MAX_COLS];
+	int32_t len[CGP_MAX_COLS];
+	uint32_t *row_len;                         /* [n] */
+	unsigned long long *block_bytes;           /* [nblocks][P]: bytes of the block's rows per partition, then their start offsets */
+	const unsigned long long *file_start;      /* [P]: offset of the first ROW byte of partition p in the output */
+	uint8_t *out;
+};
+
+__device__ __forceinline__ unsigned int copy_row_len(const CopyParams &A, int64_t r)
+{
+	unsigned int b = A.binary ? 2u : 0u;
+	for (int c = 0; c < A.ncols; c++)
+	{
+		bool isnull = A.nulls[c] && A.nulls[c][r];
+		if (A.binary) b += 4u + (isnull ? 0u : (unsigned int) A.len[c]);
+		else b += 1u + (isnull ? 2u : decimal_text_len(A.cols[c][r]));
+	}
+	return b;
+}
+
+/* the row description from either COPY entry point's arguments */
+static CopyParams copy_params(const int32_t *d_index, int64_t n, int32_t P, const int64_t *const *d_cols, const uint8_t *const *d_nulls,
+							  const int32_t *col_len, int32_t ncols, int32_t binary)
+{
+	CopyParams A;
+	memset(&A, 0, sizeof A);
+	A.index = d_index; A.n = n; A.P = P; A.ncols = ncols; A.binary = binary ? 1 : 0;
+	for (int c = 0; c < ncols; c++) { A.cols[c] = d_cols[c]; A.nulls[c] = d_nulls ? d_nulls[c] : nullptr; A.len[c] = col_len[c]; }
+	return A;
+}
+
 __global__ void __launch_bounds__(CGP_THREADS)
-cg_partition_copy_bytes_kernel(const __grid_constant__ CopyBytesParams A)
+cg_partition_copy_bytes_kernel(const __grid_constant__ CopyParams A, unsigned long long *bytes, unsigned long long *rows)
 {
 	extern __shared__ unsigned int s_copy[];            /* [P] bytes, [P] rows of this block (< 2^32: 4096 rows) */
 	unsigned int *s_bytes = s_copy, *s_rows = s_copy + A.P;
@@ -910,15 +741,8 @@ cg_partition_copy_bytes_kernel(const __grid_constant__ CopyBytesParams A)
 	{
 		int64_t r = base + i;
 		if (r >= A.n) break;
-		unsigned int b = A.binary ? 2u : 0u;
-		for (int c = 0; c < A.ncols; c++)
-		{
-			bool isnull = A.nulls[c] && A.nulls[c][r];
-			if (A.binary) b += 4u + (isnull ? 0u : (unsigned int) A.len[c]);
-			else b += 1u + (isnull ? 2u : decimal_text_len(A.cols[c][r]));
-		}
 		int p = A.index[r];
-		atomicAdd(&s_bytes[p], b);
+		atomicAdd(&s_bytes[p], copy_row_len(A, r));
 		atomicAdd(&s_rows[p], 1u);
 	}
 	__syncthreads();
@@ -926,8 +750,8 @@ cg_partition_copy_bytes_kernel(const __grid_constant__ CopyBytesParams A)
 	{
 		if (s_rows[p])
 		{
-			atomicAdd(A.bytes + p, (unsigned long long) s_bytes[p]);
-			atomicAdd(A.rows + p, (unsigned long long) s_rows[p]);
+			atomicAdd(bytes + p, (unsigned long long) s_bytes[p]);
+			atomicAdd(rows + p, (unsigned long long) s_rows[p]);
 		}
 	}
 }
@@ -948,18 +772,9 @@ extern "C" int cg_partition_copy_bytes(const int32_t *d_index, int64_t n, int32_
 	CG_CUDA(cudaMemsetAsync(d_acc, 0, 2 * (size_t) P * sizeof(unsigned long long), ctx->compute));
 	if (n > 0)
 	{
-		CopyBytesParams A;
-		memset(&A, 0, sizeof A);
-		A.index = d_index; A.n = n; A.P = P; A.ncols = ncols; A.binary = binary ? 1 : 0;
-		for (int c = 0; c < ncols; c++)
-		{
-			A.cols[c] = d_cols[c];
-			A.nulls[c] = d_nulls ? d_nulls[c] : nullptr;
-			A.len[c] = col_len[c];
-		}
-		A.bytes = d_acc; A.rows = d_acc + P;
+		const CopyParams A = copy_params(d_index, n, P, d_cols, d_nulls, col_len, ncols, binary);
 		int64_t nblocks = (n + CGP_ROWS_PER_BLOCK - 1) / CGP_ROWS_PER_BLOCK;
-		cg_partition_copy_bytes_kernel<<<(unsigned) nblocks, CGP_THREADS, 2 * P * sizeof(unsigned int), ctx->compute>>>(A);
+		cg_partition_copy_bytes_kernel<<<(unsigned) nblocks, CGP_THREADS, 2 * P * sizeof(unsigned int), ctx->compute>>>(A, d_acc, d_acc + P);
 		CG_CUDA(cudaGetLastError()); g_cg_launches++;
 	}
 	std::vector<unsigned long long> h(2 * (size_t) P, 0);
@@ -982,39 +797,13 @@ extern "C" int cg_partition_copy_bytes(const int32_t *d_index, int64_t n, int32_
  *    text    fields separated by '\t', row ended by '\n', NULL as "\N", integers in decimal (pg_lltoa)
  *    binary  "PGCOPY\n\377\r\n\0" + int32 flags 0 + int32 extension length 0, then per row int16 field count and per
  *            field int32 length (-1 = NULL) + the value in network byte order, then int16 -1
- *  Here every row's byte length is known before anything is written (cg_partition_copy_bytes_kernel's arithmetic), so a
- *  row's place in its file is a segmented prefix sum in input order -- per block and partition (shared memory), across
- *  blocks (cg_partition_scan2_kernel), inside a warp step (peers of the same partition to the left) -- and all rows are
+ *  Here every row's byte length is known before anything is written (copy_row_len), so a row's place in its file is a
+ *  segmented prefix sum in input order -- per block and partition (shared memory), across blocks (partition_scan_blocks),
+ *  inside a warp step (peers of the same partition to the left) -- and all rows are
  *  formatted in parallel straight into one device buffer that holds the P files back to back.
  * ------------------------------------------------------------------------------ */
-struct CopyWriteParams
-{
-	const int32_t *index;
-	int64_t n;
-	int32_t P, ncols, binary;
-	const int64_t *cols[CGP_MAX_COLS];
-	const uint8_t *nulls[CGP_MAX_COLS];
-	int32_t len[CGP_MAX_COLS];
-	uint32_t *row_len;                         /* [n] */
-	unsigned long long *block_bytes;           /* [nblocks][P]: bytes of the block's rows per partition, then their start offsets */
-	const unsigned long long *file_start;      /* [P]: offset of the first ROW byte of partition p in the output */
-	uint8_t *out;
-};
-
-__device__ __forceinline__ unsigned int copy_row_len(const CopyWriteParams &A, int64_t r)
-{
-	unsigned int b = A.binary ? 2u : 0u;
-	for (int c = 0; c < A.ncols; c++)
-	{
-		bool isnull = A.nulls[c] && A.nulls[c][r];
-		if (A.binary) b += 4u + (isnull ? 0u : (unsigned int) A.len[c]);
-		else b += 1u + (isnull ? 2u : decimal_text_len(A.cols[c][r]));
-	}
-	return b;
-}
-
 __global__ void __launch_bounds__(CGP_THREADS)
-cg_copy_len_kernel(const __grid_constant__ CopyWriteParams A)
+cg_copy_len_kernel(const __grid_constant__ CopyParams A)
 {
 	extern __shared__ unsigned int s_bytes[];            /* [P] */
 	for (int p = threadIdx.x; p < A.P; p += CGP_THREADS) s_bytes[p] = 0;
@@ -1048,7 +837,7 @@ __device__ __forceinline__ uint8_t *put_decimal(uint8_t *p, int64_t v)
 }
 
 __global__ void __launch_bounds__(CGP_THREADS)
-cg_copy_write_kernel(const __grid_constant__ CopyWriteParams A)
+cg_copy_write_kernel(const __grid_constant__ CopyParams A)
 {
 	extern __shared__ unsigned long long s_run[];        /* [warps][P] running byte offsets */
 	constexpr int WARPS = CGP_THREADS / 32;
@@ -1148,26 +937,19 @@ extern "C" int cg_partition_copy_serialize(const int32_t *d_index, int64_t n, in
 	for (int c = 0; c < ncols; c++)
 		if (binary && col_len[c] != 2 && col_len[c] != 4 && col_len[c] != 8) return cg_set_error(CG_EUNSUPPORTED, "binary width %d", col_len[c]);
 	const int64_t nblocks = (n + CGP_ROWS_PER_BLOCK - 1) / CGP_ROWS_PER_BLOCK;
-	CgAsyncBuf len_buf, block_buf, tot_buf;
+	CgAsyncBuf len_buf, block_buf, tot_buf, chunk_buf;
 	CG_CUDA(len_buf.alloc(sizeof(uint32_t) * (size_t) std::max<int64_t>(n, 1), ctx->compute));
 	CG_CUDA(block_buf.alloc(sizeof(unsigned long long) * (size_t) std::max<int64_t>(nblocks, 1) * P, ctx->compute));
-	/* [P] totals, [P] row starts, [P] file begins, [P] file ends (8 bytes each), then present[P] (one byte each) */
-	const size_t tot_bytes = sizeof(unsigned long long) * 4 * (size_t) P + (size_t) P;
-	CG_CUDA(tot_buf.alloc(tot_bytes, ctx->compute));
+	CG_CUDA(tot_buf.alloc(sizeof(unsigned long long) * P, ctx->compute));
 	unsigned long long *d_tot = tot_buf.as<unsigned long long>();
-	CG_CUDA(cudaMemsetAsync(d_tot, 0, tot_bytes, ctx->compute));
-	CopyWriteParams A;
-	memset(&A, 0, sizeof A);
-	A.index = d_index; A.n = n; A.P = P; A.ncols = ncols; A.binary = binary ? 1 : 0;
-	for (int c = 0; c < ncols; c++) { A.cols[c] = d_cols[c]; A.nulls[c] = d_nulls ? d_nulls[c] : nullptr; A.len[c] = col_len[c]; }
+	CopyParams A = copy_params(d_index, n, P, d_cols, d_nulls, col_len, ncols, binary);
 	A.row_len = len_buf.as<uint32_t>(); A.block_bytes = block_buf.as<unsigned long long>(); A.out = d_out;
 	std::vector<unsigned long long> totals(P, 0);
 	if (n > 0)
 	{
 		cg_copy_len_kernel<<<(unsigned) nblocks, CGP_THREADS, P * sizeof(unsigned int), ctx->compute>>>(A);
 		CG_CUDA(cudaGetLastError()); g_cg_launches++;
-		cg_partition_scan2_kernel<<<P, 1024, 0, ctx->compute>>>(A.block_bytes, d_tot, nblocks, P);
-		CG_CUDA(cudaGetLastError()); g_cg_launches++;
+		if (int rc = partition_scan_blocks(ctx, A.block_bytes, d_tot, nblocks, P, &chunk_buf)) return rc;
 		CG_CUDA(cudaMemcpyAsync(totals.data(), d_tot, sizeof(unsigned long long) * P, cudaMemcpyDeviceToHost, ctx->compute));
 		CG_CUDA(cudaStreamSynchronize(ctx->compute));
 	}
@@ -1189,16 +971,12 @@ extern "C" int cg_partition_copy_serialize(const int32_t *d_index, int64_t n, in
 	if ((int64_t) off > out_capacity || (off > 0 && !d_out))
 		return cg_set_error(CG_EINVAL, "the partition files need %llu bytes, the output buffer holds %lld", off, (long long) out_capacity);
 	if (off == 0) return CG_OK;
-	unsigned long long *d_rows_at = d_tot + P, *d_begin = d_tot + 2 * P, *d_end = d_tot + 3 * P;
-	uint8_t *d_present = (uint8_t *) (d_tot + 4 * P);
-	static unsigned long long *h_pin = nullptr;
-	if (!h_pin) CG_CUDA(cudaHostAlloc((void **) &h_pin, sizeof(unsigned long long) * (4 * CGP_MAX_P + 4), cudaHostAllocDefault));
-	memcpy(h_pin, rows_at.data(), sizeof(unsigned long long) * P);
-	memcpy(h_pin + P, begin.data(), sizeof(unsigned long long) * P);
-	memcpy(h_pin + 2 * P, end.data(), sizeof(unsigned long long) * P);
-	memcpy(h_pin + 3 * P, present.data(), (size_t) P);
-	CG_CUDA(cudaMemcpyAsync(d_rows_at, h_pin, sizeof(unsigned long long) * 3 * P + (size_t) P, cudaMemcpyHostToDevice, ctx->compute));
-	A.file_start = d_rows_at;
+	const size_t pb = sizeof(unsigned long long) * P;
+	const void *d[4];
+	if (int rc = upload_small(ctx, {{rows_at.data(), pb}, {begin.data(), pb}, {end.data(), pb}, {present.data(), (size_t) P}}, d)) return rc;
+	A.file_start = (const unsigned long long *) d[0];
+	const unsigned long long *d_begin = (const unsigned long long *) d[1], *d_end = (const unsigned long long *) d[2];
+	const uint8_t *d_present = (const uint8_t *) d[3];
 	if (n > 0)
 	{
 		static bool smem_configured = false;

@@ -690,14 +690,16 @@ def test_copy_many_partitions(cg, P, binary, gen_empty):
 
 
 def test_copy_five_million_rows(cg):
-    """5M rows = 1221 blocks: cg_partition_scan2_kernel gives every thread a run of two blocks"""
+    """5M rows = 1221 blocks of 4096 rows: the block offset scan in one chunk of 2048 blocks; 9M rows = 2198 blocks: the
+    offsets of the second chunk carry the first chunk's bytes"""
     rng = np.random.default_rng(5)
-    n, P = 5_000_000, 3
-    index = rng.integers(0, P, n)
-    k = rng.integers(pr.INT64_MIN, pr.INT64_MAX, n, dtype=np.int64, endpoint=True)
-    a = rng.integers(-1000, 1000, n)
-    for binary in (False, True):
-        _check_files(index, [k, a], [8, 4], P, binary)
+    P = 3
+    for n in (5_000_000, 9_000_000):
+        index = rng.integers(0, P, n)
+        k = rng.integers(pr.INT64_MIN, pr.INT64_MAX, n, dtype=np.int64, endpoint=True)
+        a = rng.integers(-1000, 1000, n)
+        for binary in (False, True):
+            _check_files(index, [k, a], [8, 4], P, binary)
 
 
 @pytest.mark.parametrize("binary", [False, True])

@@ -913,47 +913,49 @@ def test_varlena_columns_with_nulls_wide_values_and_bad_scale(cg, oracle):
 def test_join_rows_matches_a_row_at_a_time_join(cg, oracle):
     """cg_join_rows: the merge-side join emitting (key, b.payload, p.payload) rows -- the multiset of rows equals a
     nested-loop join on the host (duplicates on both sides, NULL keys join nothing, the key equal to the table's EMPTY
-    sentinel, an empty side, capacity handling)"""
+    sentinel, an empty side, capacity handling).  600 000 probe rows are 2344 blocks of 256: the offsets of the second
+    scan chunk of 2048 blocks carry the first chunk's rows"""
     import torch
     from collections import Counter
     from citus_b200 import capi
     rng = np.random.default_rng(12)
-    nb, npr = 30_000, 50_000
-    bk = rng.integers(0, 5000, nb); bk[:3] = -2**63
-    pk = rng.integers(0, 6000, npr); pk[:2] = -2**63
-    bx = rng.integers(-2**40, 2**40, nb)
-    py = rng.integers(-2**40, 2**40, npr)
-    bn = (rng.random(nb) < 0.05).astype(np.uint8)
-    pn = (rng.random(npr) < 0.05).astype(np.uint8)
-    d = [torch.from_numpy(x).cuda() for x in (bk, bx, pk, py)]
-    dbn, dpn = torch.from_numpy(bn).cuda(), torch.from_numpy(pn).cuda()
-    n = cg.join_rows(d[0].data_ptr(), d[1].data_ptr(), nb, d[2].data_ptr(), d[3].data_ptr(), npr,
-                     d_build_nulls=dbn.data_ptr(), d_probe_nulls=dpn.data_ptr())
-    joined, jsum = cg.join_count_sum(d[0].data_ptr(), d[1].data_ptr(), nb, d[2].data_ptr(), d[3].data_ptr(), npr,
-                                     d_build_nulls=dbn.data_ptr(), d_probe_nulls=dpn.data_ptr())
-    wj, ws = oracle.join_count_sum(bk, bx, pk, py, bn, pn)
-    assert n == joined == wj and jsum == ws
-    out = [torch.empty(n, dtype=torch.int64, device="cuda") for _ in range(3)]
-    n2 = cg.join_rows(d[0].data_ptr(), d[1].data_ptr(), nb, d[2].data_ptr(), d[3].data_ptr(), npr, capacity=n,
-                      d_out=[o.data_ptr() for o in out], d_build_nulls=dbn.data_ptr(), d_probe_nulls=dpn.data_ptr())
-    assert n2 == n
-    got = Counter(zip(*(o.cpu().tolist() for o in out)))
-    by_key = {}
-    for k, x, z in zip(bk.tolist(), bx.tolist(), bn.tolist()):
-        if not z:
-            by_key.setdefault(k, []).append(x)
-    want = Counter()
-    for k, y, z in zip(pk.tolist(), py.tolist(), pn.tolist()):
-        if not z:
-            for x in by_key.get(k, ()):
-                want[(k, x, y)] += 1
-    assert got == want
-    # the emitted rows add up to the aggregate form's sum
-    assert int((out[1].cpu().numpy().astype(object) + out[2].cpu().numpy().astype(object)).sum()) == ws
-    with pytest.raises(capi.CitusGpuError):
-        cg.join_rows(d[0].data_ptr(), d[1].data_ptr(), nb, d[2].data_ptr(), d[3].data_ptr(), npr, capacity=n - 1,
-                     d_out=[o.data_ptr() for o in out], d_build_nulls=dbn.data_ptr(), d_probe_nulls=dpn.data_ptr())
-    assert cg.join_rows(d[0].data_ptr(), d[1].data_ptr(), 0, d[2].data_ptr(), d[3].data_ptr(), npr) == 0
+    nb = 30_000
+    for npr, pkeys in ((50_000, 6000), (600_000, 60_000)):
+        bk = rng.integers(0, 5000, nb); bk[:3] = -2**63
+        pk = rng.integers(0, pkeys, npr); pk[:2] = -2**63
+        bx = rng.integers(-2**40, 2**40, nb)
+        py = rng.integers(-2**40, 2**40, npr)
+        bn = (rng.random(nb) < 0.05).astype(np.uint8)
+        pn = (rng.random(npr) < 0.05).astype(np.uint8)
+        d = [torch.from_numpy(x).cuda() for x in (bk, bx, pk, py)]
+        dbn, dpn = torch.from_numpy(bn).cuda(), torch.from_numpy(pn).cuda()
+        n = cg.join_rows(d[0].data_ptr(), d[1].data_ptr(), nb, d[2].data_ptr(), d[3].data_ptr(), npr,
+                         d_build_nulls=dbn.data_ptr(), d_probe_nulls=dpn.data_ptr())
+        joined, jsum = cg.join_count_sum(d[0].data_ptr(), d[1].data_ptr(), nb, d[2].data_ptr(), d[3].data_ptr(), npr,
+                                         d_build_nulls=dbn.data_ptr(), d_probe_nulls=dpn.data_ptr())
+        wj, ws = oracle.join_count_sum(bk, bx, pk, py, bn, pn)
+        assert n == joined == wj and jsum == ws
+        out = [torch.empty(n, dtype=torch.int64, device="cuda") for _ in range(3)]
+        n2 = cg.join_rows(d[0].data_ptr(), d[1].data_ptr(), nb, d[2].data_ptr(), d[3].data_ptr(), npr, capacity=n,
+                          d_out=[o.data_ptr() for o in out], d_build_nulls=dbn.data_ptr(), d_probe_nulls=dpn.data_ptr())
+        assert n2 == n
+        got = Counter(zip(*(o.cpu().tolist() for o in out)))
+        by_key = {}
+        for k, x, z in zip(bk.tolist(), bx.tolist(), bn.tolist()):
+            if not z:
+                by_key.setdefault(k, []).append(x)
+        want = Counter()
+        for k, y, z in zip(pk.tolist(), py.tolist(), pn.tolist()):
+            if not z:
+                for x in by_key.get(k, ()):
+                    want[(k, x, y)] += 1
+        assert got == want
+        # the emitted rows add up to the aggregate form's sum
+        assert int((out[1].cpu().numpy().astype(object) + out[2].cpu().numpy().astype(object)).sum()) == ws
+        with pytest.raises(capi.CitusGpuError):
+            cg.join_rows(d[0].data_ptr(), d[1].data_ptr(), nb, d[2].data_ptr(), d[3].data_ptr(), npr, capacity=n - 1,
+                         d_out=[o.data_ptr() for o in out], d_build_nulls=dbn.data_ptr(), d_probe_nulls=dpn.data_ptr())
+        assert cg.join_rows(d[0].data_ptr(), d[1].data_ptr(), 0, d[2].data_ptr(), d[3].data_ptr(), npr) == 0
 
 
 @pytest.mark.parametrize("tma", [1, 0])
