@@ -31,6 +31,7 @@ CG_MAX_QEXPR, CG_QX_AND, CG_QX_OR = 16, -1, -2
 CG_MAX_FILTER_QUALS = 8
 CG_MAX_WORDS = 32
 CG_MAX_IN_LISTS, CG_MAX_IN_VALUES, CG_IN_REFUTE_MAX = 8, 1024, 100
+CG_PSTATE_PACKED_DIRTY, CG_PSTATE_WIDE_DIRTY, CG_PSTATE_READ_PACKED_DIRECT, CG_PSTATE_TABLE_INITIALISED = 1, 2, 4, 8
 
 
 class CgSkipNode(C.Structure):
@@ -122,6 +123,8 @@ SYMBOLS = [
                                    C.POINTER(C.c_uint64)]),
     ("cg_partial_dense_words_enqueue", C.c_int, [_P, C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),
     ("cg_partial_check", C.c_int, [_P]),
+    ("cg_partial_packed_state", C.c_int, [_P, _P, C.c_uint64, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_uint32),
+                                          C.POINTER(C.c_uint64)]),
     ("cg_gen_set_compression", C.c_int, [C.c_int32]),
     ("cg_jit_launches", C.c_uint64, []),
     ("cg_jit_compiles", C.c_uint64, []),

@@ -602,6 +602,15 @@ class GpuColumnarAgg:
         """wait for the partial's pending work and raise what its kernels flagged"""
         check(lib().cg_partial_check(self.h))
 
+    def packed_state(self):
+        """(pack_shift C, pack_word, state bits capi.CG_PSTATE_*, packed words: uint64 array, one per entry; empty when
+        the partial has no packed words) -- a read that changes nothing"""
+        shift, word, state, n = C.c_int32(), C.c_int32(), C.c_uint32(), C.c_uint64()
+        check(lib().cg_partial_packed_state(self.h, None, 0, C.byref(shift), C.byref(word), C.byref(state), C.byref(n)))
+        words = np.zeros(n.value, np.uint64)
+        check(lib().cg_partial_packed_state(self.h, words.ctypes.data, n.value, None, None, None, C.byref(n)))
+        return shift.value, word.value, state.value, words
+
     def dense_words(self):
         p, total, stride = C.c_void_p(), C.c_int64(), C.c_int32()
         check(lib().cg_partial_dense_words(self.h, C.byref(p), C.byref(total), C.byref(stride)))

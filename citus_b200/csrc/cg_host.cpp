@@ -2031,6 +2031,29 @@ extern "C" int cg_partial_check(CgPartial *p)
 	return pending_errors(ctx, p);
 }
 
+extern "C" int cg_partial_packed_state(CgPartial *p, uint64_t *h_words, uint64_t capacity, int32_t *pack_shift, int32_t *pack_word,
+									   uint32_t *state, uint64_t *nwords)
+{
+	if (!p) return cg_set_error(CG_EINVAL, "NULL partial");
+	CgContext *ctx = cg_ctx();
+	if (!ctx) return CG_EINVAL;
+	const uint64_t n = p->d_packed ? p->entries : 0;
+	if (pack_shift) *pack_shift = p->d_packed ? p->pack_shift : 0;
+	if (pack_word) *pack_word = p->d_packed ? p->pack_word : 0;
+	if (state)
+		*state = (p->packed_dirty ? CG_PSTATE_PACKED_DIRTY : 0u) | (p->wide_dirty ? CG_PSTATE_WIDE_DIRTY : 0u) |
+				 (p->read_packed_direct ? CG_PSTATE_READ_PACKED_DIRECT : 0u) | (p->table_initialised ? CG_PSTATE_TABLE_INITIALISED : 0u);
+	if (nwords) *nwords = n;
+	/* only waits: nothing is enqueued on the compute stream, so an open scan chain stays open (cg_chain_end is for enqueues) */
+	CG_CUDA(cudaStreamSynchronize(ctx->compute));
+	if (h_words && capacity)
+	{
+		if (capacity < n) return cg_set_error(CG_EINVAL, "%llu packed words do not fit %llu", (unsigned long long) n, (unsigned long long) capacity);
+		if (n) CG_CUDA(cudaMemcpy(h_words, p->d_packed, n * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+	}
+	return CG_OK;
+}
+
 extern "C" int cg_partial_dense_words(CgPartial *p, uint64_t **d_words, int64_t *total_words, int32_t *stride)
 {
 	if (!p) return cg_set_error(CG_EINVAL, "NULL partial");

@@ -502,6 +502,17 @@ int cg_partial_dense_words(CgPartial *p, uint64_t **d_words, int64_t *total_word
 int cg_partial_dense_words_enqueue(CgPartial *p, uint64_t **d_words, int64_t *total_words, int32_t *stride);
 /* Waits for the partial's pending work and reports what its kernels flagged. */
 int cg_partial_check(CgPartial *p);
+/* Read-only view of the optimistic packing (cg_partial_set_packing): C (0 = the partial has no packed words), the
+ * accumulator word the packed sum drains into, the CG_PSTATE_* bits, and the packed words themselves -- one per table
+ * entry, ((sum << C) + rows) mod 2^64 -- copied into h_words (NULL or capacity 0: *nwords only).  Waits for the work
+ * already enqueued on the library's stream and enqueues none: the partial, its words and flags, and whether the next scan
+ * may overlap the previous one are all left as they were. */
+#define CG_PSTATE_PACKED_DIRTY 1u       /* packed words were added since the last drain or reset */
+#define CG_PSTATE_WIDE_DIRTY 2u         /* the wide accumulator words were written since the last reset */
+#define CG_PSTATE_READ_PACKED_DIRECT 4u /* a read decoded result rows straight from the packed words since the last drain */
+#define CG_PSTATE_TABLE_INITIALISED 8u  /* the wide table was initialised at least once */
+int cg_partial_packed_state(CgPartial *p, uint64_t *h_words, uint64_t capacity, int32_t *pack_shift, int32_t *pack_word,
+							uint32_t *state, uint64_t *nwords);
 
 /* ---------------------------------------------------------------------------------- *
  *  Hash repartition (map side): worker_partition_query_result's per-row routing

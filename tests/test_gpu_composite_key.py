@@ -252,6 +252,7 @@ def test_export_merge_rows_and_encoded_merge_values_round_trip(cg, oracle):
             keys = torch.zeros(ng, dtype=torch.int64, device="cuda")
             kn = torch.ones(ng, dtype=torch.uint8, device="cuda")
             words = torch.zeros(ng * nw, dtype=torch.int64, device="cuda")
+            torch.cuda.synchronize()                                # the fills run on torch's stream, the export on the library's
             got_n = src.export_device(keys.data_ptr(), kn.data_ptr(), words.data_ptr(), ng)
             assert got_n == ng
             assert int(kn.sum()) == 0                               # a composite partial has no NULL key: codes only
@@ -462,8 +463,10 @@ def test_a_null_key_flag_is_refused_by_a_composite_partial(cg, oracle):
         keys = torch.zeros(ng, dtype=torch.int64, device="cuda")
         dkn = torch.zeros(ng, dtype=torch.uint8, device="cuda")
         words = torch.zeros(ng * nw, dtype=torch.int64, device="cuda")
+        torch.cuda.synchronize()                                    # the fills run on torch's stream, the export on the library's
         src.export_device(keys.data_ptr(), dkn.data_ptr(), words.data_ptr(), ng)
         dkn[5] = 1
+        torch.cuda.synchronize()
         with pytest.raises(capi.CitusGpuError) as e:
             dst.merge_rows(keys.data_ptr(), dkn.data_ptr(), words.data_ptr(), ng)
         assert e.value.code == capi.CG_EINVAL

@@ -405,10 +405,12 @@ def test_merge_rows_low_words_that_add_past_2_64(cg):
         words = torch.tensor([[w - 2**64 if w >= 2**63 else w for w in r] for r in rows], dtype=torch.int64, device="cuda")
         keys = torch.full((3,), 2, dtype=torch.int64, device="cuda")
         kn = torch.zeros(3, dtype=torch.uint8, device="cuda")
+        torch.cuda.synchronize()                                 # the fills run on torch's stream, the merge on the library's
         p.merge_rows(keys.data_ptr(), kn.data_ptr(), words.data_ptr(), 3)
         g = list(p.groups().values())[0]
         assert g[0]["sum"] == sum(r[1] + (r[2] << 32) for r in rows) and g[1]["count"] == 4
         big = torch.tensor([[2**32, 5, 0, 0]], dtype=torch.int64, device="cuda")
+        torch.cuda.synchronize()
         p.merge_rows(keys.data_ptr(), kn.data_ptr(), big.data_ptr(), 1)
         with pytest.raises(capi.CitusGpuError) as e:
             p.groups()

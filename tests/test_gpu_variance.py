@@ -263,6 +263,7 @@ def test_export_merge_rows_round_trip_and_the_carry_chain(cg):
         keys = torch.zeros(8, dtype=torch.int64, device="cuda")
         kn = torch.zeros(8, dtype=torch.uint8, device="cuda")
         words = torch.zeros(8 * nw, dtype=torch.int64, device="cuda")
+        torch.cuda.synchronize()                   # the fills run on torch's stream, the library's kernels on its own
         rows = a.export_device(keys.data_ptr(), kn.data_ptr(), words.data_ptr(), 8)
         assert rows == 4
         b.merge_rows(keys.data_ptr(), kn.data_ptr(), words.data_ptr(), rows)
@@ -281,6 +282,7 @@ def test_export_merge_rows_round_trip_and_the_carry_chain(cg):
         try:
             t = torch.tensor([[w - 2**64 if w >= 2**63 else w for w in r] for r in hand], dtype=torch.int64, device="cuda")
             k3 = torch.full((3,), 1, dtype=torch.int64, device="cuda")
+            torch.cuda.synchronize()
             c.merge_rows(k3.data_ptr(), kn.data_ptr(), t.data_ptr(), 3)
             g = c.groups()[1]
             assert g[0]["count"] == sum(r[0] - r[7] for r in hand) and g[1]["count"] == 10
@@ -311,6 +313,7 @@ def test_groups_of_2_32_rows_and_host_row_merges_are_refused(cg):
             kn = torch.zeros(1, dtype=torch.uint8, device="cuda")
             big = torch.zeros((1, nw), dtype=torch.int64, device="cuda")
             big[0, 0] = 2**32
+            torch.cuda.synchronize()
             p.merge_rows(keys.data_ptr(), kn.data_ptr(), big.data_ptr(), 1)
             with pytest.raises(capi.CitusGpuError) as e:
                 p.groups()
