@@ -18,7 +18,8 @@ CG_OK, CG_EINVAL, CG_ECUDA, CG_ENOMEM, CG_ECORRUPT, CG_ETABLEFULL, CG_EUNSUPPORT
 CG_COMM_ID_BYTES = 128
 CG_COMM_SUM, CG_COMM_MIN, CG_COMM_MAX = 0, 1, 2
 CG_TYPE_INT, CG_TYPE_FLOAT = 0, 1
-CG_OP = {"<": 0, "<=": 1, "=": 2, ">=": 3, ">": 4, "<>": 5, "in": 6, "not in": 7, "is null": 8, "is not null": 9}
+CG_OP = {"<": 0, "<=": 1, "=": 2, ">=": 3, ">": 4, "<>": 5, "in": 6, "not in": 7, "is null": 8, "is not null": 9,
+         "col <": 16, "col <=": 17, "col =": 18, "col >=": 19, "col >": 20, "col <>": 21}
 CG_AGG_COUNT_STAR, CG_AGG_COUNT, CG_AGG_SUM, CG_AGG_MIN, CG_AGG_MAX = range(5)
 CG_AGG_BIT_AND, CG_AGG_BIT_OR, CG_AGG_BOOL_AND, CG_AGG_BOOL_OR = range(5, 9)
 CG_AGG_VARIANCE = 9

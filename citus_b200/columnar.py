@@ -246,7 +246,8 @@ def variance(col, filter=None):
 
 
 def flatten_where(where):
-    """WHERE as a nested tuple tree -- ("and" | "or", arm, arm, ...) over atoms (column, op, constant), (column, "in" |
+    """WHERE as a nested tuple tree -- ("and" | "or", arm, arm, ...) over atoms (column, op, constant), (column, op,
+    Col(other)), (column, "in" |
     "not in", (value, ...)) and (column, "is null" | "is not null"); a plain list of atoms is their AND -- to (atoms, postfix
     tokens).  The tokens are empty for a plain AND-list."""
     if not (isinstance(where, tuple) and where and where[0] in ("and", "or")):
@@ -291,11 +292,21 @@ def _konst(k, col, float_cols):
     return int(np.float64(k).view(np.int64)) if col in float_cols else int(k)
 
 
+@dataclass(frozen=True)
+class Col:
+    """the right-hand side of a column-to-column atom: (0, "<", Col(3)) is "column 0 < column 3" of the same row"""
+    index: int
+
+
 def _set_atom(q, atom, float_cols, lists):
-    """one atom: (column, op, constant); (column, "in" | "not in", (v, ...)) with None for a NULL element -- the list goes
-    to `lists`, [(elements, float?)], and konst is its index; (column, "is null" | "is not null")"""
+    """one atom: (column, op, constant); (column, op, Col(other)); (column, "in" | "not in", (v, ...)) with None for a NULL
+    element -- the list goes to `lists`, [(elements, float?)], and konst is its index; (column, "is null" | "is not null")"""
     col, op = atom[0], atom[1]
     q.column = col
+    if len(atom) == 3 and isinstance(atom[2], Col):
+        q.op = capi.CG_OP["col " + op]
+        q.konst = atom[2].index
+        return
     q.op = capi.CG_OP[op]
     if op in ("is null", "is not null"):
         if len(atom) != 2:

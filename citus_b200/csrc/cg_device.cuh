@@ -174,17 +174,38 @@ __device__ __forceinline__ bool set_contains(const uint64_t *s, uint32_t len, ui
 	return __ldg(b) == key;
 }
 
+/* sign of x * m - y, exact in 128 bits (m > 0) */
+__device__ __forceinline__ int cmp_scaled(int64_t x, int64_t m, int64_t y)
+{
+	const int64_t h = __mul64hi(x, m), yh = y >> 63;
+	const uint64_t l = (uint64_t) x * (uint64_t) m;
+	return h != yh ? (h < yh ? -1 : 1) : ((l > (uint64_t) y) - (l < (uint64_t) y));
+}
+
+/* sign of x - y for a column atom's two sides: integer-like after scale alignment (KCmp), float in float8 btree order
+ * (cg_set_code is that order as unsigned) */
+__device__ __forceinline__ int col_cmp(int64_t x, int64_t y, bool isfloat, const KCmp &kc)
+{
+	if (isfloat)
+	{
+		const uint64_t a = cg_set_code(x, true), b = cg_set_code(y, true);
+		return (a > b) - (a < b);
+	}
+	return kc.right ? -cmp_scaled(y, kc.mul, x) : cmp_scaled(x, kc.mul, y);
+}
+
 /*
  * K3: the WHERE tree ([PG] ExecQual under ExecScan, columnar_customscan.c:1907-1913) under three-valued
  * logic: an atom on a NULL input is not TRUE, AND/OR combine "is TRUE" bits (there is no NOT node: it is
  * folded into the comparison operators), the row passes iff the root is TRUE.  Without a tree the atoms
  * are an AND-list.  The list and NULL-test atoms have TRUE and FALSE of their own (include/citus_gpu.h, CgQual):
- * IS [NOT] NULL is never UNKNOWN, and a list with a NULL element makes "not found" UNKNOWN.
+ * IS [NOT] NULL is never UNKNOWN, and a list with a NULL element makes "not found" UNKNOWN.  A column atom is UNKNOWN
+ * when either of its columns is NULL.
  */
 template <int NCC>
 __device__ __forceinline__ uint32_t eval_atoms(const KPlan &P, const int64_t (&v)[NCC], uint32_t nullmask, int n, const uint8_t *col,
 											   const uint8_t *op, const int64_t *k, const int64_t *lo, const int64_t *hi, const uint8_t *neg,
-											   const KSet *ks, uint32_t *falsity = nullptr)
+											   const KSet *ks, const KCmp *kc, uint32_t *falsity = nullptr)
 {
 	uint32_t truth = 0, fals = 0;
 #pragma unroll 1
@@ -199,6 +220,24 @@ __device__ __forceinline__ uint32_t eval_atoms(const KPlan &P, const int64_t (&v
 			const bool r = P.isfloat[c] ? qual_true(x, op[q], k[q], true) : (((x >= lo[q]) && (x <= hi[q])) != (bool) neg[q]);
 			t = r && !isnull;
 			f = !r && !isnull;
+		}
+		else if (op[q] >= CG_OP_COL_LT)
+		{
+			const KCmp cc = kc[q];
+			const bool known = !isnull && !((nullmask >> cc.col2) & 1u);
+			const int s = col_cmp(x, pick<NCC>(v, cc.col2), P.isfloat[c], cc);
+			bool r;
+			switch (op[q])
+			{
+				case CG_OP_COL_LT: r = s < 0; break;
+				case CG_OP_COL_LE: r = s <= 0; break;
+				case CG_OP_COL_EQ: r = s == 0; break;
+				case CG_OP_COL_GE: r = s >= 0; break;
+				case CG_OP_COL_GT: r = s > 0; break;
+				default: r = s != 0; break;
+			}
+			t = r && known;
+			f = !r && known;
 		}
 		else if (op[q] >= CG_OP_IS_NULL)
 		{
@@ -243,7 +282,7 @@ __device__ __forceinline__ bool eval_postfix(uint32_t truth, int n, const int8_t
 template <int NCC>
 __device__ __forceinline__ bool eval_where(const KPlan &P, const int64_t (&v)[NCC], uint32_t nullmask)
 {
-	uint32_t truth = eval_atoms<NCC>(P, v, nullmask, P.nquals, P.qcol, P.qop, P.qk, P.qlo, P.qhi, P.qneg, P.qset);
+	uint32_t truth = eval_atoms<NCC>(P, v, nullmask, P.nquals, P.qcol, P.qop, P.qk, P.qlo, P.qhi, P.qneg, P.qset, P.qcc);
 	if (P.nqexpr == 0) return truth == (1u << P.nquals) - 1u;
 	return eval_postfix(truth, P.nqexpr, P.qexpr);
 }
@@ -257,7 +296,7 @@ __device__ __forceinline__ uint32_t eval_filters(const KPlan &P, const int64_t (
 	if (argtrue) *argtrue = 0u;
 	if (P.nfquals == 0) return 0u;
 	uint32_t fals = 0;
-	uint32_t truth = eval_atoms<NCC>(P, v, nullmask, P.nfquals, P.fcol, P.fop, P.fk, P.flo, P.fhi, P.fneg, P.fset, &fals);
+	uint32_t truth = eval_atoms<NCC>(P, v, nullmask, P.nfquals, P.fcol, P.fop, P.fk, P.flo, P.fhi, P.fneg, P.fset, P.fcc, &fals);
 	uint32_t rejected = 0, at = 0;
 #pragma unroll 1
 	for (int a = 0; a < P.naggs; a++)

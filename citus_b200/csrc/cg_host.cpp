@@ -1491,14 +1491,19 @@ extern "C" int cg_scan_relation(const CgRelation *rel, const CgScanDesc *desc, C
 	/* projection */
 	std::vector<int32_t> staged, slot_of_att(rel->natts, -1);
 	auto need = [&](int c) { if (slot_of_att[c] < 0) { slot_of_att[c] = (int32_t) staged.size(); staged.push_back(c); } };
-	for (int q = 0; q < desc->nquals; q++) if (desc->quals[q].column >= 0 && desc->quals[q].column < rel->natts) need(desc->quals[q].column);
+	/* a column atom reads its other column too (CgQual.konst) */
+	auto need_atom = [&](const CgQual &q) {
+		if (q.column >= 0 && q.column < rel->natts) need(q.column);
+		if (cg_op_is_column(q.op) && q.konst >= 0 && q.konst < rel->natts) need((int) q.konst);
+	};
+	for (int q = 0; q < desc->nquals; q++) need_atom(desc->quals[q]);
 	for (int g = 0; g < desc->ngroup_cols; g++) if (desc->group_cols[g] >= 0 && desc->group_cols[g] < rel->natts) need(desc->group_cols[g]);
 	for (int a = 0; a < desc->naggs; a++)
 		for (int f = 0; f < desc->aggs[a].nfactors && f < 3; f++)
 			if (desc->aggs[a].column[f] >= 0 && desc->aggs[a].column[f] < rel->natts) need(desc->aggs[a].column[f]);
 	if (cg_desc_uses_pool(desc))
 		for (int q = 0; q < desc->nfilter_quals && q < CG_MAX_FILTER_QUALS; q++)
-			if (desc->filter_quals[q].column >= 0 && desc->filter_quals[q].column < rel->natts) need(desc->filter_quals[q].column);
+			need_atom(desc->filter_quals[q]);
 	if (staged.empty()) need(0);   /* count(*) only: the reference still reads the first column's skip nodes; we read its chunk row counts */
 
 	KPlan plan;

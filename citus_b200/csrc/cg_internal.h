@@ -243,6 +243,17 @@ static inline __host__ __device__ uint64_t cg_set_code(int64_t v, bool isfloat)
 	return (u >> 63) ? ~u : (u | 0x8000000000000000ull);
 }
 
+/* the other side of a column atom "x <op> y" (x = the atom's plan column): y is plan column col2.  Integer-like sides
+ * compare x * mul with y (right = 0) or x with y * mul (right = 1), exactly in 128 bits; mul = 10^(scale difference), 1
+ * for equal scales, char(1) and float sides (float sides compare their cg_set_code) */
+struct KCmp
+{
+	int64_t mul;
+	uint8_t col2;
+	uint8_t right;
+	uint8_t pad[6];
+};
+
 struct KPlan
 {
 	const uint8_t *arena;
@@ -331,7 +342,13 @@ struct KPlan
 	const uint64_t *sets;
 	KSet qset[CG_MAX_QUALS];
 	KSet fset[CG_MAX_FILTER_QUALS];
+	/* column atoms (qop / fop CG_OP_COL_*): the other side of WHERE / pool atom q is qcc / fcc [q].  Behind the lists, so
+	 * that the generated kernels of plans without column atoms restate the struct without them (cg_jit.cpp) */
+	KCmp qcc[CG_MAX_QUALS];
+	KCmp fcc[CG_MAX_FILTER_QUALS];
 };
+
+static inline __host__ __device__ bool cg_op_is_column(int op) { return op >= CG_OP_COL_LT && op <= CG_OP_COL_NE; }
 
 static inline bool cg_desc_has_filters(const CgScanDesc *d)
 {

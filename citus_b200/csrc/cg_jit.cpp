@@ -338,6 +338,14 @@ static bool plan_has_sets(const KPlan &plan)
 	return false;
 }
 
+/* some WHERE or pool atom compares two columns: the prelude defines their comparison helpers */
+static bool plan_has_column_atoms(const KPlan &plan)
+{
+	for (int q = 0; q < plan.nquals; q++) if (cg_op_is_column(plan.qop[q])) return true;
+	for (int q = 0; q < plan.nfquals; q++) if (cg_op_is_column(plan.fop[q])) return true;
+	return false;
+}
+
 /* The host's structs restated for NVRTC.  A plan without bool_and / bool_or arguments restates KPlan up to fexpr and
  * KAgg's barg byte as padding: its kernel reads nothing behind them (the arguments' trees are written out as code), so
  * the plan parameter it declares is a prefix of the one the host passes, and its source is the one such plans had
@@ -386,9 +394,10 @@ static void gen_prelude(std::string &s, const KPlan &plan)
 	if (composite) addf(s, "  int32_t composite; int64_t kmin[%d]; uint64_t kradix[%d];%s", CG_MAX_GROUP_COLS, CG_MAX_GROUP_COLS, sets ? "\n" : " };\n");
 	if (sets) addf(s, "  const uint64_t *sets; KSet qset[%d]; KSet fset[%d]; };\n", CG_MAX_QUALS, CG_MAX_FILTER_QUALS);
 	/* the text above must describe the host's structs exactly (without arguments: the prefix up to fexpr; with arguments
-	 * only: the prefix up to argexpr; with a composite key: the prefix up to the lists) */
+	 * only: the prefix up to argexpr; with a composite key: the prefix up to the lists; with lists: the prefix up to the
+	 * column atoms' KCmp entries, which the generated code never reads -- their columns and scales are written out) */
 	const auto upto = [](size_t off) { return (off + alignof(KPlan) - 1) / alignof(KPlan) * alignof(KPlan); };
-	const size_t size = sets ? sizeof(KPlan) : composite ? upto(offsetof(KPlan, sets)) : args ? upto(offsetof(KPlan, composite))
+	const size_t size = sets ? upto(offsetof(KPlan, qcc)) : composite ? upto(offsetof(KPlan, sets)) : args ? upto(offsetof(KPlan, composite))
 																					   : upto(offsetof(KPlan, nargexpr));
 	addf(s, "static_assert(sizeof(DevChunkCol) == %zu, \"DevChunkCol\");\n", sizeof(DevChunkCol));
 	addf(s, "static_assert(sizeof(KAgg) == %zu, \"KAgg\");\n", sizeof(KAgg));
@@ -439,6 +448,14 @@ static void gen_prelude(std::string &s, const KPlan &plan)
 			"  const uint64_t *b = sets + k.off; uint32_t n = k.len;\n"
 			"  for (uint32_t i = 0; i < k.steps; i++) { const uint32_t h = n >> 1; b = (__ldg(b + h) <= key) ? b + h : b; n -= h; }\n"
 			"  return __ldg(b) == key; }\n";
+	if (plan_has_column_atoms(plan))
+		/* column atoms (cg_device.cuh, col_cmp): float sides compare their cg_set_code, integer-like sides of different scales
+		 * the sign of x * m - y in 128 bits */
+		s +=
+			"__device__ __forceinline__ uint64_t col_code_f(int64_t v) { uint64_t u = (uint64_t) v; if (u == 0x8000000000000000ull) u = 0;\n"
+			"  if ((u & 0x7fffffffffffffffull) > 0x7ff0000000000000ull) return ~0ull; return (u >> 63) ? ~u : (u | 0x8000000000000000ull); }\n"
+			"__device__ __forceinline__ int cmp_scaled(int64_t x, int64_t m, int64_t y) { const int64_t h = __mul64hi(x, m), yh = y >> 63;\n"
+			"  const uint64_t l = (uint64_t) x * (uint64_t) m; return h != yh ? (h < yh ? -1 : 1) : ((l > (uint64_t) y) - (l < (uint64_t) y)); }\n";
 }
 
 static bool col_nullable(const JitShape &sh, int c) { return (sh.nullable >> c) & 1u; }
@@ -591,6 +608,22 @@ static std::string found_var(const char *prefix, int q) { return "h" + std::stri
 /* one atom "column <op> constant" on plan column c, its constants in P.<arr>k / <arr>lo / <arr>hi / <arr>neg [q]; an atom
  * on a NULL input is not TRUE (three-valued logic).  IS [NOT] NULL reads only the NULL flag (in the plain form, where the
  * column has no NULL, it is a constant); IN / NOT IN read found_var(prefix, q) and the list's NULL flag P.<arr>set[q].nnull */
+/* the other side of column atom q of the WHERE list (arr "q") or the pool (arr "f") */
+static const KCmp &atom_cmp(const KPlan &plan, const char *arr, int q) { return arr[0] == 'q' ? plan.qcc[q] : plan.fcc[q]; }
+
+/* "neither column of atom q is NULL" as a prefix "!z<c> && ..." ("" when neither column is nullable) */
+static std::string atom_known(const KPlan &plan, const JitShape &sh, int c, int op, const char *arr, int q)
+{
+	std::string nn;
+	if (col_nullable(sh, c)) nn += "!z" + std::to_string(c) + " && ";
+	if (cg_op_is_column(op))
+	{
+		const int c2 = atom_cmp(plan, arr, q).col2;
+		if (c2 != c && col_nullable(sh, c2)) nn += "!z" + std::to_string(c2) + " && ";
+	}
+	return nn;
+}
+
 static std::string atom_expr(const KPlan &plan, const JitShape &sh, int c, int op, bool neg, const char *arr, int q, const char *prefix)
 {
 	char buf[256], nn[32] = "";
@@ -598,6 +631,20 @@ static std::string atom_expr(const KPlan &plan, const JitShape &sh, int c, int o
 	{
 		if (!col_nullable(sh, c)) return op == CG_OP_IS_NULL ? "false" : "true";
 		snprintf(buf, sizeof buf, "%sz%d", op == CG_OP_IS_NULL ? "" : "!", c);
+		return buf;
+	}
+	if (cg_op_is_column(op))
+	{
+		/* the columns, the operator and the scale factor are the plan's shape: all of them are written out */
+		const char *ops[] = {"<", "<=", "==", ">=", ">", "!="};
+		const char *o = ops[op - CG_OP_COL_LT];
+		const KCmp &kc = atom_cmp(plan, arr, q);
+		const std::string known = atom_known(plan, sh, c, op, arr, q);
+		if (plan.isfloat[c]) snprintf(buf, sizeof buf, "%s(col_code_f(v%d) %s col_code_f(v%d))", known.c_str(), c, o, kc.col2);
+		else if (kc.mul == 1) snprintf(buf, sizeof buf, "%s(v%d %s v%d)", known.c_str(), c, o, kc.col2);
+		/* x op y * m  <=>  sign(x - y * m) op 0  <=>  0 op sign(y * m - x) */
+		else if (kc.right) snprintf(buf, sizeof buf, "%s(0 %s cmp_scaled(v%d, %lldll, v%d))", known.c_str(), o, kc.col2, (long long) kc.mul, c);
+		else snprintf(buf, sizeof buf, "%s(cmp_scaled(v%d, %lldll, v%d) %s 0)", known.c_str(), c, (long long) kc.mul, kc.col2, o);
 		return buf;
 	}
 	if (col_nullable(sh, c)) snprintf(nn, sizeof nn, "!z%d && ", c);
@@ -722,6 +769,7 @@ static void gen_row(std::string &s, const KPlan &plan, const JitShape &sh, int u
 			if (op == CG_OP_IS_NULL || op == CG_OP_IS_NOT_NULL) addf(s, "%sconst bool uf%d = !u%d;\n", T, q, q);     /* never UNKNOWN */
 			else if (op == CG_OP_IN) addf(s, "%sconst bool uf%d = %s!%s && !P.fset[%d].nnull;\n", T, q, nn.c_str(), found_var("u", q).c_str(), q);
 			else if (op == CG_OP_NOT_IN) addf(s, "%sconst bool uf%d = %s%s;\n", T, q, nn.c_str(), found_var("u", q).c_str());
+			else if (cg_op_is_column(op)) addf(s, "%sconst bool uf%d = %s!u%d;\n", T, q, atom_known(plan, sh, c, op, "f", q).c_str(), q);
 			else if (col_nullable(sh, c)) addf(s, "%sconst bool uf%d = !z%d && !u%d;\n", T, q, c, q);
 			else addf(s, "%sconst bool uf%d = !u%d;\n", T, q, q);
 		}

@@ -50,8 +50,10 @@ static int validate_atoms(const char *what, const CgQual *quals, int n, int natt
 	{
 		if (quals[q].column < 0 || quals[q].column >= natts)
 			return cg_set_error(CG_EINVAL, "%s %d: column %d out of range", what, q, quals[q].column);
-		if (quals[q].op < CG_OP_LT || quals[q].op > CG_OP_IS_NOT_NULL)
+		if (quals[q].op < CG_OP_LT || (quals[q].op > CG_OP_IS_NOT_NULL && !cg_op_is_column(quals[q].op)))
 			return cg_set_error(CG_EINVAL, "%s %d: bad operator", what, q);
+		if (cg_op_is_column(quals[q].op) && (quals[q].konst < 0 || quals[q].konst >= natts))
+			return cg_set_error(CG_EINVAL, "%s %d: other column %lld out of range", what, q, (long long) quals[q].konst);
 		if ((quals[q].op == CG_OP_IN || quals[q].op == CG_OP_NOT_IN) && (quals[q].konst < 0 || quals[q].konst >= nin_lists))
 			return cg_set_error(CG_EINVAL, "%s %d: list %lld of %d", what, q, (long long) quals[q].konst, nin_lists);
 		if ((quals[q].op == CG_OP_IS_NULL || quals[q].op == CG_OP_IS_NOT_NULL) && quals[q].konst != 0)
@@ -77,6 +79,27 @@ static int validate_lists(const CgScanDesc *d)
 }
 
 static inline bool op_is_list(int op) { return op == CG_OP_IN || op == CG_OP_NOT_IN; }
+
+/* the comparison class of a column atom's side: integer-like (int, bool, numeric), char(1) or float */
+enum { CMP_INTEGER = 0, CMP_CHAR = 1, CMP_FLOAT = 2 };
+static int cmp_class(const CgColumnDesc &c)
+{
+	const int cls = cg_type_class(c);
+	return cls == CG_TYPE_FLOAT ? CMP_FLOAT : cls == CG_TYPE_BPCHAR1 ? CMP_CHAR : CMP_INTEGER;
+}
+
+/* column atoms compare two columns of one class (include/citus_gpu.h, CgQual) */
+static int validate_column_atoms(const char *what, const CgQual *quals, int n, const CgColumnDesc *columns)
+{
+	for (int q = 0; q < n; q++)
+	{
+		if (!cg_op_is_column(quals[q].op)) continue;
+		const int a = quals[q].column, b = (int) quals[q].konst;
+		if (cmp_class(columns[a]) != cmp_class(columns[b]))
+			return cg_set_error(CG_EUNSUPPORTED, "%s %d: columns %d and %d are of different comparison classes", what, q, a, b);
+	}
+	return CG_OK;
+}
 
 std::vector<int64_t> cg_where_lists(const CgScanDesc *d)
 {
@@ -120,11 +143,13 @@ static int validate_desc(const CgScanDesc *d, const CgColumnDesc *columns, int n
 	int rc = validate_lists(d);
 	if (rc) return rc;
 	if ((rc = validate_atoms("qual", d->quals, d->nquals, natts, d->nin_lists))) return rc;
+	if ((rc = validate_column_atoms("qual", d->quals, d->nquals, columns))) return rc;
 	if (d->nqual_expr < 0 || d->nqual_expr > CG_MAX_QEXPR) return cg_set_error(CG_EINVAL, "nqual_expr %d out of range", d->nqual_expr);
 	if (d->nqual_expr > 0 && (rc = validate_postfix("qual_expr", d->qual_expr, d->nqual_expr, d->nquals))) return rc;
 	if (d->nfilter_quals < 0 || d->nfilter_quals > CG_MAX_FILTER_QUALS)
 		return cg_set_error(CG_EINVAL, "nfilter_quals %d out of range", d->nfilter_quals);
 	if ((rc = validate_atoms("filter qual", d->filter_quals, d->nfilter_quals, natts, d->nin_lists))) return rc;
+	if ((rc = validate_column_atoms("filter qual", d->filter_quals, d->nfilter_quals, columns))) return rc;
 	for (int a = 0; a < CG_MAX_AGGS; a++)
 	{
 		const int n = d->nfilter_expr[a];
@@ -626,6 +651,7 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 	auto atom_range = [](const CgQual &q, int64_t *lo_out, int64_t *hi_out, uint8_t *neg_out) {
 		int64_t k = q.konst, lo = INT64_MIN, hi = INT64_MAX;
 		bool neg = false;
+		if (cg_op_is_column(q.op)) { *lo_out = *hi_out = 0; *neg_out = 0; return; }     /* no constant: KCmp instead */
 		switch (q.op)
 		{
 			case CG_OP_LT: if (k == INT64_MIN) { lo = 1; hi = 0; } else hi = k - 1; break;
@@ -664,6 +690,21 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 		ks->steps = (uint8_t) steps;
 		ks->nnull = (uint8_t) (L.nnulls > 0);
 	};
+	/* column atoms: the other column is a plan column too; integer-like sides of different scales align on the larger one */
+	auto cmp_of = [&](const CgQual &q, KCmp *kc) -> int {
+		memset(kc, 0, sizeof *kc);
+		kc->mul = 1;
+		if (!cg_op_is_column(q.op)) return CG_OK;
+		int pc; USE_OR_FAIL(pc, (int) q.konst);
+		kc->col2 = (uint8_t) pc;
+		const CgColumnDesc &x = columns[q.column], &y = columns[q.konst];
+		if (cmp_class(x) != CMP_INTEGER) return CG_OK;
+		const int sx = cg_type_class(x) == CG_TYPE_NUMERIC ? cg_type_scale(x) : 0;
+		const int sy = cg_type_class(y) == CG_TYPE_NUMERIC ? cg_type_scale(y) : 0;
+		kc->right = (uint8_t) (sx > sy);
+		for (int i = 0; i < (sx > sy ? sx - sy : sy - sx); i++) kc->mul *= 10;      /* <= 10^18 */
+		return CG_OK;
+	};
 	plan->nquals = desc->nquals;
 	for (int q = 0; q < desc->nquals; q++)
 	{
@@ -673,6 +714,7 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 		plan->qk[q] = desc->quals[q].konst;
 		atom_range(desc->quals[q], &plan->qlo[q], &plan->qhi[q], &plan->qneg[q]);
 		set_of(desc->quals[q], plan->isfloat[pc], &plan->qset[q]);
+		if ((rc = cmp_of(desc->quals[q], &plan->qcc[q]))) return rc;
 	}
 	plan->slices = 1; plan->slice_rows = 1u << 30; plan->max_cg_rows = 0;
 	plan->nqexpr = desc->nqual_expr;
@@ -713,6 +755,7 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 			plan->fk[q] = desc->filter_quals[q].konst;
 			atom_range(desc->filter_quals[q], &plan->flo[q], &plan->fhi[q], &plan->fneg[q]);
 			set_of(desc->filter_quals[q], plan->isfloat[pc], &plan->fset[q]);
+			if ((rc = cmp_of(desc->filter_quals[q], &plan->fcc[q]))) return rc;
 		}
 		for (int a = 0; a < desc->naggs; a++)
 		{
@@ -760,7 +803,7 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 bool cg_build_fast_plan(const CgScanDesc *desc, const KPlan &plan, bool all8, FPlan *fast)
 {
 	if (!all8 || plan.ngroup > 1 || plan.composite || plan.nqexpr != 0 || plan.nfquals != 0) return false;
-	for (int q = 0; q < plan.nquals; q++) if (plan.qop[q] > CG_OP_NE) return false;     /* IN lists and NULL tests */
+	for (int q = 0; q < plan.nquals; q++) if (plan.qop[q] > CG_OP_NE) return false;     /* IN lists, NULL tests, column atoms */
 	for (int c = 0; c < plan.ncols; c++) if (plan.isfloat[c]) return false;
 	memset(fast, 0, sizeof *fast);
 	bool used[CG_KMAX_COLS] = {false};

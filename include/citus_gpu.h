@@ -178,7 +178,9 @@ typedef struct CgRelation
  *  split planner/multi_logical_optimizer.c:3160-3484.
  * ---------------------------------------------------------------------------------- */
 enum { CG_OP_LT = 0, CG_OP_LE = 1, CG_OP_EQ = 2, CG_OP_GE = 3, CG_OP_GT = 4, CG_OP_NE = 5,
-	   CG_OP_IN = 6, CG_OP_NOT_IN = 7, CG_OP_IS_NULL = 8, CG_OP_IS_NOT_NULL = 9 };
+	   CG_OP_IN = 6, CG_OP_NOT_IN = 7, CG_OP_IS_NULL = 8, CG_OP_IS_NOT_NULL = 9,
+	   CG_OP_COL_LT = 16, CG_OP_COL_LE = 17, CG_OP_COL_EQ = 18, CG_OP_COL_GE = 19, CG_OP_COL_GT = 20, CG_OP_COL_NE = 21 };
+/* 10 .. 15 are not operators: a descriptor that uses one is CG_EINVAL, as it was before the column atoms existed */
 
 /* one atom of a predicate tree: "column <op> constant" (btree operators), a list membership test or a NULL test.
  * CG_OP_IN / CG_OP_NOT_IN ([PG] ScalarArrayOpExpr "x = ANY(array)" / "x <> ALL(array)", which is how IN and NOT IN lists
@@ -196,12 +198,28 @@ enum { CG_OP_LT = 0, CG_OP_LE = 1, CG_OP_EQ = 2, CG_OP_GE = 3, CG_OP_GT = 4, CG_
  * Chunk-group skipping follows the reference ([PG] predicate_refuted_by with weak = false over the pushed-down clauses):
  * an IS test is never pushed down and refutes nothing; NOT IN refutes nothing (as <> does); IN refutes a chunk's
  * [min, max] iff its list has at most 100 elements (nvalues + nnulls, duplicates included), no NULL element, and every
- * element lies outside [min, max]. */
+ * element lies outside [min, max].
+ * CG_OP_COL_LT .. CG_OP_COL_NE ([PG] OpExpr "x <op> y" over two Vars of the scanned relation): "column <op> other", with
+ * konst the 0-based attribute index of the other column (it may be the column itself).  Any atom may use them, as above.
+ * With y the other column's value of the same row:
+ *                       x or y is NULL   otherwise
+ *     x <op> y          UNKNOWN          TRUE or FALSE
+ * The two columns must be of one comparison class, else the descriptor is CG_EUNSUPPORTED:
+ *     integer-like   int1 / 2 / 4 / 8, bool, numeric(p, s) in any pairing: exact on the mathematical values.  The side of
+ *                    the smaller scale is multiplied by 10^(scale difference) (an integer column has scale 0), in 128 bits,
+ *                    so int8 < numeric(12, 2) compares x * 100 with y as [PG]'s cast to numeric does
+ *     char(1)        against char(1) only: the unsigned byte
+ *     float          float4 / float8 in any pairing: float4 widened to float8 (exact), float8 btree order (every NaN
+ *                    equals every NaN and is above +inf, -0.0 equals +0.0)
+ * An integer-like column against a float column is CG_EUNSUPPORTED ([PG] casts it to float8, which rounds int8).  A
+ * column atom is never pushed down ([PG] ExtractPushdownClause wants a constant side): it refutes no chunk group and adds
+ * no bound. */
 typedef struct CgQual
 {
 	int32_t column;   /* 0-based attribute index */
 	int32_t op;       /* CG_OP_* */
-	int64_t konst;    /* integer, or float8 bits for float columns; IN / NOT IN: list index; IS [NOT] NULL: 0 */
+	int64_t konst;    /* integer, or float8 bits for float columns; IN / NOT IN: list index; IS [NOT] NULL: 0;
+					   * CG_OP_COL_*: the other column's attribute index */
 } CgQual;
 
 #define CG_MAX_IN_LISTS 8

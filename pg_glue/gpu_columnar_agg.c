@@ -163,13 +163,64 @@ btree_strategy(Oid opno, Oid type)
 	return get_op_opfamily_strategy(opno, get_opclass_family(opclass));
 }
 
-/* one WHERE atom "Var op Const" (or commuted) -> CgQual; false when it is anything else */
+/* the pairs of column types a column atom compares: integers of any width, floats of any width, and bool, date, timestamp,
+ * timestamptz each with itself.  date / timestamp / timestamptz against one another are refused: their comparison converts
+ * units (and, for timestamptz, uses the session time zone), so it is not a comparison of the decoded integers */
+static bool
+column_pair_supported(Oid a, Oid b)
+{
+	const bool ia = a == INT2OID || a == INT4OID || a == INT8OID, ib = b == INT2OID || b == INT4OID || b == INT8OID;
+	const bool fa = a == FLOAT4OID || a == FLOAT8OID, fb = b == FLOAT4OID || b == FLOAT8OID;
+	if (ia || ib)
+		return ia && ib;
+	if (fa || fb)
+		return fa && fb;
+	return a == b && (a == BOOLOID || a == DATEOID || a == TIMESTAMPOID || a == TIMESTAMPTZOID);
+}
+
+/* btree strategy -> the atom's operator ("<>", the negator of "=", has no strategy); -1 for anything else */
+static int
+strategy_op(int strategy, Oid opno)
+{
+	switch (strategy)
+	{
+		case BTLessStrategyNumber: return CG_OP_LT;
+		case BTLessEqualStrategyNumber: return CG_OP_LE;
+		case BTEqualStrategyNumber: return CG_OP_EQ;
+		case BTGreaterEqualStrategyNumber: return CG_OP_GE;
+		case BTGreaterStrategyNumber: return CG_OP_GT;
+		default: return strcmp(get_opname(opno), "<>") == 0 ? CG_OP_NE : -1;
+	}
+}
+
+/* "Var op Var" over two columns of the scanned relation -> a CG_OP_COL_* atom; false for any other pair of types */
+static bool
+translate_column_atom(Var *x, Var *y, Oid opno, TupleDesc tupdesc, CgQual *qual)
+{
+	int attlen, type_class;
+	if (x->varno != y->varno || x->varlevelsup != 0 || y->varlevelsup != 0 || x->varattno <= 0 || x->varattno > tupdesc->natts ||
+		y->varattno <= 0 || y->varattno > tupdesc->natts || !type_is_supported(x->vartype, &attlen, &type_class) ||
+		!type_is_supported(y->vartype, &attlen, &type_class) || !column_pair_supported(x->vartype, y->vartype))
+		return false;
+	/* the strategy in the left type's default operator family, which holds the cross-type operators of its family */
+	const int cgop = strategy_op(btree_strategy(opno, x->vartype), opno);
+	if (cgop < 0)
+		return false;
+	qual->column = x->varattno - 1;
+	qual->op = CG_OP_COL_LT + (cgop - CG_OP_LT);
+	qual->konst = y->varattno - 1;
+	return true;
+}
+
+/* one WHERE atom "Var op Const" (or commuted) or "Var op Var" -> CgQual; false when it is anything else */
 static bool
 translate_atom(OpExpr *op, TupleDesc tupdesc, CgQual *qual)
 {
 	if (list_length(op->args) != 2)
 		return false;
 	Node *l = (Node *) linitial(op->args), *r = (Node *) lsecond(op->args);
+	if (strip_to_var(l) && strip_to_var(r))
+		return translate_column_atom(strip_to_var(l), strip_to_var(r), op->opno, tupdesc, qual);
 	Var *var = strip_to_var(l);
 	Const *konst = (r && IsA(r, Const)) ? (Const *) r : NULL;
 	Oid opno = op->opno;
@@ -186,21 +237,9 @@ translate_atom(OpExpr *op, TupleDesc tupdesc, CgQual *qual)
 	int attlen, type_class;
 	if (!type_is_supported(var->vartype, &attlen, &type_class) || konst->consttype != var->vartype)
 		return false;
-	int strategy = btree_strategy(opno, var->vartype);
-	int cgop;
-	switch (strategy)
-	{
-		case BTLessStrategyNumber: cgop = CG_OP_LT; break;
-		case BTLessEqualStrategyNumber: cgop = CG_OP_LE; break;
-		case BTEqualStrategyNumber: cgop = CG_OP_EQ; break;
-		case BTGreaterEqualStrategyNumber: cgop = CG_OP_GE; break;
-		case BTGreaterStrategyNumber: cgop = CG_OP_GT; break;
-		default:
-			if (strcmp(get_opname(opno), "<>") != 0)
-				return false;
-			cgop = CG_OP_NE;
-			break;
-	}
+	int cgop = strategy_op(btree_strategy(opno, var->vartype), opno);
+	if (cgop < 0)
+		return false;
 	qual->column = var->varattno - 1;
 	qual->op = cgop;
 	if (type_class == CG_TYPE_FLOAT)
@@ -293,8 +332,9 @@ translate_bool_var(Node *node, bool negated, TupleDesc tupdesc, CgQual *qual)
 
 /* boolean tree -> atoms appended to atoms[0 .. *natoms) (at most max_atoms) + postfix tokens appended to tokens[0 .. *ntokens)
  * (at most CG_MAX_QEXPR): the WHERE list (quals / qual_expr), aggregate FILTERs (filter_quals / filter_expr[a]) and the
- * predicate arguments of bool_and / bool_or / every (filter_quals / arg_expr[a]).  An atom is "Var op Const", a bare bool
- * Var, NOT over a bare bool Var, an IN / NOT IN list over a Var (its list goes to desc's list table) or "Var IS [NOT] NULL".
+ * predicate arguments of bool_and / bool_or / every (filter_quals / arg_expr[a]).  An atom is "Var op Const", "Var op Var"
+ * (column_pair_supported), a bare bool Var, NOT over a bare bool Var, an IN / NOT IN list over a Var (its list goes to
+ * desc's list table) or "Var IS [NOT] NULL".
  * false when a node is anything else or the tree is too big */
 static bool
 translate_where(Node *node, TupleDesc tupdesc, CgScanDesc *desc, CgQual *atoms, int32_t *natoms, int max_atoms, int8_t *tokens,
