@@ -103,6 +103,11 @@ class CgScanStats(C.Structure):
                 ("kernel_ms", C.c_double), ("h2d_bytes", C.c_int64)]
 
 
+class CgJoinSide(C.Structure):
+    _fields_ = [("d_cols", C.POINTER(C.c_void_p)), ("d_nulls", C.POINTER(C.c_void_p)), ("ncols", C.c_int32),
+                ("key", C.c_int32), ("nrows", C.c_int64)]
+
+
 class CgGenColumn(C.Structure):
     _fields_ = [("attlen", C.c_int32), ("kind", C.c_int32), ("lo", C.c_int64), ("hi", C.c_int64),
                 ("null_ppm", C.c_uint32), ("reserved", C.c_uint32)]
@@ -184,6 +189,8 @@ SYMBOLS = [
     ("cg_gen_relation_view", C.c_int, [_P, C.POINTER(CgRelation)]),
     ("cg_gen_relation_free", None, [_P]),
     ("cg_join_rows", C.c_int, [_P, _P, _P, C.c_int64, _P, _P, _P, C.c_int64, C.c_int64, _P, _P, _P, C.POINTER(C.c_int64)]),
+    ("cg_join_aggregate", C.c_int, [C.POINTER(CgJoinSide), C.POINTER(CgJoinSide), C.POINTER(CgColumnDesc), C.POINTER(CgScanDesc), _P,
+                                    C.POINTER(CgScanStats)]),
     ("cg_partial_merge_values", C.c_int, [_P, C.c_int64, _P, _P, _P, _P, _P, _P, _P]),
     ("cg_agg_column", C.c_int, [C.c_int32, C.c_int32, _P, _P, C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int64),
                                C.POINTER(C.c_uint64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),

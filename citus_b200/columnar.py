@@ -518,6 +518,36 @@ class GpuColumnarAgg:
         check(lib().cg_scan_relation(C.byref(rel.view), C.byref(self.desc), self.h, C.byref(st) if want_stats else None))
         return st
 
+    def join_aggregate(self, build_ptrs, build_key, nbuild, probe_ptrs, probe_key, nprobe, build_null_ptrs=None,
+                       probe_null_ptrs=None, want_stats=True, columns=None):
+        """cg_join_aggregate: this partial's query over the equi-join of two device-resident sides (device pointers of
+        int64 columns, as join_rows takes them; a null list holds None or a device byte array per column).  The joined
+        row's attributes are the build columns, then the probe columns; the partial's column descriptors describe them
+        (columns = other descriptors [(attlen, type_class)] for this call only)"""
+        keep = []
+
+        def side(ptrs, nulls, key, n):
+            cols = (C.c_void_p * len(ptrs))(*ptrs)
+            nul = None if nulls is None else (C.c_void_p * len(ptrs))(*nulls)
+            keep.extend([cols, nul])
+            s = capi.CgJoinSide()
+            s.d_cols = C.cast(cols, C.POINTER(C.c_void_p))
+            s.d_nulls = None if nul is None else C.cast(nul, C.POINTER(C.c_void_p))
+            s.ncols, s.key, s.nrows = len(ptrs), key, n
+            return s
+
+        b = side(build_ptrs, build_null_ptrs, build_key, nbuild)
+        p = side(probe_ptrs, probe_null_ptrs, probe_key, nprobe)
+        cols = self.cols
+        if columns is not None:
+            cols = (CgColumnDesc * len(columns))()
+            for i, (l, t) in enumerate(columns):
+                cols[i].attlen, cols[i].type_class = l, t
+        st = CgScanStats()
+        check(lib().cg_join_aggregate(C.byref(b), C.byref(p), cols, C.byref(self.desc), self.h,
+                                      C.byref(st) if want_stats else None))
+        return st
+
     def ngroups(self):
         n = C.c_int64()
         check(lib().cg_partial_ngroups(self.h, C.byref(n)))

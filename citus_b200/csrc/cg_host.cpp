@@ -1326,6 +1326,97 @@ extern "C" int cg_scan_shard(const CgShard *sh, const CgScanDesc *desc, CgPartia
 	return stats_end(ctx, into, before, filtered, selected.size(), bytes, stats);
 }
 
+/* the comparison class of a join key column (0 = float, not a join key) and its numeric scale */
+static int join_key_class(const CgColumnDesc &c, int *scale)
+{
+	*scale = cg_type_class(c) == CG_TYPE_NUMERIC ? cg_type_scale(c) : 0;
+	switch (cg_type_class(c))
+	{
+		case CG_TYPE_INT:
+		case CG_TYPE_NUMERIC: return 1;
+		case CG_TYPE_BPCHAR1: return 2;
+		default: return 0;
+	}
+}
+
+extern "C" int cg_join_aggregate(const CgJoinSide *build, const CgJoinSide *probe, const CgColumnDesc *columns, const CgScanDesc *desc,
+								 CgPartial *into, CgScanStats *stats)
+{
+	CgContext *ctx = cg_ctx();
+	if (!ctx) return CG_EINVAL;
+	if (!build || !probe || !columns || !desc || !into) return cg_set_error(CG_EINVAL, "NULL argument");
+	const CgJoinSide *sides[2] = {build, probe};
+	for (const CgJoinSide *s : sides)
+	{
+		if (s->ncols < 1 || s->key < 0 || s->key >= s->ncols || s->nrows < 0 || !s->d_cols)
+			return cg_set_error(CG_EINVAL, "join side: ncols %d, key %d, nrows %lld", s->ncols, s->key, (long long) s->nrows);
+		if (!s->d_cols[s->key]) return cg_set_error(CG_EINVAL, "NULL join key column");
+	}
+	if ((int64_t) build->ncols + probe->ncols > 256) return cg_set_error(CG_EUNSUPPORTED, "more than 256 attributes");
+	const int natts = build->ncols + probe->ncols;
+	for (int a = 0; a < desc->naggs && a < CG_MAX_AGGS; a++)
+		if (desc->aggs[a].term_abs_bound != 0)
+			return cg_set_error(CG_EINVAL, "aggregate %d has a term_abs_bound: the joined rows are not known before the probe, so no bound holds", a);
+	int sb, sp;
+	const int kb = join_key_class(columns[build->key], &sb), kp = join_key_class(columns[build->ncols + probe->key], &sp);
+	if (kb == 0 || kp == 0) return cg_set_error(CG_EUNSUPPORTED, "float join key");
+	if (kb != kp || sb != sp) return cg_set_error(CG_EUNSUPPORTED, "join keys of different classes or numeric scales");
+	KPlan plan;
+	bool all8 = false;
+	std::vector<uint64_t> codes;
+	int rc = cg_build_plan(desc, columns, natts, nullptr, into, &plan, &all8, &codes);
+	if (rc) return rc;
+	/* what the kernels read of each side: its key and its plan columns */
+	uint64_t bytes = 0;
+	for (int si = 0; si < 2; si++)
+	{
+		const CgJoinSide &s = *sides[si];
+		const int base = si ? build->ncols : 0;
+		std::vector<bool> read(s.ncols, false);
+		read[s.key] = true;
+		for (int c = 0; c < plan.ncols; c++)
+			if (plan.slot[c] >= base && plan.slot[c] < base + s.ncols) read[plan.slot[c] - base] = true;
+		for (int i = 0; i < s.ncols; i++)
+		{
+			if (!read[i]) continue;
+			if (!s.d_cols[i]) return cg_set_error(CG_EINVAL, "NULL device pointer for column %d of the %s side", i, si ? "probe" : "build");
+			bytes += 8 * (uint64_t) s.nrows + (s.d_nulls && s.d_nulls[i] ? (uint64_t) s.nrows : 0);
+		}
+	}
+	if (build->nrows == 0 || probe->nrows == 0)
+	{
+		if (stats) memset(stats, 0, sizeof *stats);
+		return CG_OK;
+	}
+	rc = before_scan(ctx, into);
+	if (rc) return rc;
+	unsigned long long before[3];
+	rc = stats_begin(ctx, into, stats, before);
+	if (rc) return rc;
+	rc = upload_sets(ctx, into, codes, &plan);
+	if (rc) return rc;
+	if (stats)
+	{
+		rc = cg_chain_end(ctx, ctx->compute);
+		if (rc) return rc;
+		CG_CUDA(cudaEventRecord(ctx->ev_a, ctx->compute));
+	}
+	rc = cg_launch_join_aggregate(ctx, plan, sides, ctx->compute);
+	if (rc) return rc;
+	rc = after_launch(ctx, into, false, false, 0);
+	if (rc) return rc;
+	if (!stats) return CG_OK;
+	rc = cg_chain_end(ctx, ctx->compute);
+	if (rc) return rc;
+	CG_CUDA(cudaEventRecord(ctx->ev_b, ctx->compute));
+	rc = stats_end(ctx, into, before, 0, 0, bytes, stats);
+	if (rc) return rc;
+	float ms = 0;
+	CG_CUDA(cudaEventElapsedTime(&ms, ctx->ev_a, ctx->ev_b));
+	stats->kernel_ms = ms;
+	return CG_OK;
+}
+
 /* ------------------------------------------------------------------------------ *
  *  DMA staging: when the relation's pages sit in pinned (registered) host memory the copy
  *  engine moves them itself, so no host core touches the data: one 1-D cudaMemcpyAsync per

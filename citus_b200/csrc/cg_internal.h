@@ -596,6 +596,10 @@ int cg_partition_route_scatter_async(const int64_t *d_keys, const uint8_t *d_nul
 									 const int64_t *const *d_cols, int32_t ncols, int64_t *const *d_out, int64_t *d_counts,
 									 cudaEvent_t after_counts, const CgScatterHook *peer_hook = nullptr);
 
+/* cg_join.cu: build the chained join table over sides[0] and run the plan over the joined rows of sides[1] (cg_join_aggregate;
+ * a plan column's slot is its joined-row attribute: build columns first, then probe columns), on `stream` */
+int cg_launch_join_aggregate(CgContext *ctx, const KPlan &plan, const CgJoinSide *const sides[2], cudaStream_t stream);
+
 /* cg_comm.cu */
 void cg_comm_set_peer_window(int on);
 

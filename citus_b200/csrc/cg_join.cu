@@ -19,10 +19,15 @@
  * Open addressing over a separate key array (like the GROUP BY table in cg_scan.cu), load factor
  * <= 1/2, 64-bit CAS to claim a slot; values are one 32-byte sector per slot
  * [rows, sum of low 32 bits, sum of payload >> 32, unused].
+ *
+ * Two more forms follow: cg_join_rows emits the joined rows into device arrays, and cg_join_aggregate runs any scan
+ * plan (WHERE tree, group key, aggregates) over the joined rows into a CgPartial, through the row path the
+ * interpretive scan kernel uses (cg_device.cuh).  Both build one chained table over the build side.
  */
 #include <vector>
 
 #include "cg_internal.h"
+#include "cg_device.cuh"
 
 #define CGJ_THREADS 256
 #define CGJ_EMPTY ((long long) 0x8000000000000000ull)
@@ -245,6 +250,39 @@ cg_join_rows_build_kernel(JoinRowsTable T, const long long *keys, const uint8_t 
 	}
 }
 
+static size_t join_a64(size_t x) { return (x + 63) & ~(size_t) 63; }
+
+/*
+ * The chained table over the build keys, in one stream-ordered allocation (no host synchronisation): init and build
+ * launches on `stream`.  The allocation holds the table, then `extra` bytes for the caller (*d_extra, 64-byte aligned),
+ * then two zeroed words (*d_words): [0] is the caller's, [1] counts build rows that found no slot.  That count stays 0:
+ * the table has at least 2 * nbuild slots and a claim probes every one of them.
+ */
+static int join_rows_table_build(CgContext *ctx, const int64_t *d_keys, const uint8_t *d_nulls, int64_t nbuild, size_t extra,
+								 cudaStream_t stream, CgAsyncBuf *mem, JoinRowsTable *T, uint8_t **d_extra, unsigned long long **d_words)
+{
+	join_table_size(nbuild, &T->cap, &T->shift);
+	const size_t kb = join_a64((T->cap + 1) * 8), cb = join_a64((T->cap + 1) * 4), hb = join_a64((T->cap + 1) * 8),
+				 nb = join_a64((size_t) nbuild * 8);
+	if (mem->alloc(kb + cb + hb + nb + extra + 64, stream) != cudaSuccess)
+	{
+		cudaGetLastError();
+		return cg_set_error(CG_ENOMEM, "cudaMallocAsync of %zu bytes for the join failed", kb + cb + hb + nb + extra);
+	}
+	uint8_t *d = mem->as<uint8_t>();
+	T->keys = (long long *) d; T->count = (unsigned int *) (d + kb); T->head = (long long *) (d + kb + cb); T->next = (long long *) (d + kb + cb + hb);
+	*d_extra = d + kb + cb + hb + nb;
+	*d_words = (unsigned long long *) (d + kb + cb + hb + nb + extra);
+	T->errors = *d_words + 1;
+	CG_CUDA(cudaMemsetAsync(*d_words, 0, 16, stream));
+	const unsigned blocks = (unsigned) (ctx->sm_count * 8);
+	cg_join_rows_init_kernel<<<blocks, CGJ_THREADS, 0, stream>>>(*T);
+	CG_CUDA(cudaGetLastError()); g_cg_launches++;
+	cg_join_rows_build_kernel<<<blocks, CGJ_THREADS, 0, stream>>>(*T, (const long long *) d_keys, d_nulls, (long long) nbuild);
+	CG_CUDA(cudaGetLastError()); g_cg_launches++;
+	return CG_OK;
+}
+
 /* matches[r] = rows probe row r joins; block sums for the scan (partition_scan_blocks with one partition) */
 __global__ void __launch_bounds__(CGJ_THREADS)
 cg_join_rows_count_kernel(JoinRowsTable T, const long long *keys, const uint8_t *nulls, long long n, unsigned int *matches,
@@ -317,29 +355,14 @@ extern "C" int cg_join_rows(const int64_t *d_build_keys, const uint8_t *d_build_
 	*nrows = 0;
 	if (nbuild == 0 || nprobe == 0) return CG_OK;
 	JoinRowsTable T;
-	join_table_size(nbuild, &T.cap, &T.shift);
 	const long long nblocks = (nprobe + CGJ_THREADS - 1) / CGJ_THREADS;
-	auto a16 = [](size_t x) { return (x + 63) & ~(size_t) 63; };
-	const size_t kb = a16((T.cap + 1) * 8), cb = a16((T.cap + 1) * 4), hb = a16((T.cap + 1) * 8), nb = a16((size_t) nbuild * 8),
-				 mb = a16((size_t) nprobe * 4), bb = a16((size_t) nblocks * 8);
+	const size_t mb = join_a64((size_t) nprobe * 4), bb = join_a64((size_t) nblocks * 8);
 	CgAsyncBuf mem;
-	if (mem.alloc(kb + cb + hb + nb + mb + bb + 64, ctx->compute) != cudaSuccess)
-	{
-		cudaGetLastError();
-		return cg_set_error(CG_ENOMEM, "cudaMallocAsync of %zu bytes for the join failed", kb + cb + hb + nb + mb + bb);
-	}
-	uint8_t *d = mem.as<uint8_t>();
-	T.keys = (long long *) d; T.count = (unsigned int *) (d + kb); T.head = (long long *) (d + kb + cb); T.next = (long long *) (d + kb + cb + hb);
-	unsigned int *d_matches = (unsigned int *) (d + kb + cb + hb + nb);
-	unsigned long long *d_block = (unsigned long long *) (d + kb + cb + hb + nb + mb);
-	unsigned long long *d_tot = (unsigned long long *) (d + kb + cb + hb + nb + mb + bb);     /* [0] total rows, [1] errors */
-	T.errors = d_tot + 1;
-	CG_CUDA(cudaMemsetAsync(d_tot, 0, 16, ctx->compute));
-	const unsigned blocks = (unsigned) (ctx->sm_count * 8);
-	cg_join_rows_init_kernel<<<blocks, CGJ_THREADS, 0, ctx->compute>>>(T);
-	CG_CUDA(cudaGetLastError()); g_cg_launches++;
-	cg_join_rows_build_kernel<<<blocks, CGJ_THREADS, 0, ctx->compute>>>(T, (const long long *) d_build_keys, d_build_nulls, (long long) nbuild);
-	CG_CUDA(cudaGetLastError()); g_cg_launches++;
+	uint8_t *d_extra;
+	unsigned long long *d_tot;     /* [0] total rows, [1] errors */
+	if (int rc = join_rows_table_build(ctx, d_build_keys, d_build_nulls, nbuild, mb + bb, ctx->compute, &mem, &T, &d_extra, &d_tot)) return rc;
+	unsigned int *d_matches = (unsigned int *) d_extra;
+	unsigned long long *d_block = (unsigned long long *) (d_extra + mb);
 	cg_join_rows_count_kernel<<<(unsigned) nblocks, CGJ_THREADS, 0, ctx->compute>>>(T, (const long long *) d_probe_keys, d_probe_nulls, (long long) nprobe,
 																				  d_matches, d_block);
 	CG_CUDA(cudaGetLastError()); g_cg_launches++;
@@ -361,4 +384,126 @@ extern "C" int cg_join_rows(const int64_t *d_build_keys, const uint8_t *d_build_
 	CG_CUDA(cudaGetLastError()); g_cg_launches++;
 	CG_CUDA(cudaStreamSynchronize(ctx->compute));
 	return CG_OK;
+}
+
+/* ------------------------------------------------------------------------------ *
+ *  Any scan query over the joined rows (cg_join_aggregate):
+ *      SELECT <group key, aggregates> FROM build b JOIN probe p USING (key) WHERE ... GROUP BY ...
+ *  the Agg <- HashJoin of the MERGE task (planner/multi_physical_planner.c:598-687 gives it the worker half of the
+ *  aggregates, the GROUP BY and the WHERE).  The build side goes into cg_join_rows' chained table; one thread per probe
+ *  row loads the probe side's plan columns once (coalesced), finds the key's slot and walks the chain, and for every build
+ *  row gathers the build side's plan columns and hands the joined row to the row path of the interpretive scan kernel
+ *  (process_row, cg_device.cuh).  The joined rows are never materialised.
+ * ------------------------------------------------------------------------------ */
+/* where plan column c of the joined row comes from: column col[c] (null array nul[c], may be NULL) of the probe side
+ * (probe bit c set) or of the build side */
+struct JoinAggCols
+{
+	const long long *col[CG_KMAX_COLS];
+	const uint8_t *nul[CG_KMAX_COLS];
+	uint32_t probe;
+};
+
+template <int NCC, int NAC, int MODE, bool VAR>
+__global__ void __launch_bounds__(CGJ_THREADS, 4)
+cg_join_agg_kernel(const __grid_constant__ KPlan P, const JoinAggCols J, const JoinRowsTable T, const long long *keys, const uint8_t *key_nulls,
+				   long long n)
+{
+	ThreadAcc<NAC, VAR> acc;
+	thread_acc_init(P, acc);
+	uint32_t removed = 0;
+	unsigned long long joined = 0;
+	for (long long r = (long long) blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (long long) gridDim.x * blockDim.x)
+	{
+		if (key_nulls && key_nulls[r]) continue;
+		const long long key = keys[r];
+		const unsigned long long slot = key == CGJ_EMPTY ? T.cap : join_find<FIND>(T.keys, T.cap, T.shift, key);
+		if (slot == ~0ull) continue;
+		long long b = (long long) __ldg((const unsigned long long *) T.head + slot);
+		if (b < 0) continue;
+		int64_t v[NCC];
+		uint32_t pnull = 0;
+#pragma unroll
+		for (int c = 0; c < NCC; c++)
+		{
+			v[c] = 0;
+			if (c < P.ncols && ((J.probe >> c) & 1u))
+			{
+				v[c] = J.col[c][r];
+				if (J.nul[c] && J.nul[c][r]) pnull |= 1u << c;
+			}
+		}
+		for (; b >= 0; b = (long long) __ldg((const unsigned long long *) T.next + b))
+		{
+			uint32_t nullmask = pnull;
+#pragma unroll
+			for (int c = 0; c < NCC; c++)
+				if (c < P.ncols && !((J.probe >> c) & 1u))
+				{
+					v[c] = __ldg(J.col[c] + b);
+					if (J.nul[c] && __ldg(J.nul[c] + b)) nullmask |= 1u << c;
+				}
+			joined++;
+			process_row<NCC, NAC, MODE, VAR>(P, v, nullmask, acc, removed);
+		}
+	}
+	flush_thread<NAC, MODE, VAR>(P, acc, removed, joined);
+}
+
+template <int MODE, bool VAR>
+static int launch_join_agg(CgContext *ctx, const KPlan &plan, const JoinAggCols &J, const JoinRowsTable &T, const long long *keys,
+						   const uint8_t *key_nulls, long long n, cudaStream_t stream)
+{
+	auto kernel = cg_join_agg_kernel<CG_KMAX_COLS, CG_MAX_AGGS, MODE, VAR>;
+	int occ = 0;
+	CG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, CGJ_THREADS, 0));
+	if (occ < 1) occ = 1;
+	long long grid = (long long) ctx->sm_count * occ, need = (n + CGJ_THREADS - 1) / CGJ_THREADS;
+	if (grid > need) grid = need;
+	bool overlap;
+	int rc = cg_chain_scan(ctx, stream, false, &overlap);     /* an ordinary launch: ends a chain */
+	if (rc) return rc;
+	kernel<<<(unsigned) grid, CGJ_THREADS, 0, stream>>>(plan, J, T, keys, key_nulls, n);
+	CG_CUDA(cudaGetLastError()); g_cg_launches++;
+	return CG_OK;
+}
+
+int cg_launch_join_aggregate(CgContext *ctx, const KPlan &plan, const CgJoinSide *const sides[2], cudaStream_t stream)
+{
+	const CgJoinSide &b = *sides[0], &p = *sides[1];
+	JoinAggCols J;
+	memset(&J, 0, sizeof J);
+	for (int c = 0; c < plan.ncols; c++)
+	{
+		/* a plan column's slot is its joined-row attribute: build columns first, then probe columns */
+		const bool probe = plan.slot[c] >= b.ncols;
+		const CgJoinSide &s = probe ? p : b;
+		const int i = probe ? plan.slot[c] - b.ncols : plan.slot[c];
+		J.col[c] = (const long long *) s.d_cols[i];
+		J.nul[c] = s.d_nulls ? s.d_nulls[i] : nullptr;
+		if (probe) J.probe |= 1u << c;
+	}
+	int rc = cg_chain_end(ctx, stream);
+	if (rc) return rc;
+	JoinRowsTable T;
+	CgAsyncBuf mem;
+	uint8_t *d_extra;
+	unsigned long long *d_words;
+	rc = join_rows_table_build(ctx, b.d_cols[b.key], b.d_nulls ? b.d_nulls[b.key] : nullptr, b.nrows, 0, stream, &mem, &T, &d_extra, &d_words);
+	if (rc) return rc;
+	const long long *keys = (const long long *) p.d_cols[p.key];
+	const uint8_t *key_nulls = p.d_nulls ? p.d_nulls[p.key] : nullptr;
+	const bool var = cg_plan_has_variance(plan.aggs, plan.naggs);
+	switch (plan.mode)
+	{
+		case CG_MODE_GLOBAL:
+			return var ? launch_join_agg<CG_MODE_GLOBAL, true>(ctx, plan, J, T, keys, key_nulls, p.nrows, stream)
+					   : launch_join_agg<CG_MODE_GLOBAL, false>(ctx, plan, J, T, keys, key_nulls, p.nrows, stream);
+		case CG_MODE_DENSE:
+			return var ? launch_join_agg<CG_MODE_DENSE, true>(ctx, plan, J, T, keys, key_nulls, p.nrows, stream)
+					   : launch_join_agg<CG_MODE_DENSE, false>(ctx, plan, J, T, keys, key_nulls, p.nrows, stream);
+		default:
+			return var ? launch_join_agg<CG_MODE_HASH, true>(ctx, plan, J, T, keys, key_nulls, p.nrows, stream)
+					   : launch_join_agg<CG_MODE_HASH, false>(ctx, plan, J, T, keys, key_nulls, p.nrows, stream);
+	}
 }

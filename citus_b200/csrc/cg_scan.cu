@@ -27,98 +27,6 @@
 #include "cg_device.cuh"
 
 /*
- * Find (or claim) the table entry of a group key.  Returns the word pointer of the
- * entry (word 0 = rows in group) or NULL after raising an error flag.
- *   dense: entry = key - key_min, NULL key -> entry `capacity`
- *   hash : open addressing, linear probing over a separate key array (8 B per slot, so the
- *          probed working set is a quarter of an array-of-structs table), 64-bit CAS to claim
- *          a slot; the NULL group and the key equal to the EMPTY sentinel live in two extra
- *          entries behind the addressable ones
- */
-template <int MODE>
-__device__ __forceinline__ uint64_t *find_entry(const KPlan &P, int64_t key, bool key_null)
-{
-	if (MODE == CG_MODE_DENSE)
-	{
-		uint64_t slot = dense_slot_of_packed(P, key, key_null);
-		return slot == ~0ull ? nullptr : P.table + slot * (uint64_t) P.stride;
-	}
-	else
-	{
-		if (key_null) return P.table + P.capacity * (uint64_t) P.stride;
-		if (key == CG_HASH_EMPTY) return P.table + (P.capacity + 1) * (uint64_t) P.stride;
-		uint64_t mask = P.capacity - 1;
-		uint64_t h = cg_home_slot(key, P.hash_shift);
-		for (uint32_t probes = 0; probes < 8192; probes++)
-		{
-			unsigned long long *kp = (unsigned long long *) (P.hkeys + h);
-			long long cur = (long long) __ldcg(kp);     /* L2: keys only ever go EMPTY -> key */
-			if (cur == key) return P.table + h * (uint64_t) P.stride;
-			if (cur == CG_HASH_EMPTY)
-			{
-				long long old = (long long) atomicCAS(kp, (unsigned long long) CG_HASH_EMPTY, (unsigned long long) key);
-				if (old == CG_HASH_EMPTY || old == key) return P.table + h * (uint64_t) P.stride;
-			}
-			h = (h + 1) & mask;
-		}
-		atomicOr(P.stats + 2, CG_ERRFLAG_TABLE_FULL);
-		return nullptr;
-	}
-}
-
-/* per-thread accumulators of the plain-aggregate mode */
-template <int NAC, bool VAR>
-struct ThreadAcc
-{
-	uint64_t w[NAC][3];     /* [agg][word0, word0+1, NULL-input count] */
-	uint64_t rows;
-	uint64_t q[NAC][VAR ? 4 : 1];   /* VAR: [agg][sum(x^2) word qword + l] */
-};
-
-template <int NCC, int NAC, int MODE, bool VAR>
-__device__ __forceinline__ void process_row(const KPlan &P, const int64_t (&v)[NCC], uint32_t nullmask,
-											ThreadAcc<NAC, VAR> &acc, uint32_t &removed)
-{
-	/* K3: WHERE tree, three-valued: an atom on a NULL input is not TRUE */
-	if (!eval_where<NCC>(P, v, nullmask))
-	{
-		removed++;
-		return;
-	}
-	if (MODE != CG_MODE_GLOBAL)
-	{
-		int64_t key;
-		bool key_null;
-		if (!group_key<NCC>(P, v, nullmask, key, key_null)) return;
-		uint64_t *entry = find_entry<MODE>(P, key, key_null);
-		if (entry != nullptr) global_accumulate<NCC, NAC, VAR>(P, entry, v, nullmask);
-		return;
-	}
-	acc.rows++;
-	auto term = [&](int a, const KAgg &g, bool noinput, uint64_t w0, uint64_t w1) {
-		if (noinput) acc.w[a][2]++;
-		else
-		{
-			acc.w[a][0] = word_combine(P.wordop[g.word0], acc.w[a][0], w0);
-			if (two_sum_limbs<VAR>(g)) acc.w[a][1] += w1;
-		}
-	};
-	if constexpr (VAR)
-		row_terms<NCC, NAC, true>(P, v, nullmask, term, [&](int a, const KAgg &g, uint64_t lo, uint64_t hi) {
-			/* a thread's limb sums grow by < 2^32 per row; the one-word form is bounded by the table's own guarantee */
-			if (g.qlimbs == 1) acc.q[a][0] += lo;
-			else
-			{
-#pragma unroll
-				for (int l = 0; l < 4; l++)
-					if (l < g.qlimbs) acc.q[a][l] += square_limb(lo, hi, l);
-			}
-		});
-	else
-		row_terms<NCC, NAC>(P, v, nullmask, term);
-}
-
-/*
  * The fused kernel.  Persistent CTAs stride over the selected chunk groups; inside a
  * chunk group every thread takes two consecutive rows per step (one 16-byte load per
  * 8-byte column) and U steps are loaded before any is consumed.
@@ -131,19 +39,7 @@ __global__ void __launch_bounds__(CG_THREADS, 4)
 cg_scan_kernel(const __grid_constant__ KPlan P)
 {
 	ThreadAcc<NAC, VAR> acc;
-	acc.rows = 0;
-#pragma unroll
-	for (int a = 0; a < NAC; a++)
-	{
-		acc.w[a][0] = (a < P.naggs && P.aggs[a].kind != CG_AGG_COUNT_STAR) ? word_identity(P.wordop[P.aggs[a].word0]) : 0;
-		acc.w[a][1] = 0;
-		acc.w[a][2] = 0;
-		if constexpr (VAR)
-		{
-#pragma unroll
-			for (int l = 0; l < 4; l++) acc.q[a][l] = 0;
-		}
-	}
+	thread_acc_init(P, acc);
 	uint32_t removed = 0;
 	unsigned long long scanned = 0;
 	const uint32_t tid = threadIdx.x;
@@ -231,53 +127,8 @@ cg_scan_kernel(const __grid_constant__ KPlan P)
 		}
 	}
 
-	/* counters and (plain aggregate) the block's accumulators: warp shuffle reduce, then one
-	 * atomic per warp and word */
-	unsigned long long rem = warp_reduce_word(removed, CG_WORD_ADD);
-	unsigned long long scn = warp_reduce_word(scanned, CG_WORD_ADD);
-	if ((tid & 31) == 0)
-	{
-		if (scn) atomicAdd(P.stats + 0, scn);
-		if (rem) atomicAdd(P.stats + 1, rem);
-	}
-	if (MODE == CG_MODE_GLOBAL)
-	{
-		uint64_t rows_passed = warp_reduce_word(acc.rows, CG_WORD_ADD);
-		if ((tid & 31) == 0 && rows_passed) atomicAdd((unsigned long long *) P.table, (unsigned long long) rows_passed);
-#pragma unroll
-		for (int a = 0; a < NAC; a++)
-		{
-			if (a < P.naggs && (P.aggs[a].kind != CG_AGG_COUNT_STAR || P.aggs[a].filt))
-			{
-				const KAgg &g = P.aggs[a];
-				uint64_t nulls = warp_reduce_word(acc.w[a][2], CG_WORD_ADD);
-				uint64_t x0 = warp_reduce_word(acc.w[a][0], P.wordop[g.word0]);
-				uint64_t x1 = warp_reduce_word(acc.w[a][1], CG_WORD_ADD);
-				if ((tid & 31) == 0)
-				{
-					if (nulls) atomicAdd((unsigned long long *) P.table + g.nullword, (unsigned long long) nulls);
-					if (g.kind != CG_AGG_COUNT && g.kind != CG_AGG_COUNT_STAR)
-					{
-						if (x0 != word_identity(P.wordop[g.word0])) word_apply_global(P.table + g.word0, P.wordop[g.word0], x0);
-						if (two_sum_limbs<VAR>(g) && x1)
-							atomicAdd((unsigned long long *) P.table + g.word0 + 1, (unsigned long long) x1);
-					}
-				}
-				if constexpr (VAR)
-				{
-					if (g.kind == CG_AGG_VARIANCE)
-					{
-#pragma unroll
-						for (int l = 0; l < 4; l++)
-						{
-							const uint64_t x = warp_reduce_word(acc.q[a][l], CG_WORD_ADD);
-							if ((tid & 31) == 0 && l < g.qlimbs && x) atomicAdd((unsigned long long *) P.table + g.qword + l, (unsigned long long) x);
-						}
-					}
-				}
-			}
-		}
-	}
+	/* counters and (plain aggregate) the block's accumulators */
+	flush_thread<NAC, MODE, VAR>(P, acc, removed, scanned);
 }
 
 template <int NCC, int NAC, int MODE, bool ALL8, int U, bool VAR = false>

@@ -645,6 +645,49 @@ int cg_join_rows(const int64_t *d_build_keys, const uint8_t *d_build_nulls, cons
 				 const int64_t *d_probe_keys, const uint8_t *d_probe_nulls, const int64_t *d_probe_payload, int64_t nprobe,
 				 int64_t capacity, int64_t *d_out_key, int64_t *d_out_build_payload, int64_t *d_out_probe_payload, int64_t *nrows);
 
+/* One side of a join: ncols device arrays of nrows values each, in the scan kernels' decoded form (integer types
+ * sign-extended to int64, bool 0 / 1, char(1) as the unsigned byte, numeric(p, s) as value * 10^s, float4 / float8 as
+ * float8 bits -- what cg_comm_exchange_result delivers for int columns).  d_nulls: NULL, or per column NULL or a device
+ * byte array (non-zero = NULL).  key = index of the join key column among them. */
+typedef struct CgJoinSide
+{
+	const int64_t *const *d_cols;
+	const uint8_t *const *d_nulls;
+	int32_t ncols;
+	int32_t key;
+	int64_t nrows;
+} CgJoinSide;
+
+/* Any scan query over the equi-join of two device-resident sides, folded into `into`:
+ *     SELECT <desc's group key and aggregates> FROM build b JOIN probe p ON b.key = p.key WHERE <desc's WHERE tree> GROUP BY ...
+ * which is what the MERGE task of a repartition join runs (planner/multi_physical_planner.c:598-687 puts the worker
+ * half of the aggregates, the GROUP BY and the WHERE over the join).
+ *   Attributes.  A joined row has build->ncols + probe->ncols attributes, build columns first, then probe columns;
+ *   columns[] describes them and desc refers to them by that numbering everywhere (WHERE atoms, group columns,
+ *   aggregate factors, FILTER and bool-argument atoms, IN lists, column atoms).  A factor product or a column atom may
+ *   mix the sides (sum(b.x * p.y), WHERE b.d < p.d).  into must come from cg_partial_create with the same desc and
+ *   columns (a different aggregate list or key form is CG_EINVAL).
+ *   Join.  Keys are equal when their int64 values are equal; a NULL key joins nothing, on either side; INT64_MIN is a key
+ *   like any other.  The two key columns must be of one class: integer-like with equal numeric scale (int widths may
+ *   differ, as int48eq allows) or char(1) with char(1).  A float key, or integer-like keys of different scales, is
+ *   CG_EUNSUPPORTED.
+ *   Everything else follows a scan row: three-valued WHERE, NULL inputs, FILTER, bool arguments, overflow checks,
+ *   composite codes (the caller supplies key_col_min / key_col_max), dense or hash tables and the error flags.
+ *   enable_qual_pushdown has no effect: there are no skip lists, so nothing is skipped.
+ *   term_abs_bound must be 0 in every aggregate (CG_EINVAL otherwise): the number of joined rows is not known before the
+ *   probe, so no bound * max_rows proof can hold; sums keep two limb words and every integer term is overflow-checked.
+ *   Asynchronous on the library's stream unless stats is given, like cg_scan_shard: kernel-raised errors surface at the
+ *   next call that reads the partial.  The join table is allocated in stream order, without a host synchronisation, so
+ *   one call per local partition can be enqueued back to back.
+ *   stats: rows_scanned = joined rows handed to WHERE, rows_removed_by_filter, rows_passed; kernel_ms = device time of
+ *   the build and the probe-aggregate launches; bytes_scanned = 8 bytes per row for the key column and each plan column
+ *   of a side, plus one byte per row for each null array read; the chunk-group fields and h2d_bytes are 0.
+ *   Refusals: CG_EINVAL for a NULL pointer for a key or plan column, key or ncols out of range, nrows < 0, a nonzero
+ *   term_abs_bound or a desc that does not match the partial; CG_EUNSUPPORTED for plans over the kernels' column limit
+ *   (8), as for a scan.  nrows == 0 on either side is a no-op that returns CG_OK. */
+int cg_join_aggregate(const CgJoinSide *build, const CgJoinSide *probe, const CgColumnDesc *columns, const CgScanDesc *desc,
+					  CgPartial *into, CgScanStats *stats);
+
 /* exact bounds from the skip lists (min/max of every chunk that survives chunk-group
  * skipping): the packed group key range and |argument| of every aggregate (0 = unknown,
  * e.g. a chunk without min/max).  Feed them to cg_partial_create / CgAggSpec.term_abs_bound. */
