@@ -32,6 +32,8 @@ CG_MAX_QEXPR, CG_QX_AND, CG_QX_OR = 16, -1, -2
 CG_MAX_FILTER_QUALS = 8
 CG_MAX_WORDS = 32
 CG_MAX_IN_LISTS, CG_MAX_IN_VALUES, CG_IN_REFUTE_MAX = 8, 1024, 100
+CG_MAX_CASE_ARMS = 16
+CG_CASE_NULL, CG_CASE_CONST, CG_CASE_PRODUCT = 0, 1, 2
 CG_PSTATE_PACKED_DIRTY, CG_PSTATE_WIDE_DIRTY, CG_PSTATE_READ_PACKED_DIRECT, CG_PSTATE_TABLE_INITIALISED = 1, 2, 4, 8
 
 
@@ -81,6 +83,11 @@ class CgAggSpec(C.Structure):
                 ("term_abs_bound", C.c_int64)]
 
 
+class CgCaseArm(C.Structure):
+    _fields_ = [("nwhen", C.c_int32), ("when", C.c_int8 * CG_MAX_QEXPR), ("form", C.c_int32), ("nfactors", C.c_int32),
+                ("column", C.c_int32 * 3), ("a", C.c_int64 * 3), ("b", C.c_int64 * 3)]
+
+
 class CgScanDesc(C.Structure):
     _fields_ = [("nquals", C.c_int32), ("quals", CgQual * CG_MAX_QUALS),
                 ("enable_qual_pushdown", C.c_int32), ("ngroup_cols", C.c_int32),
@@ -93,7 +100,9 @@ class CgScanDesc(C.Structure):
                 ("composite_key", C.c_int32), ("key_col_min", C.c_int64 * CG_MAX_GROUP_COLS),
                 ("key_col_max", C.c_int64 * CG_MAX_GROUP_COLS),
                 ("nin_lists", C.c_int32), ("in_lists", CgInList * CG_MAX_IN_LISTS),
-                ("nin_values", C.c_int32), ("in_values", C.c_int64 * CG_MAX_IN_VALUES)]
+                ("nin_values", C.c_int32), ("in_values", C.c_int64 * CG_MAX_IN_VALUES),
+                ("case_first", C.c_int32 * CG_MAX_AGGS), ("case_narms", C.c_int32 * CG_MAX_AGGS), ("ncase_arms", C.c_int32),
+                ("reserved2", C.c_int32), ("case_arms", CgCaseArm * CG_MAX_CASE_ARMS)]
 
 
 class CgScanStats(C.Structure):

@@ -199,26 +199,53 @@ class Agg:
     term_abs_bound: int = 0
     filter: object = None        # FILTER (WHERE ...): a WHERE-style tree of (column, op, constant) atoms, None = none
     arg: object = None           # bool_and / bool_or: the predicate argument, a tree in the same form as `filter`
+    case: object = None          # a Case argument (then factors is empty), None = none
+
+
+@dataclass(frozen=True)
+class Const:
+    """a constant CASE result: an integer (pre-scaled to the aggregate's scale), or a float for a float aggregate"""
+    value: object
+
+
+_NO_ELSE = object()
+
+
+@dataclass
+class Case:
+    """CASE WHEN tree THEN result ... [ELSE result] END as an aggregate argument: arms = [(tree, result), ...] with trees in
+    the FILTER form (they share the FILTER atom pool); a result is None (NULL), Const(k), a column index, or a factor list
+    [(column, a, b), ...] (a product of at most three affine factors).  Without else_ the value of a row no tree accepts
+    is NULL."""
+    arms: list
+    else_: object = _NO_ELSE
+
+
+def _arg(kind, col, is_float=False, filter=None):
+    if isinstance(col, Case):
+        return Agg(kind, [], is_float, filter=filter, case=col)
+    return Agg(kind, [(col, 0, 1)], is_float, filter=filter)
 
 
 def count_star(filter=None):
     return Agg(CG_AGG_COUNT_STAR, filter=filter)
 
 
-def count(col, filter=None):
-    return Agg(CG_AGG_COUNT, [(col, 0, 1)], filter=filter)
+def count(col, filter=None, is_float=False):
+    """count(x); with a Case, is_float says whether its results are float (their NULLs are what count counts)"""
+    return _arg(CG_AGG_COUNT, col, is_float, filter)
 
 
 def sum_(col, is_float=False, filter=None):
-    return Agg(CG_AGG_SUM, [(col, 0, 1)], is_float, filter=filter)
+    return _arg(CG_AGG_SUM, col, is_float, filter)
 
 
 def min_(col, is_float=False, filter=None):
-    return Agg(CG_AGG_MIN, [(col, 0, 1)], is_float, filter=filter)
+    return _arg(CG_AGG_MIN, col, is_float, filter)
 
 
 def max_(col, is_float=False, filter=None):
-    return Agg(CG_AGG_MAX, [(col, 0, 1)], is_float, filter=filter)
+    return _arg(CG_AGG_MAX, col, is_float, filter)
 
 
 def bit_and(col, filter=None):
@@ -242,7 +269,25 @@ def bool_or(tree, filter=None):
 def variance(col, filter=None):
     """the state of var_pop / var_samp / variance / stddev_pop / stddev_samp / stddev over an integer column: fetch()
     gives N in count, sum(x) in sum and sum(x^2) in sumsq; numeric_var_out() makes the SQL value"""
-    return Agg(capi.CG_AGG_VARIANCE, [(col, 0, 1)], filter=filter)
+    return _arg(capi.CG_AGG_VARIANCE, col, filter=filter)
+
+
+def _f8(x):
+    return int(np.float64(x).view(np.int64))
+
+
+def _case_arm(tokens, result, is_float):
+    """one arm as (nwhen tokens, form, columns, a, b): the descriptor's CgCaseArm fields"""
+    if result is None:
+        return (tuple(tokens), capi.CG_CASE_NULL, (), (0,), ())
+    if isinstance(result, Const):
+        return (tuple(tokens), capi.CG_CASE_CONST, (), (_f8(result.value) if is_float else int(result.value),), ())
+    factors = [(result, 0, 1)] if isinstance(result, (int, np.integer)) else list(result)
+    if not 1 <= len(factors) <= 3:
+        raise ValueError("a CASE product has 1 to 3 factors")
+    conv = _f8 if is_float else int
+    return (tuple(tokens), capi.CG_CASE_PRODUCT, tuple(int(c) for c, _, _ in factors), tuple(conv(a) for _, a, _ in factors),
+            tuple(conv(b) for _, _, b in factors))
 
 
 def flatten_where(where):
@@ -372,6 +417,35 @@ def make_desc(quals=(), group_cols=(), aggs=(), qual_pushdown=True, expected_gro
             n[i] = len(tok)
             for j, t in enumerate(tok):
                 expr[i][j] = t
+    # CASE arms: WHEN trees over the same pool; identical arm lists (avg's sum and count) share one range
+    arms, ranges = [], {}
+    for i, a in enumerate(aggs):
+        if a.case is None:
+            continue
+        lst = [_case_arm(_filter_tokens(tree, pool), res, a.is_float) for tree, res in a.case.arms]
+        if a.case.else_ is not _NO_ELSE:
+            lst.append(_case_arm((), a.case.else_, a.is_float))
+        if len(pool) > capi.CG_MAX_FILTER_QUALS or any(len(arm[0]) > capi.CG_MAX_QEXPR for arm in lst):
+            raise capi.CitusGpuError(capi.CG_EUNSUPPORTED, "CASE WHEN trees too large")
+        key = tuple(lst)
+        if key not in ranges:
+            ranges[key] = len(arms)
+            arms.extend(lst)
+        d.case_first[i], d.case_narms[i] = ranges[key], len(lst)
+    if len(arms) > capi.CG_MAX_CASE_ARMS:
+        raise capi.CitusGpuError(capi.CG_EINVAL, "too many CASE arms")        # the library's code for ncase_arms > CG_MAX_CASE_ARMS
+    d.ncase_arms = len(arms)
+    for k, (tokens, form, cols, aa, bb) in enumerate(arms):
+        A = d.case_arms[k]
+        A.nwhen, A.form, A.nfactors = len(tokens), form, len(cols)
+        for j, t in enumerate(tokens):
+            A.when[j] = t
+        for f, c in enumerate(cols):
+            A.column[f] = c
+        for f, x in enumerate(aa):
+            A.a[f] = x
+        for f, x in enumerate(bb):
+            A.b[f] = x
     d.nfilter_quals = len(pool)
     for i, atom in enumerate(pool):
         _set_atom(d.filter_quals[i], atom, float_cols, lists)

@@ -290,14 +290,18 @@ __device__ __forceinline__ bool eval_where(const KPlan &P, const int64_t (&v)[NC
 
 /* aggregate FILTERs of a row that passed WHERE, same three-valued logic: bit a set = aggregate a has a filter and
  * it is not TRUE, or (bool_and / bool_or) its predicate argument is UNKNOWN, so the row is no input of a.  Bit a of
- * *argtrue = the predicate argument of aggregate a is TRUE. */
+ * *argtrue = the predicate argument of aggregate a is TRUE.  *pooltruth = the "is TRUE" bits of the pool's atoms (the
+ * CASE arms' WHEN trees read them). */
 template <int NCC>
-__device__ __forceinline__ uint32_t eval_filters(const KPlan &P, const int64_t (&v)[NCC], uint32_t nullmask, uint32_t *argtrue = nullptr)
+__device__ __forceinline__ uint32_t eval_filters(const KPlan &P, const int64_t (&v)[NCC], uint32_t nullmask, uint32_t *argtrue = nullptr,
+												 uint32_t *pooltruth = nullptr)
 {
 	if (argtrue) *argtrue = 0u;
+	if (pooltruth) *pooltruth = 0u;
 	if (P.nfquals == 0) return 0u;
 	uint32_t fals = 0;
 	uint32_t truth = eval_atoms<NCC>(P, v, nullmask, P.nfquals, P.fcol, P.fop, P.fk, P.flo, P.fhi, P.fneg, P.fset, P.fcc, &fals);
+	if (pooltruth) *pooltruth = truth;
 	uint32_t rejected = 0, at = 0;
 #pragma unroll 1
 	for (int a = 0; a < P.naggs; a++)
@@ -492,6 +496,55 @@ __device__ __forceinline__ uint64_t dense_slot_of_packed(const KPlan &P, int64_t
 	return ~0ull;
 }
 
+/*
+ * The value of a CASE argument (KPlan.arms[first .. first + n)) for a row its FILTER accepted: the first arm whose WHEN tree
+ * is TRUE over the pool atoms' "is TRUE" bits `truth` (UNKNOWN is not TRUE), else the ELSE arm, else NULL.  Only the chosen
+ * arm's result is evaluated, so an arm that was not chosen raises nothing.  Sets isnull, or the integer term it / the float
+ * term ft; a product arm is int_term's product over the arm's factors, with its overflow check when g.ovchk.
+ */
+template <int NCC>
+__device__ __forceinline__ void case_term(const KPlan &P, const KAgg &g, int first, int n, uint32_t truth, const int64_t (&v)[NCC],
+										  uint32_t nullmask, bool &isnull, int64_t &it, double &ft)
+{
+	int chosen = -1;
+#pragma unroll 1
+	for (int i = first; i < first + n; i++)
+		if (P.arms[i].nwhen == 0 || eval_postfix(truth, P.arms[i].nwhen, P.arms[i].when))
+		{
+			chosen = i;
+			break;
+		}
+	if (chosen < 0 || P.arms[chosen].form == CG_CASE_NULL)
+	{
+		isnull = true;
+		return;
+	}
+	const KArm &A = P.arms[chosen];
+	if (A.form == CG_CASE_CONST)
+	{
+		it = A.a[0];
+		ft = __longlong_as_double(A.a[0]);
+		return;
+	}
+	bool ovf = false;
+#pragma unroll
+	for (int f = 0; f < 3; f++)
+		if (f < A.nfactors)
+		{
+			const int c = A.pcol[f];
+			const int64_t x = pick<NCC>(v, c);
+			isnull = isnull || ((nullmask >> c) & 1u);
+			if (g.is_float) ft *= __longlong_as_double(A.a[f]) + __longlong_as_double(A.b[f]) * __longlong_as_double(x);
+			else if (!g.ovchk) it *= A.a[f] + A.b[f] * x;
+			else
+			{
+				const int64_t t = add_ovf(A.a[f], mul_ovf(A.b[f], x, ovf), ovf);
+				it = f ? mul_ovf(it, t, ovf) : t;
+			}
+		}
+	if (ovf && !isnull) atomicOr(P.stats + 2, CG_ERRFLAG_TERM_OVERFLOW);
+}
+
 /* the sum(x^2) callback of the kernels built without CG_AGG_VARIANCE (it is never called) */
 struct NoSquares
 {
@@ -508,12 +561,14 @@ struct NoSquares
  * VAR: the plan may hold CG_AGG_VARIANCE aggregates.  Their term is sum's (w0, w1 of x), and before it
  * sq(a, g, lo, hi) receives x^2 = hi:lo (unsigned 128 bits, from |x|).  Without VAR the kind is not compiled in, so the
  * kernels of the other plans are what they were.
+ * CASE: the plan may hold CASE arguments (KPlan.arms); an aggregate with arms takes its term from case_term.  Without CASE
+ * the arms are not compiled in, as VAR does for variance.
  */
-template <int NCC, int NA, bool VAR = false, class Term, class Sq = NoSquares>
+template <int NCC, int NA, bool VAR = false, bool CASE = false, class Term, class Sq = NoSquares>
 __device__ __forceinline__ void row_terms(const KPlan &P, const int64_t (&v)[NCC], uint32_t nullmask, Term term, Sq sq = Sq())
 {
-	uint32_t argtrue;
-	const uint32_t rejected = eval_filters<NCC>(P, v, nullmask, &argtrue);
+	uint32_t argtrue, truth;
+	const uint32_t rejected = eval_filters<NCC>(P, v, nullmask, &argtrue, CASE ? &truth : nullptr);
 #pragma unroll
 	for (int a = 0; a < NA; a++)
 	{
@@ -528,15 +583,23 @@ __device__ __forceinline__ void row_terms(const KPlan &P, const int64_t (&v)[NCC
 			}
 			int64_t it = 1;
 			double ft = 1.0;
+			if (CASE && P.cnarms[a] > 0)
+			{
+				/* a row the FILTER rejected is no input: its CASE is not consulted */
+				if (!isnull) case_term<NCC>(P, g, P.cfirst[a], P.cnarms[a], truth, v, nullmask, isnull, it, ft);
+			}
+			else
+			{
 #pragma unroll
-			for (int f = 0; f < 3; f++)
-				if (f < g.nfactors)
-				{
-					int c = g.pcol[f];
-					isnull = isnull || ((nullmask >> c) & 1u);
-					if (g.is_float) ft *= __longlong_as_double(g.a[f]) + __longlong_as_double(g.b[f]) * __longlong_as_double(pick<NCC>(v, c));
-				}
-			if (!g.is_float) it = int_term<NCC>(g, v, isnull, P.stats);
+				for (int f = 0; f < 3; f++)
+					if (f < g.nfactors)
+					{
+						int c = g.pcol[f];
+						isnull = isnull || ((nullmask >> c) & 1u);
+						if (g.is_float) ft *= __longlong_as_double(g.a[f]) + __longlong_as_double(g.b[f]) * __longlong_as_double(pick<NCC>(v, c));
+					}
+				if (!g.is_float) it = int_term<NCC>(g, v, isnull, P.stats);
+			}
 			if (isnull) { term(a, g, true, 0ull, 0ull); continue; }
 			if (g.kind == CG_AGG_COUNT) continue;
 			uint64_t w0, w1 = 0;
@@ -601,7 +664,7 @@ __device__ __forceinline__ void squares_apply_global(uint64_t *q, int qlimbs, ui
 }
 
 /* one row into an entry of the global group table (word 0 = rows in the group) */
-template <int NCC, int NA, bool VAR = false>
+template <int NCC, int NA, bool VAR = false, bool CASE = false>
 __device__ __forceinline__ void global_accumulate(const KPlan &P, uint64_t *entry, const int64_t (&v)[NCC], uint32_t nullmask)
 {
 	atomicAdd((unsigned long long *) entry, 1ull);
@@ -614,10 +677,10 @@ __device__ __forceinline__ void global_accumulate(const KPlan &P, uint64_t *entr
 		}
 	};
 	if constexpr (VAR)
-		row_terms<NCC, NA, true>(P, v, nullmask, term,
-								 [&](int, const KAgg &g, uint64_t lo, uint64_t hi) { squares_apply_global(entry + g.qword, g.qlimbs, lo, hi); });
+		row_terms<NCC, NA, true, CASE>(P, v, nullmask, term,
+									   [&](int, const KAgg &g, uint64_t lo, uint64_t hi) { squares_apply_global(entry + g.qword, g.qlimbs, lo, hi); });
 	else
-		row_terms<NCC, NA>(P, v, nullmask, term);
+		row_terms<NCC, NA, false, CASE>(P, v, nullmask, term);
 }
 
 /* ------------------------------------------------------------------------------ *
@@ -692,7 +755,7 @@ __device__ __forceinline__ void thread_acc_init(const KPlan &P, ThreadAcc<NAC, V
 	}
 }
 
-template <int NCC, int NAC, int MODE, bool VAR>
+template <int NCC, int NAC, int MODE, bool VAR, bool CASE = false>
 __device__ __forceinline__ void process_row(const KPlan &P, const int64_t (&v)[NCC], uint32_t nullmask,
 											ThreadAcc<NAC, VAR> &acc, uint32_t &removed)
 {
@@ -708,7 +771,7 @@ __device__ __forceinline__ void process_row(const KPlan &P, const int64_t (&v)[N
 		bool key_null;
 		if (!group_key<NCC>(P, v, nullmask, key, key_null)) return;
 		uint64_t *entry = find_entry<MODE>(P, key, key_null);
-		if (entry != nullptr) global_accumulate<NCC, NAC, VAR>(P, entry, v, nullmask);
+		if (entry != nullptr) global_accumulate<NCC, NAC, VAR, CASE>(P, entry, v, nullmask);
 		return;
 	}
 	acc.rows++;
@@ -721,7 +784,7 @@ __device__ __forceinline__ void process_row(const KPlan &P, const int64_t (&v)[N
 		}
 	};
 	if constexpr (VAR)
-		row_terms<NCC, NAC, true>(P, v, nullmask, term, [&](int a, const KAgg &g, uint64_t lo, uint64_t hi) {
+		row_terms<NCC, NAC, true, CASE>(P, v, nullmask, term, [&](int a, const KAgg &g, uint64_t lo, uint64_t hi) {
 			/* a thread's limb sums grow by < 2^32 per row; the one-word form is bounded by the table's own guarantee */
 			if (g.qlimbs == 1) acc.q[a][0] += lo;
 			else
@@ -732,7 +795,7 @@ __device__ __forceinline__ void process_row(const KPlan &P, const int64_t (&v)[N
 			}
 		});
 	else
-		row_terms<NCC, NAC>(P, v, nullmask, term);
+		row_terms<NCC, NAC, false, CASE>(P, v, nullmask, term);
 }
 
 /* the end of a kernel that ran process_row: the row counters into P.stats ([0] rows handed to WHERE, [1] rows removed)

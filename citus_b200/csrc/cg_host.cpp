@@ -523,19 +523,41 @@ extern "C" int cg_relation_bounds(const CgRelation *rel, const CgScanDesc *desc,
 			const CgAggSpec &s = desc->aggs[a];
 			term_abs_bound[a] = 0;
 			if (!cg_kind_sums(s.kind) || s.is_float) continue;
-			__int128 bound = 1;
+			/* |prod (a + b x)| over the factors' column bounds; false = unknown */
+			auto product_bound = [&](int nfactors, const int32_t *column, const int64_t *fa, const int64_t *fb, __int128 *out) {
+				__int128 bound = 1;
+				for (int f = 0; f < nfactors; f++)
+				{
+					int c = column[f];
+					if (c < 0 || c >= (int) unknown.size() || unknown[c]) return false;
+					if (cmin[c] > cmax[c]) { bound = 0; continue; }   /* no values at all */
+					__int128 lo = (__int128) fa[f] + (__int128) fb[f] * cmin[c];
+					__int128 hi = (__int128) fa[f] + (__int128) fb[f] * cmax[c];
+					__int128 m = std::max(lo < 0 ? -lo : lo, hi < 0 ? -hi : hi);
+					bound *= m;
+					if (bound > ((__int128) 1 << 62)) return false;
+				}
+				*out = bound;
+				return true;
+			};
+			__int128 bound = 0;
 			bool ok = true;
-			for (int f = 0; f < s.nfactors && ok; f++)
+			if (desc->case_narms[a] > 0)
 			{
-				int c = s.column[f];
-				if (unknown[c]) { ok = false; break; }
-				if (cmin[c] > cmax[c]) { bound = 0; continue; }   /* no values at all */
-				__int128 lo = (__int128) s.a[f] + (__int128) s.b[f] * cmin[c];
-				__int128 hi = (__int128) s.a[f] + (__int128) s.b[f] * cmax[c];
-				__int128 m = std::max(lo < 0 ? -lo : lo, hi < 0 ? -hi : hi);
-				bound *= m;
-				if (bound > ((__int128) 1 << 62)) ok = false;
+				/* CASE: the largest bound over the arms (a constant counts |k|, a NULL arm nothing); the WHEN atoms add none */
+				for (int i = desc->case_first[a]; i < desc->case_first[a] + desc->case_narms[a] && ok; i++)
+				{
+					if (i < 0 || i >= CG_MAX_CASE_ARMS) { ok = false; break; }
+					const CgCaseArm &A = desc->case_arms[i];
+					__int128 m = 0;
+					if (A.form == CG_CASE_CONST) m = A.a[0] < 0 ? -(__int128) A.a[0] : (__int128) A.a[0];
+					else if (A.form == CG_CASE_PRODUCT) ok = product_bound(A.nfactors, A.column, A.a, A.b, &m);
+					bound = std::max(bound, m);
+				}
+				ok = ok && bound <= ((__int128) 1 << 62);
 			}
+			else
+				ok = product_bound(s.nfactors, s.column, s.a, s.b, &bound);
 			if (ok) term_abs_bound[a] = bound == 0 ? 1 : (int64_t) bound;
 		}
 	return CG_OK;
@@ -1595,6 +1617,11 @@ extern "C" int cg_scan_relation(const CgRelation *rel, const CgScanDesc *desc, C
 	if (cg_desc_uses_pool(desc))
 		for (int q = 0; q < desc->nfilter_quals && q < CG_MAX_FILTER_QUALS; q++)
 			need_atom(desc->filter_quals[q]);
+	for (int a = 0; a < desc->naggs; a++)
+		for (int i = desc->case_first[a]; desc->case_narms[a] > 0 && i < desc->case_first[a] + desc->case_narms[a] && i >= 0 && i < CG_MAX_CASE_ARMS; i++)
+			if (desc->case_arms[i].form == CG_CASE_PRODUCT)
+				for (int f = 0; f < desc->case_arms[i].nfactors && f < 3; f++)
+					if (desc->case_arms[i].column[f] >= 0 && desc->case_arms[i].column[f] < rel->natts) need(desc->case_arms[i].column[f]);
 	if (staged.empty()) need(0);   /* count(*) only: the reference still reads the first column's skip nodes; we read its chunk row counts */
 
 	KPlan plan;

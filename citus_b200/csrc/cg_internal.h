@@ -254,6 +254,19 @@ struct KCmp
 	uint8_t pad[6];
 };
 
+/* one CASE arm (CgCaseArm) with its columns as plan columns: WHEN tree when[0 .. nwhen) over the filter atoms (0 tokens =
+ * ELSE); result form CG_CASE_*: the constant a[0], or the product over nfactors of (a[f] + b[f] * v[pcol[f]]) */
+struct KArm
+{
+	int64_t a[3];
+	int64_t b[3];
+	int8_t nwhen;
+	int8_t form;
+	int8_t nfactors;
+	int8_t pcol[3];
+	int8_t when[CG_MAX_QEXPR];
+};
+
 struct KPlan
 {
 	const uint8_t *arena;
@@ -346,6 +359,13 @@ struct KPlan
 	 * that the generated kernels of plans without column atoms restate the struct without them (cg_jit.cpp) */
 	KCmp qcc[CG_MAX_QUALS];
 	KCmp fcc[CG_MAX_FILTER_QUALS];
+	/* CASE arguments (CgScanDesc.case_arms): aggregate a with cnarms[a] > 0 takes its term from arms[cfirst[a] ..
+	 * cfirst[a] + cnarms[a]).  Behind the column atoms, so that the generated kernels of plans without CASE restate the
+	 * struct without them (cg_jit.cpp) */
+	int32_t ncase;                /* arms in use, 0 = no CASE */
+	int8_t cfirst[CG_MAX_AGGS];
+	int8_t cnarms[CG_MAX_AGGS];
+	KArm arms[CG_MAX_CASE_ARMS];
 };
 
 static inline __host__ __device__ bool cg_op_is_column(int op) { return op >= CG_OP_COL_LT && op <= CG_OP_COL_NE; }
@@ -357,11 +377,19 @@ static inline bool cg_desc_has_filters(const CgScanDesc *d)
 	return false;
 }
 
-/* the filter atom pool is read by some FILTER or some bool_and / bool_or argument */
+/* some aggregate's argument is a CASE */
+static inline bool cg_desc_has_case(const CgScanDesc *d)
+{
+	for (int a = 0; a < d->naggs && a < CG_MAX_AGGS; a++)
+		if (d->case_narms[a] > 0) return true;
+	return false;
+}
+
+/* the filter atom pool is read by some FILTER, some bool_and / bool_or argument or some CASE arm */
 static inline bool cg_desc_uses_pool(const CgScanDesc *d)
 {
 	for (int a = 0; a < d->naggs && a < CG_MAX_AGGS; a++)
-		if (d->nfilter_expr[a] > 0 || d->narg_expr[a] > 0) return true;
+		if (d->nfilter_expr[a] > 0 || d->narg_expr[a] > 0 || d->case_narms[a] > 0) return true;
 	return false;
 }
 

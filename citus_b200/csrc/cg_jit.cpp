@@ -245,9 +245,10 @@ static void choose_shape(const KPlan &plan, uint32_t nullable, JitShape *sh)
 			if (agg_is_var(g)) { sh->qcell[a] = nhot; nhot += g.qlimbs; }
 		}
 		/* rejected rows are common, not rare like NULL inputs: a filtered aggregate's no-input counter gets a cell too, and
-		 * so does the counter of a bool_and / bool_or, whose UNKNOWN rows are as common as its atoms' NULLs */
+		 * so does the counter of a bool_and / bool_or, whose UNKNOWN rows are as common as its atoms' NULLs, and that of a
+		 * CASE, whose NULL results are as common as its arms' WHEN trees fail */
 		for (int a = 0; a < plan.naggs; a++)
-			if (plan.nfexpr[a] > 0 || plan.aggs[a].barg) sh->ncell[a] = nhot++;
+			if (plan.nfexpr[a] > 0 || plan.aggs[a].barg || plan.cnarms[a] > 0) sh->ncell[a] = nhot++;
 		size_t bytes = (size_t) plan.capacity * nhot * sizeof(uint64_t) * JIT_THREADS;
 		if (plan.capacity <= 4096 && bytes <= 200 * 1024)
 		{
@@ -360,9 +361,10 @@ static_assert(offsetof(KPlan, naggs) == offsetof(KPlan, gcol) + 4 && (offsetof(K
 static void gen_prelude(std::string &s, const KPlan &plan)
 {
 	const bool args = plan_has_args(plan);
-	const bool sets = plan_has_sets(plan);
-	/* plans with IN lists restate the whole struct, plans with a composite key all but the lists; the others stop at fexpr
-	 * or argexpr as before */
+	/* plans with CASE arms restate the whole struct, plans with IN lists all but the column atoms and the arms, plans with
+	 * a composite key all but the lists; the others stop at fexpr or argexpr as before */
+	const bool cases = plan.ncase > 0;
+	const bool sets = plan_has_sets(plan) || cases;
 	const bool composite = plan.composite || sets;
 	const bool tail = args || composite;
 	s +=
@@ -370,6 +372,11 @@ static void gen_prelude(std::string &s, const KPlan &plan)
 		"typedef unsigned short uint16_t; typedef short int16_t; typedef unsigned char uint8_t; typedef signed char int8_t;\n"
 		"struct DevChunkCol { uint64_t values_off; uint64_t exists_off; uint64_t rank_off; uint32_t value_count; uint32_t row_count; };\n";
 	if (sets) s += "struct KSet { uint16_t off; uint16_t len; uint8_t steps; uint8_t nnull; uint8_t pad[2]; };\n";
+	if (cases)
+		addf(s,
+			 "struct KCmp { int64_t mul; uint8_t col2; uint8_t right; uint8_t pad[6]; };\n"
+			 "struct KArm { int64_t a[3]; int64_t b[3]; int8_t nwhen; int8_t form; int8_t nfactors; int8_t pcol[3]; int8_t when[%d]; };\n",
+			 CG_MAX_QEXPR);
 	s += args ? "struct KAgg { int8_t kind; int8_t nfactors; int8_t is_float; int8_t nlimbs; int8_t pcol[3]; int8_t word0; int8_t nullword; int8_t ovchk; int8_t filt; int8_t barg;"
 			  : "struct KAgg { int8_t kind; int8_t nfactors; int8_t is_float; int8_t nlimbs; int8_t pcol[3]; int8_t word0; int8_t nullword; int8_t ovchk; int8_t filt; int8_t pad;";
 	/* the sum(x^2) fields sit in KAgg's padding: plans without a variance aggregate restate the struct without them */
@@ -392,15 +399,19 @@ static void gen_prelude(std::string &s, const KPlan &plan)
 		 tail ? "\n" : " };\n");
 	if (tail) addf(s, "  int32_t nargexpr[%d]; int8_t argexpr[%d][%d];%s", CG_MAX_AGGS, CG_MAX_AGGS, CG_MAX_QEXPR, composite ? "\n" : " };\n");
 	if (composite) addf(s, "  int32_t composite; int64_t kmin[%d]; uint64_t kradix[%d];%s", CG_MAX_GROUP_COLS, CG_MAX_GROUP_COLS, sets ? "\n" : " };\n");
-	if (sets) addf(s, "  const uint64_t *sets; KSet qset[%d]; KSet fset[%d]; };\n", CG_MAX_QUALS, CG_MAX_FILTER_QUALS);
+	if (sets) addf(s, "  const uint64_t *sets; KSet qset[%d]; KSet fset[%d];%s", CG_MAX_QUALS, CG_MAX_FILTER_QUALS, cases ? "\n" : " };\n");
+	if (cases)
+		addf(s, "  KCmp qcc[%d]; KCmp fcc[%d]; int32_t ncase; int8_t cfirst[%d]; int8_t cnarms[%d]; KArm arms[%d]; };\n", CG_MAX_QUALS,
+			 CG_MAX_FILTER_QUALS, CG_MAX_AGGS, CG_MAX_AGGS, CG_MAX_CASE_ARMS);
 	/* the text above must describe the host's structs exactly (without arguments: the prefix up to fexpr; with arguments
 	 * only: the prefix up to argexpr; with a composite key: the prefix up to the lists; with lists: the prefix up to the
 	 * column atoms' KCmp entries, which the generated code never reads -- their columns and scales are written out) */
 	const auto upto = [](size_t off) { return (off + alignof(KPlan) - 1) / alignof(KPlan) * alignof(KPlan); };
-	const size_t size = sets ? upto(offsetof(KPlan, qcc)) : composite ? upto(offsetof(KPlan, sets)) : args ? upto(offsetof(KPlan, composite))
-																					   : upto(offsetof(KPlan, nargexpr));
+	const size_t size = cases ? sizeof(KPlan) : sets ? upto(offsetof(KPlan, qcc)) : composite ? upto(offsetof(KPlan, sets))
+																			   : args ? upto(offsetof(KPlan, composite)) : upto(offsetof(KPlan, nargexpr));
 	addf(s, "static_assert(sizeof(DevChunkCol) == %zu, \"DevChunkCol\");\n", sizeof(DevChunkCol));
 	addf(s, "static_assert(sizeof(KAgg) == %zu, \"KAgg\");\n", sizeof(KAgg));
+	if (cases) addf(s, "static_assert(sizeof(KArm) == %zu, \"KArm\");\n", sizeof(KArm));
 	addf(s, "static_assert(sizeof(KPlan) == %zu, \"KPlan\");\n", size);
 	/* (NVRTC has no offsetof; same field order + same total size is the check) */
 	s +=
@@ -579,6 +590,7 @@ static std::string agg_noinput_expr(const KPlan &plan, int a, const JitShape &sh
 {
 	const KAgg &g = plan.aggs[a];
 	std::string e = g.kind == CG_AGG_COUNT_STAR ? std::string() : agg_null_expr(g, sh);
+	if (plan.cnarms[a] > 0) e = "cn" + std::to_string(a);     /* the CASE's value is NULL (gen_case) */
 	if (plan.nargexpr[a] > 0) e += (e.empty() ? "" : " || ") + ("(!at" + std::to_string(a) + " && !af" + std::to_string(a) + ")");
 	if (plan.nfexpr[a] > 0) e += (e.empty() ? "!f" : " || !f") + std::to_string(a);
 	return e;
@@ -679,6 +691,72 @@ static std::string where_expr(const KPlan &plan)
 		return e;
 	}
 	return tree_expr(plan.nqexpr, plan.qexpr, "t");
+}
+
+/* The CASE argument of aggregate a as straight-line first-TRUE selection over the WHEN trees (pool atoms u<q>): defines
+ * cn<a> = the value is NULL, and it<a> (integer) or ft<a> (float) -- and ov<a> for an overflow-checked term -- from the
+ * chosen arm only, so an arm that was not chosen raises nothing.  The arms' structure (their number, WHEN trees, result
+ * forms and factor columns) is the query shape; their constants stay kernel parameters, P.arms[i], except that a bare
+ * column factor (0 + 1 * x) is written out, as term_expr does. */
+static void gen_case(std::string &s, const KPlan &plan, const JitShape &sh, int a, const char *C)
+{
+	const KAgg &g = plan.aggs[a];
+	const bool fl = g.is_float;
+	addf(s, "%sbool cn%d = true;\n%s%s %ct%d = %s;\n", C, a, C, fl ? "double" : "int64_t", fl ? 'f' : 'i', a, fl ? "0.0" : "0");
+	if (!fl && g.ovchk) addf(s, "%sbool ov%d = false;\n", C, a);
+	bool has_else = false;
+	for (int i = plan.cfirst[a]; i < plan.cfirst[a] + plan.cnarms[a]; i++)
+	{
+		const KArm &A = plan.arms[i];
+		const bool first = i == plan.cfirst[a];
+		if (A.nwhen == 0)
+		{
+			addf(s, "%s%s{", C, first ? "" : "else ");
+			has_else = true;
+		}
+		else addf(s, "%s%sif (%s) {", C, first ? "" : "else ", tree_expr(A.nwhen, A.when, "u").c_str());
+		if (A.form == CG_CASE_CONST)
+		{
+			if (fl) addf(s, " cn%d = false; ft%d = __longlong_as_double(P.arms[%d].a[0]);", a, a, i);
+			else addf(s, " cn%d = false; it%d = P.arms[%d].a[0];", a, a, i);
+		}
+		else if (A.form == CG_CASE_PRODUCT)
+		{
+			std::string nul, e;
+			bool seen[CG_KMAX_COLS] = {false};
+			for (int f = 0; f < A.nfactors; f++)
+			{
+				const int c = A.pcol[f];
+				if (col_nullable(sh, c) && !seen[c]) nul += (nul.empty() ? "(z" : " || z") + std::to_string(c);
+				seen[c] = true;
+				char buf[256];
+				const bool bare = A.a[f] == 0 && (fl ? A.b[f] == 0x3ff0000000000000ll : A.b[f] == 1);
+				if (fl)
+				{
+					if (bare) snprintf(buf, sizeof buf, "__longlong_as_double(v%d)", c);
+					else snprintf(buf, sizeof buf, "(__longlong_as_double(P.arms[%d].a[%d]) + __longlong_as_double(P.arms[%d].b[%d]) * __longlong_as_double(v%d))",
+								  i, f, i, f, c);
+					e += (f ? " * " : "") + std::string(buf);
+				}
+				else if (g.ovchk)
+				{
+					if (bare) snprintf(buf, sizeof buf, "v%d", c);
+					else snprintf(buf, sizeof buf, "add_ovf(P.arms[%d].a[%d], mul_ovf(P.arms[%d].b[%d], v%d, ov%d), ov%d)", i, f, i, f, c, a, a);
+					e = f ? "mul_ovf(" + e + ", " + buf + ", ov" + std::to_string(a) + ")" : std::string(buf);
+				}
+				else
+				{
+					if (bare) snprintf(buf, sizeof buf, "v%d", c);
+					else snprintf(buf, sizeof buf, "(P.arms[%d].a[%d] + P.arms[%d].b[%d] * v%d)", i, f, i, f, c);
+					e += (f ? " * " : "") + std::string(buf);
+				}
+			}
+			if (!nul.empty()) nul += ")";
+			addf(s, " cn%d = %s; %ct%d = %s;", a, nul.empty() ? "false" : nul.c_str(), fl ? 'f' : 'i', a, e.c_str());
+		}
+		s += " }\n";
+		if (has_else) break;
+	}
 }
 
 /* updates of a group entry in global memory (`e` = its word pointer): the TABLE kind, and the NULL-key group of
@@ -882,6 +960,7 @@ static void gen_row(std::string &s, const KPlan &plan, const JitShape &sh, int u
 	for (int a = 0; a < plan.naggs; a++)
 	{
 		const KAgg &g = plan.aggs[a];
+		if (plan.cnarms[a] > 0) gen_case(s, plan, sh, a, C);
 		an[a] = agg_noinput_expr(plan, a, sh);
 		if (!an[a].empty()) addf(s, "%sconst bool an%d = %s;\n", C, a, an[a].c_str());
 		if (!agg_has_value(g)) continue;
@@ -891,12 +970,13 @@ static void gen_row(std::string &s, const KPlan &plan, const JitShape &sh, int u
 			w0v[a] = "(at" + std::to_string(a) + " ? 0xffffffffffffffffull : 0ull)";
 			continue;
 		}
-		std::string e = term_expr(g, a);
-		if (g.is_float) addf(s, "%sconst double ft%d = %s;\n", C, a, e.c_str());
+		const bool cs = plan.cnarms[a] > 0;     /* gen_case defined the term */
+		std::string e = cs ? std::string() : term_expr(g, a);
+		if (g.is_float) { if (!cs) addf(s, "%sconst double ft%d = %s;\n", C, a, e.c_str()); }
 		else
 		{
-			if (g.ovchk) addf(s, "%sbool ov%d = false;\n", C, a);
-			addf(s, "%sconst int64_t it%d = %s;\n", C, a, e.c_str());
+			if (g.ovchk && !cs) addf(s, "%sbool ov%d = false;\n", C, a);
+			if (!cs) addf(s, "%sconst int64_t it%d = %s;\n", C, a, e.c_str());
 			if (g.ovchk)
 				addf(s, "%sif (%sov%d) raise_flag(P.stats, %lluull);\n", C, an[a].empty() ? "" : ("!an" + std::to_string(a) + " && ").c_str(),
 					 a, (unsigned long long) CG_ERRFLAG_TERM_OVERFLOW);

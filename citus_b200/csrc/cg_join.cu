@@ -404,7 +404,7 @@ struct JoinAggCols
 	uint32_t probe;
 };
 
-template <int NCC, int NAC, int MODE, bool VAR>
+template <int NCC, int NAC, int MODE, bool VAR, bool CASE = false>
 __global__ void __launch_bounds__(CGJ_THREADS, 4)
 cg_join_agg_kernel(const __grid_constant__ KPlan P, const JoinAggCols J, const JoinRowsTable T, const long long *keys, const uint8_t *key_nulls,
 				   long long n)
@@ -444,17 +444,17 @@ cg_join_agg_kernel(const __grid_constant__ KPlan P, const JoinAggCols J, const J
 					if (J.nul[c] && __ldg(J.nul[c] + b)) nullmask |= 1u << c;
 				}
 			joined++;
-			process_row<NCC, NAC, MODE, VAR>(P, v, nullmask, acc, removed);
+			process_row<NCC, NAC, MODE, VAR, CASE>(P, v, nullmask, acc, removed);
 		}
 	}
 	flush_thread<NAC, MODE, VAR>(P, acc, removed, joined);
 }
 
-template <int MODE, bool VAR>
+template <int MODE, bool VAR, bool CASE = false>
 static int launch_join_agg(CgContext *ctx, const KPlan &plan, const JoinAggCols &J, const JoinRowsTable &T, const long long *keys,
 						   const uint8_t *key_nulls, long long n, cudaStream_t stream)
 {
-	auto kernel = cg_join_agg_kernel<CG_KMAX_COLS, CG_MAX_AGGS, MODE, VAR>;
+	auto kernel = cg_join_agg_kernel<CG_KMAX_COLS, CG_MAX_AGGS, MODE, VAR, CASE>;
 	int occ = 0;
 	CG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, CGJ_THREADS, 0));
 	if (occ < 1) occ = 1;
@@ -493,6 +493,14 @@ int cg_launch_join_aggregate(CgContext *ctx, const KPlan &plan, const CgJoinSide
 	if (rc) return rc;
 	const long long *keys = (const long long *) p.d_cols[p.key];
 	const uint8_t *key_nulls = p.d_nulls ? p.d_nulls[p.key] : nullptr;
+	/* plans with a CASE argument: one instance per table kind, variance included */
+	if (plan.ncase > 0)
+		switch (plan.mode)
+		{
+			case CG_MODE_GLOBAL: return launch_join_agg<CG_MODE_GLOBAL, true, true>(ctx, plan, J, T, keys, key_nulls, p.nrows, stream);
+			case CG_MODE_DENSE: return launch_join_agg<CG_MODE_DENSE, true, true>(ctx, plan, J, T, keys, key_nulls, p.nrows, stream);
+			default: return launch_join_agg<CG_MODE_HASH, true, true>(ctx, plan, J, T, keys, key_nulls, p.nrows, stream);
+		}
 	const bool var = cg_plan_has_variance(plan.aggs, plan.naggs);
 	switch (plan.mode)
 	{

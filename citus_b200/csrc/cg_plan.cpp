@@ -114,6 +114,59 @@ std::vector<int64_t> cg_where_lists(const CgScanDesc *d)
 	return out;
 }
 
+/* the columns of an aggregate argument's factors, under the rules of the aggregate's kind */
+static int validate_factor_columns(int a, int kind, bool is_float, const int32_t *column, int nfactors, const CgColumnDesc *columns, int natts)
+{
+	for (int f = 0; f < nfactors; f++)
+	{
+		if (column[f] < 0 || column[f] >= natts) return cg_set_error(CG_EINVAL, "aggregate %d: column out of range", a);
+		const int cls = cg_type_class(columns[column[f]]);
+		if (kind == CG_AGG_VARIANCE)
+		{
+			/* the exact integer state of numeric_stddev_internal: a float argument has no such state */
+			if (cls == CG_TYPE_BPCHAR1) return cg_set_error(CG_EINVAL, "aggregate %d: variance over a char(1) column", a);
+			if (is_float || cls == CG_TYPE_FLOAT) return cg_set_error(CG_EUNSUPPORTED, "aggregate %d: variance / stddev of a float argument", a);
+		}
+		else if (kind != CG_AGG_COUNT && (cls == CG_TYPE_FLOAT) != is_float)
+			return cg_set_error(CG_EINVAL, "aggregate %d: integer/float mismatch with column %d", a, column[f]);
+	}
+	return CG_OK;
+}
+
+/* CASE arguments (CgScanDesc.case_arms; include/citus_gpu.h states the rules) */
+static int validate_case(const CgScanDesc *d, const CgColumnDesc *columns, int natts)
+{
+	if (d->ncase_arms < 0 || d->ncase_arms > CG_MAX_CASE_ARMS) return cg_set_error(CG_EINVAL, "ncase_arms %d out of range", d->ncase_arms);
+	for (int a = 0; a < CG_MAX_AGGS; a++)
+	{
+		const int n = d->case_narms[a], first = d->case_first[a];
+		if (n < 0) return cg_set_error(CG_EINVAL, "case_narms[%d] = %d", a, n);
+		if (n == 0) continue;
+		if (a >= d->naggs) return cg_set_error(CG_EINVAL, "CASE of aggregate %d of %d", a, d->naggs);
+		const CgAggSpec &s = d->aggs[a];
+		if (s.kind != CG_AGG_COUNT && s.kind != CG_AGG_SUM && s.kind != CG_AGG_MIN && s.kind != CG_AGG_MAX && s.kind != CG_AGG_VARIANCE)
+			return cg_set_error(CG_EINVAL, "aggregate %d: a CASE argument on a kind that takes none", a);
+		if (s.nfactors != 0) return cg_set_error(CG_EINVAL, "aggregate %d: a CASE argument with factors (the arms carry the terms)", a);
+		if (first < 0 || (int64_t) first + n > d->ncase_arms)
+			return cg_set_error(CG_EINVAL, "aggregate %d: arms [%d, %lld) outside [0, %d)", a, first, (long long) first + n, d->ncase_arms);
+		for (int i = first; i < first + n; i++)
+		{
+			const CgCaseArm &A = d->case_arms[i];
+			int rc;
+			if (A.nwhen < 0 || A.nwhen > CG_MAX_QEXPR) return cg_set_error(CG_EINVAL, "arm %d: nwhen %d out of range", i, A.nwhen);
+			if (A.nwhen == 0 && i != first + n - 1) return cg_set_error(CG_EINVAL, "aggregate %d: the ELSE arm %d is not its last arm", a, i);
+			if (A.nwhen > 0 && (rc = validate_postfix("CASE WHEN tree", A.when, A.nwhen, d->nfilter_quals))) return rc;
+			if (A.form != CG_CASE_NULL && A.form != CG_CASE_CONST && A.form != CG_CASE_PRODUCT)
+				return cg_set_error(CG_EINVAL, "arm %d: bad result form %d", i, A.form);
+			if (A.form != CG_CASE_PRODUCT) continue;
+			if (A.nfactors < 1 || A.nfactors > 3) return cg_set_error(CG_EINVAL, "arm %d: nfactors %d", i, A.nfactors);
+			if ((rc = validate_factor_columns(a, s.kind, s.is_float != 0, A.column, A.nfactors, columns, natts))) return rc;
+		}
+		if (s.kind == CG_AGG_VARIANCE && s.is_float) return cg_set_error(CG_EUNSUPPORTED, "aggregate %d: variance / stddev of a float argument", a);
+	}
+	return CG_OK;
+}
+
 static int validate_desc(const CgScanDesc *d, const CgColumnDesc *columns, int natts)
 {
 	if (d->nquals < 0 || d->nquals > CG_MAX_QUALS) return cg_set_error(CG_EINVAL, "nquals %d out of range", d->nquals);
@@ -172,11 +225,13 @@ static int validate_desc(const CgScanDesc *d, const CgColumnDesc *columns, int n
 		if (!d->composite_key && d->ngroup_cols == 2 && cg_decoded_len(columns[c]) > 4)
 			return cg_set_error(CG_EUNSUPPORTED, "two-column GROUP BY needs columns of at most 4 bytes");
 	}
+	if ((rc = validate_case(d, columns, natts))) return rc;
 	for (int a = 0; a < d->naggs; a++)
 	{
 		const CgAggSpec &s = d->aggs[a];
 		if (s.kind < CG_AGG_COUNT_STAR || s.kind > CG_AGG_VARIANCE) return cg_set_error(CG_EINVAL, "aggregate %d: bad kind", a);
 		if (s.nfactors < 0 || s.nfactors > 3) return cg_set_error(CG_EINVAL, "aggregate %d: nfactors", a);
+		if (d->case_narms[a] > 0) continue;     /* the arms carry the argument (validate_case) */
 		if (s.kind > CG_AGG_MAX && s.kind != CG_AGG_VARIANCE && s.term_abs_bound != 0)
 			return cg_set_error(CG_EINVAL, "aggregate %d: term_abs_bound on bit / bool kind", a);
 		if (s.kind == CG_AGG_VARIANCE)
@@ -595,6 +650,24 @@ extern "C" int cg_partial_layout(const CgPartial *p, int32_t *nwords, int32_t *w
 	return CG_OK;
 }
 
+/* aggregate a has the same CASE argument in both descriptors (both validated): the same arms in the same order, compared
+ * field by field (the arms' positions in case_arms may differ) */
+static bool same_case(const CgScanDesc *x, const CgScanDesc *y, int a)
+{
+	if (x->case_narms[a] != y->case_narms[a]) return false;
+	for (int i = 0; i < x->case_narms[a]; i++)
+	{
+		const CgCaseArm &p = x->case_arms[x->case_first[a] + i], &q = y->case_arms[y->case_first[a] + i];
+		if (p.nwhen != q.nwhen || memcmp(p.when, q.when, (size_t) p.nwhen) != 0 || p.form != q.form) return false;
+		if (p.form == CG_CASE_CONST && p.a[0] != q.a[0]) return false;
+		if (p.form != CG_CASE_PRODUCT) continue;
+		if (p.nfactors != q.nfactors) return false;
+		for (int f = 0; f < p.nfactors; f++)
+			if (p.column[f] != q.column[f] || p.a[f] != q.a[f] || p.b[f] != q.b[f]) return false;
+	}
+	return true;
+}
+
 /*
  * Kernel plan: deduplicated projection (columnar_customscan.c:1813-1851 ColumnarAttrNeeded:
  * only the columns the quals, group keys and aggregate arguments reference are read).
@@ -611,7 +684,7 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 	for (int a = 0; a < desc->naggs; a++)
 		if (memcmp(&partial->desc.aggs[a], &desc->aggs[a], sizeof(CgAggSpec)) != 0 || partial->aggs[a].filt != (desc->nfilter_expr[a] > 0) ||
 			partial->desc.narg_expr[a] != desc->narg_expr[a] ||
-			memcmp(partial->desc.arg_expr[a], desc->arg_expr[a], (size_t) desc->narg_expr[a]) != 0)
+			memcmp(partial->desc.arg_expr[a], desc->arg_expr[a], (size_t) desc->narg_expr[a]) != 0 || !same_case(&partial->desc, desc, a))
 			return cg_set_error(CG_EINVAL, "partial aggregate was created for a different aggregate list");
 	/* a composite partial's codes mean something only under its own key columns and bounds */
 	if (partial->desc.composite_key != desc->composite_key)
@@ -742,10 +815,41 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 			plan->aggs[a].pcol[f] = (int8_t) pc;
 		}
 	}
+	if (cg_desc_has_case(desc))
+	{
+		/* the arms the aggregates name (validate_case checked them), their factor columns as plan columns */
+		bool done[CG_MAX_CASE_ARMS] = {false};
+		plan->ncase = desc->ncase_arms;
+		for (int a = 0; a < desc->naggs; a++)
+		{
+			plan->cfirst[a] = (int8_t) desc->case_first[a];
+			plan->cnarms[a] = (int8_t) desc->case_narms[a];
+			for (int i = desc->case_first[a]; i < desc->case_first[a] + desc->case_narms[a]; i++)
+			{
+				if (done[i]) continue;
+				done[i] = true;
+				const CgCaseArm &A = desc->case_arms[i];
+				KArm &k = plan->arms[i];
+				k.nwhen = (int8_t) A.nwhen;
+				for (int t = 0; t < A.nwhen; t++) k.when[t] = A.when[t];
+				k.form = (int8_t) A.form;
+				k.a[0] = A.a[0];
+				if (A.form != CG_CASE_PRODUCT) continue;
+				k.nfactors = (int8_t) A.nfactors;
+				for (int f = 0; f < A.nfactors; f++)
+				{
+					int pc; USE_OR_FAIL(pc, A.column[f]);
+					k.pcol[f] = (int8_t) pc;
+					k.a[f] = A.a[f];
+					k.b[f] = A.b[f];
+				}
+			}
+		}
+	}
 	if (cg_desc_uses_pool(desc))
 	{
-		/* a column read only by a FILTER or a predicate argument is a plan column like any other (projection, column
-		 * limit) */
+		/* a column read only by a FILTER, a predicate argument or a CASE arm is a plan column like any other (projection,
+		 * column limit) */
 		plan->nfquals = desc->nfilter_quals;
 		for (int q = 0; q < desc->nfilter_quals; q++)
 		{
@@ -802,7 +906,7 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
  */
 bool cg_build_fast_plan(const CgScanDesc *desc, const KPlan &plan, bool all8, FPlan *fast)
 {
-	if (!all8 || plan.ngroup > 1 || plan.composite || plan.nqexpr != 0 || plan.nfquals != 0) return false;
+	if (!all8 || plan.ngroup > 1 || plan.composite || plan.nqexpr != 0 || plan.nfquals != 0 || plan.ncase != 0) return false;
 	for (int q = 0; q < plan.nquals; q++) if (plan.qop[q] > CG_OP_NE) return false;     /* IN lists, NULL tests, column atoms */
 	for (int c = 0; c < plan.ncols; c++) if (plan.isfloat[c]) return false;
 	memset(fast, 0, sizeof *fast);

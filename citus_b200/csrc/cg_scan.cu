@@ -34,7 +34,7 @@
  *   NAC  capacity of the per-thread aggregate accumulators (plain aggregate mode)
  *   ALL8 every plan column is 8 bytes wide (skips the width switch)
  */
-template <int NCC, int NAC, int MODE, bool ALL8, int U, bool VAR = false>
+template <int NCC, int NAC, int MODE, bool ALL8, int U, bool VAR = false, bool CASE = false>
 __global__ void __launch_bounds__(CG_THREADS, 4)
 cg_scan_kernel(const __grid_constant__ KPlan P)
 {
@@ -98,8 +98,8 @@ cg_scan_kernel(const __grid_constant__ KPlan P)
 					uint32_t r = base + (u * CG_THREADS + tid) * 2;
 					if (r < rows)
 					{
-						process_row<NCC, NAC, MODE, VAR>(P, v0[u], 0u, acc, removed);
-						if (r + 1 < rows) process_row<NCC, NAC, MODE, VAR>(P, v1[u], 0u, acc, removed);
+						process_row<NCC, NAC, MODE, VAR, CASE>(P, v0[u], 0u, acc, removed);
+						if (r + 1 < rows) process_row<NCC, NAC, MODE, VAR, CASE>(P, v1[u], 0u, acc, removed);
 					}
 				}
 			}
@@ -121,8 +121,8 @@ cg_scan_kernel(const __grid_constant__ KPlan P)
 						else
 							load_pair(vptr[c], r, len, P.isfloat[c], v0[c], v1[c]);
 					}
-				process_row<NCC, NAC, MODE, VAR>(P, v0, n0, acc, removed);
-				if (r + 1 < rows) process_row<NCC, NAC, MODE, VAR>(P, v1, n1, acc, removed);
+				process_row<NCC, NAC, MODE, VAR, CASE>(P, v0, n0, acc, removed);
+				if (r + 1 < rows) process_row<NCC, NAC, MODE, VAR, CASE>(P, v1, n1, acc, removed);
 			}
 		}
 	}
@@ -131,11 +131,11 @@ cg_scan_kernel(const __grid_constant__ KPlan P)
 	flush_thread<NAC, MODE, VAR>(P, acc, removed, scanned);
 }
 
-template <int NCC, int NAC, int MODE, bool ALL8, int U, bool VAR = false>
+template <int NCC, int NAC, int MODE, bool ALL8, int U, bool VAR = false, bool CASE = false>
 static int launch_variant(CgContext *ctx, const KPlan &plan, cudaStream_t stream)
 {
 	int occ = 0;
-	CG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, cg_scan_kernel<NCC, NAC, MODE, ALL8, U, VAR>, CG_THREADS, 0));
+	CG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, cg_scan_kernel<NCC, NAC, MODE, ALL8, U, VAR, CASE>, CG_THREADS, 0));
 	if (occ < 1) occ = 1;
 	uint32_t grid = (uint32_t) (ctx->sm_count * occ);
 	if (grid > plan.nselected) grid = plan.nselected;
@@ -143,7 +143,7 @@ static int launch_variant(CgContext *ctx, const KPlan &plan, cudaStream_t stream
 	bool overlap;
 	int rc = cg_chain_scan(ctx, stream, false, &overlap);     /* does not trigger its dependents early: ends a chain */
 	if (rc) return rc;
-	cg_scan_kernel<NCC, NAC, MODE, ALL8, U, VAR><<<grid, CG_THREADS, 0, stream>>>(plan);
+	cg_scan_kernel<NCC, NAC, MODE, ALL8, U, VAR, CASE><<<grid, CG_THREADS, 0, stream>>>(plan);
 	CG_CUDA(cudaGetLastError()); g_cg_launches++;
 	return CG_OK;
 }
@@ -173,6 +173,14 @@ static int launch_mode(CgContext *ctx, const KPlan &plan, bool all8, cudaStream_
 
 int cg_launch_scan(CgContext *ctx, const KPlan &plan, bool all8, cudaStream_t stream)
 {
+	/* plans with a CASE argument: one instantiation per table kind, any column width, variance included */
+	if (plan.ncase > 0)
+		switch (plan.mode)
+		{
+			case CG_MODE_GLOBAL: return launch_variant<CG_KMAX_COLS, CG_MAX_AGGS, CG_MODE_GLOBAL, false, 1, true, true>(ctx, plan, stream);
+			case CG_MODE_DENSE: return launch_variant<CG_KMAX_COLS, CG_MAX_AGGS, CG_MODE_DENSE, false, 1, true, true>(ctx, plan, stream);
+			default: return launch_variant<CG_KMAX_COLS, CG_MAX_AGGS, CG_MODE_HASH, false, 1, true, true>(ctx, plan, stream);
+		}
 	/* plans with a variance aggregate: one instantiation per table kind, any column width (the others keep theirs) */
 	if (cg_plan_has_variance(plan.aggs, plan.naggs))
 		switch (plan.mode)

@@ -31,16 +31,17 @@
  * Only the words every row touches get a cell; NULL-input counters and the NULL-key group
  * are rare and go straight to the global table.
  */
-template <int NCC, bool VAR>
+template <int NCC, bool VAR, bool CASE = false>
 __device__ __forceinline__ void small_accumulate(const KPlan &P, uint64_t *mine, uint32_t slot, const int64_t (&v)[NCC], uint32_t nullmask)
 {
 	uint64_t *e = mine + (size_t) slot * (uint32_t) P.nhot * CGS_THREADS;
 	e[0] += 1ull;
-	auto term = [&](int, const KAgg &g, bool noinput, uint64_t w0, uint64_t w1) {
+	auto term = [&](int a, const KAgg &g, bool noinput, uint64_t w0, uint64_t w1) {
 		if (noinput)
 		{
-			/* a filtered aggregate's no-input counter has a cell (rejected rows are common) */
-			if (g.filt || g.barg) e[P.hot_of_word[g.nullword] * CGS_THREADS] += 1ull;
+			/* a filtered aggregate's no-input counter has a cell (rejected rows are common), and so has a CASE's (arms that
+			 * give NULL are as common) */
+			if (g.filt || g.barg || (CASE && P.cnarms[a] > 0)) e[P.hot_of_word[g.nullword] * CGS_THREADS] += 1ull;
 			else atomicAdd((unsigned long long *) P.table + (uint64_t) slot * (uint64_t) P.stride + g.nullword, 1ull);
 			return;
 		}
@@ -55,7 +56,7 @@ __device__ __forceinline__ void small_accumulate(const KPlan &P, uint64_t *mine,
 	};
 	if constexpr (VAR)
 		/* sum(x^2): every limb word has a cell of its own (consecutive words: consecutive cells) */
-		row_terms<NCC, CG_MAX_AGGS, true>(P, v, nullmask, term, [&](int, const KAgg &g, uint64_t lo, uint64_t hi) {
+		row_terms<NCC, CG_MAX_AGGS, true, CASE>(P, v, nullmask, term, [&](int, const KAgg &g, uint64_t lo, uint64_t hi) {
 			uint64_t *q = e + P.hot_of_word[g.qword] * CGS_THREADS;
 			if (g.qlimbs == 1) *q += lo;
 			else
@@ -66,12 +67,12 @@ __device__ __forceinline__ void small_accumulate(const KPlan &P, uint64_t *mine,
 			}
 		});
 	else
-		row_terms<NCC, CG_MAX_AGGS>(P, v, nullmask, term);
+		row_terms<NCC, CG_MAX_AGGS, false, CASE>(P, v, nullmask, term);
 }
 
 /* K3 + K4 of one row: WHERE, the group's direct index, the terms into the group's cells (the NULL-key group's go to its
  * global entry) */
-template <int NCC, bool VAR>
+template <int NCC, bool VAR, bool CASE = false>
 __device__ __forceinline__ void small_row(const KPlan &P, uint64_t *mine, const int64_t (&v)[NCC], uint32_t nullmask, uint32_t &removed)
 {
 	if (!eval_where<NCC>(P, v, nullmask))
@@ -84,11 +85,11 @@ __device__ __forceinline__ void small_row(const KPlan &P, uint64_t *mine, const 
 	if (!group_key<NCC>(P, v, nullmask, key, key_null)) return;
 	const uint64_t slot = dense_slot_of_packed(P, key, key_null);
 	if (slot == ~0ull) return;
-	if (key_null) global_accumulate<NCC, CG_MAX_AGGS, VAR>(P, P.table + slot * (uint64_t) P.stride, v, nullmask);
-	else small_accumulate<NCC, VAR>(P, mine, (uint32_t) slot, v, nullmask);
+	if (key_null) global_accumulate<NCC, CG_MAX_AGGS, VAR, CASE>(P, P.table + slot * (uint64_t) P.stride, v, nullmask);
+	else small_accumulate<NCC, VAR, CASE>(P, mine, (uint32_t) slot, v, nullmask);
 }
 
-template <int NCC, bool ALL8, bool VAR = false>
+template <int NCC, bool ALL8, bool VAR = false, bool CASE = false>
 __global__ void __launch_bounds__(CGS_THREADS)
 cg_scan_small_kernel(const __grid_constant__ KPlan P)
 {
@@ -140,8 +141,8 @@ cg_scan_small_kernel(const __grid_constant__ KPlan P)
 					else
 						load_pair(vptr[c], r, len, P.isfloat[c], v0[c], v1[c]);
 				}
-			small_row<NCC, VAR>(P, mine, v0, n0, removed);
-			if (r + 1 < rows) small_row<NCC, VAR>(P, mine, v1, n1, removed);
+			small_row<NCC, VAR, CASE>(P, mine, v0, n0, removed);
+			if (r + 1 < rows) small_row<NCC, VAR, CASE>(P, mine, v1, n1, removed);
 		}
 	}
 
@@ -167,19 +168,19 @@ cg_scan_small_kernel(const __grid_constant__ KPlan P)
 	}
 }
 
-template <int NCC, bool ALL8, bool VAR = false>
+template <int NCC, bool ALL8, bool VAR = false, bool CASE = false>
 static int launch_small_variant(CgContext *ctx, const KPlan &plan, size_t smem, cudaStream_t stream)
 {
 	static size_t configured = 0, occ_smem = ~(size_t) 0;
 	static int occ = 0;
 	if (smem > configured)
 	{
-		CG_CUDA(cudaFuncSetAttribute(cg_scan_small_kernel<NCC, ALL8, VAR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
+		CG_CUDA(cudaFuncSetAttribute(cg_scan_small_kernel<NCC, ALL8, VAR, CASE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
 		configured = smem;
 	}
 	if (smem != occ_smem)
 	{
-		CG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, cg_scan_small_kernel<NCC, ALL8, VAR>, CGS_THREADS, smem));
+		CG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, cg_scan_small_kernel<NCC, ALL8, VAR, CASE>, CGS_THREADS, smem));
 		if (occ < 1) occ = 1;
 		occ_smem = smem;
 	}
@@ -189,7 +190,7 @@ static int launch_small_variant(CgContext *ctx, const KPlan &plan, size_t smem, 
 	bool overlap;
 	int rc = cg_chain_scan(ctx, stream, false, &overlap);     /* does not trigger its dependents early: ends a chain */
 	if (rc) return rc;
-	cg_scan_small_kernel<NCC, ALL8, VAR><<<grid, CGS_THREADS, smem, stream>>>(plan);
+	cg_scan_small_kernel<NCC, ALL8, VAR, CASE><<<grid, CGS_THREADS, smem, stream>>>(plan);
 	CG_CUDA(cudaGetLastError()); g_cg_launches++;
 	return CG_OK;
 }
@@ -203,7 +204,7 @@ static int hot_words(const KPlan &plan, int8_t *hot)
 	for (int a = 0; a < plan.naggs; a++)
 	{
 		const KAgg &g = plan.aggs[a];
-		if (g.filt || g.barg) is_hot[g.nullword] = true;
+		if (g.filt || g.barg || plan.cnarms[a] > 0) is_hot[g.nullword] = true;
 		if (g.kind == CG_AGG_COUNT_STAR || g.kind == CG_AGG_COUNT) continue;
 		is_hot[g.word0] = true;
 		if (two_sum_limbs<true>(g)) is_hot[g.word0 + 1] = true;
@@ -229,6 +230,7 @@ int cg_launch_scan_small(CgContext *ctx, const KPlan &plan_in, bool all8, cudaSt
 	KPlan plan = plan_in;
 	plan.nhot = hot_words(plan, plan.hot_of_word);
 	size_t smem = (size_t) plan.capacity * plan.nhot * sizeof(uint64_t) * CGS_THREADS;
+	if (plan.ncase > 0) return launch_small_variant<CG_KMAX_COLS, false, true, true>(ctx, plan, smem, stream);
 	if (cg_plan_has_variance(plan.aggs, plan.naggs)) return launch_small_variant<CG_KMAX_COLS, false, true>(ctx, plan, smem, stream);
 	if (plan.ncols <= 4)
 		return all8 ? launch_small_variant<4, true>(ctx, plan, smem, stream) : launch_small_variant<4, false>(ctx, plan, smem, stream);

@@ -278,6 +278,27 @@ typedef struct CgAggSpec
 #define CG_QX_OR (-2)
 #define CG_MAX_FILTER_QUALS 8
 
+/* Conditional aggregate argument ([PG] CaseExpr inside Aggref.args): sum(CASE WHEN c1 THEN r1 WHEN c2 THEN r2 ELSE r3 END).
+ * An arm is a WHEN tree and a result; nwhen = 0 marks the ELSE arm, which must be its aggregate's last arm.  The WHEN tree is
+ * the postfix token list when[0..nwhen) over CgScanDesc.filter_quals, in the filter_expr language (every atom kind).
+ * The result (form):
+ *   CG_CASE_NULL      the NULL constant
+ *   CG_CASE_CONST     the constant a[0]: an integer, or float8 bits when the aggregate is_float
+ *   CG_CASE_PRODUCT   product over nfactors (1..3) affine factors (a[f] + b[f] * column[f]), exactly as CgAggSpec's argument;
+ *                     NULL when a factor column is NULL in the row */
+#define CG_MAX_CASE_ARMS 16            /* the arms of all aggregates of a query together */
+enum { CG_CASE_NULL = 0, CG_CASE_CONST = 1, CG_CASE_PRODUCT = 2 };
+typedef struct CgCaseArm
+{
+	int32_t nwhen;                     /* 0 = ELSE */
+	int8_t when[CG_MAX_QEXPR];
+	int32_t form;                      /* CG_CASE_* */
+	int32_t nfactors;                  /* CG_CASE_PRODUCT: 1 .. 3 */
+	int32_t column[3];
+	int64_t a[3];                      /* CG_CASE_CONST: the constant in a[0] */
+	int64_t b[3];
+} CgCaseArm;
+
 typedef struct CgScanDesc
 {
 	int32_t nquals;
@@ -350,6 +371,38 @@ typedef struct CgScanDesc
 	CgInList in_lists[CG_MAX_IN_LISTS];
 	int32_t nin_values;
 	int64_t in_values[CG_MAX_IN_VALUES];
+	/* CASE arguments (CgCaseArm).  case_narms[a] > 0: aggregate a's argument is the searched CASE over the arms
+	 * case_arms[case_first[a] .. case_first[a] + case_narms[a]); two aggregates may name the same range (avg's sum and count).
+	 * case_narms[a] = 0 = no CASE, so a zero-filled tail is a query without CASE.  Per row that passes WHERE:
+	 *   - a row aggregate a's FILTER rejects is no input, and its CASE is not consulted;
+	 *   - otherwise the WHEN trees are evaluated in order under three-valued logic (UNKNOWN is not TRUE); the value is the
+	 *     result of the first arm whose tree is TRUE, else the ELSE arm's, else NULL;
+	 *   - only the chosen arm's result is evaluated: an int64 overflow or a term_abs_bound violation in an arm that was not
+	 *     chosen raises nothing; in the chosen arm it fails the scan as it does for a plain argument (CG_EUNSUPPORTED /
+	 *     CG_EINVAL);
+	 *   - a NULL value is no input: it is counted in the aggregate's no-input word, as a NULL argument is.
+	 * So sum(CASE WHEN c THEN x ELSE 0 END) gives 0 for a group whose rows all fail c, where sum(x) FILTER (WHERE c) gives
+	 * NULL; count(CASE WHEN c THEN 1 END) counts the rows where c is TRUE.
+	 * Kinds: CG_AGG_COUNT, CG_AGG_SUM, CG_AGG_MIN, CG_AGG_MAX and CG_AGG_VARIANCE, with nfactors = 0 (the arms carry the terms).
+	 * A CASE aggregate has exactly the words of its kind (with the no-input word), so fetch, export, merge and combine are
+	 * unchanged, and optimistic packing follows sum's rule.  An integer CASE has integer results at one scale the caller
+	 * chose (a, b and the constants pre-scaled; the value comes back exact at that scale, but [PG]'s display scale of a
+	 * numeric CASE whose arms differ in scale depends on which arms supplied inputs, which the words do not record); a float
+	 * CASE has float8 results.  Columns an arm reads are plan columns (staged, counted toward the column limit) and the
+	 * atoms of its WHEN tree share the filter_quals pool.  cg_relation_bounds gives a CASE sum the largest bound over its
+	 * arms (a constant counts |k|, a NULL arm 0); WHEN atoms take no part in bounds or chunk-group skipping.
+	 * A scan or join into a partial must carry the CASE arguments the partial was created with (the same arms in the same
+ * order, wherever they sit in case_arms), else CG_EINVAL.
+ * CG_EINVAL: a CASE on another kind, or with nfactors != 0; an arm range outside [0, ncase_arms) or ncase_arms >
+	 * CG_MAX_CASE_ARMS; an ELSE arm that is not the last of its range; a malformed WHEN tree or a token outside the pool; a
+	 * bad form, a product with nfactors outside 1 .. 3 or a column outside [0, natts).  Column types are checked as for a
+	 * plain argument of the kind (integer / float mismatch CG_EINVAL; variance of a float CG_EUNSUPPORTED, of char(1)
+	 * CG_EINVAL). */
+	int32_t case_first[CG_MAX_AGGS];
+	int32_t case_narms[CG_MAX_AGGS];
+	int32_t ncase_arms;
+	int32_t reserved2;
+	CgCaseArm case_arms[CG_MAX_CASE_ARMS];
 } CgScanDesc;
 
 /* EXPLAIN ANALYZE counters (columnar_customscan.c:1966-1999 and ExecScan instrumentation) */

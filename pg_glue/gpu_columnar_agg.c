@@ -384,6 +384,151 @@ translate_where(Node *node, TupleDesc tupdesc, CgScanDesc *desc, CgQual *atoms, 
 	return true;
 }
 
+/* the argument forms a CASE arm reads (include/citus_gpu.h, CgCaseArm): int2 / int4 / int8, or float8 for a float CASE */
+static bool
+case_type_supported(Oid type)
+{
+	return type == INT2OID || type == INT4OID || type == INT8OID || type == FLOAT8OID;
+}
+
+/* a CASE result: a Var of the CASE's own type (through strip_to_var) -> a bare-column product, a Const of that type -> a
+ * constant, a NULL Const -> the NULL result; false for anything else (casts, arithmetic) */
+static bool
+translate_case_result(Node *node, Oid type, TupleDesc tupdesc, CgCaseArm *arm)
+{
+	Var *var = strip_to_var(node);
+	if (var != NULL)
+	{
+		if (var->varattno <= 0 || var->varattno > tupdesc->natts || var->vartype != type)
+			return false;
+		arm->form = CG_CASE_PRODUCT;
+		arm->nfactors = 1;
+		arm->column[0] = var->varattno - 1;
+		arm->a[0] = 0;
+		if (type == FLOAT8OID) { double one = 1.0; memcpy(&arm->b[0], &one, sizeof one); }
+		else arm->b[0] = 1;
+		return true;
+	}
+	if (node == NULL || !IsA(node, Const) || ((Const *) node)->consttype != type)
+		return false;
+	const Const *k = (const Const *) node;
+	arm->form = k->constisnull ? CG_CASE_NULL : CG_CASE_CONST;
+	arm->a[0] = k->constisnull ? 0 : datum_to_i64(k->constvalue, type);      /* float8 bits for a float CASE */
+	return true;
+}
+
+/* "x = k" over a column and a non-NULL constant of its type with the type's btree equality -> one atom of the pool, appended
+ * to the arm's WHEN tree (the simple CASE's "CASE x WHEN k" and NULLIF's test) */
+static bool
+case_equality_atom(Var *var, Const *k, Oid opno, TupleDesc tupdesc, CgScanDesc *desc, CgCaseArm *arm)
+{
+	int attlen, type_class;
+	if (var == NULL || k == NULL || k->constisnull || var->varattno <= 0 || var->varattno > tupdesc->natts ||
+		!type_is_supported(var->vartype, &attlen, &type_class) || k->consttype != var->vartype ||
+		btree_strategy(opno, var->vartype) != BTEqualStrategyNumber || desc->nfilter_quals >= CG_MAX_FILTER_QUALS || arm->nwhen >= CG_MAX_QEXPR)
+		return false;
+	CgQual *q = &desc->filter_quals[desc->nfilter_quals];
+	q->column = var->varattno - 1;
+	q->op = CG_OP_EQ;
+	q->konst = datum_to_i64(k->constvalue, var->vartype);
+	arm->when[arm->nwhen++] = (int8_t) desc->nfilter_quals++;
+	return true;
+}
+
+/* the next free arm of the descriptor (zeroed), NULL when CG_MAX_CASE_ARMS are taken */
+static CgCaseArm *
+next_arm(CgScanDesc *desc)
+{
+	if (desc->ncase_arms >= CG_MAX_CASE_ARMS)
+		return NULL;
+	CgCaseArm *arm = &desc->case_arms[desc->ncase_arms++];
+	memset(arm, 0, sizeof *arm);
+	return arm;
+}
+
+/*
+ * A conditional aggregate argument -> the arms of aggregate desc->naggs (include/citus_gpu.h, CgScanDesc.case_arms):
+ *   CASE WHEN c THEN r ... [ELSE r] END     each WHEN through translate_where into the filter atom pool
+ *   CASE x WHEN k THEN r ... END            each WHEN a CaseTestExpr = Const, as the atom "x = k"
+ *   COALESCE(x, k)                          WHEN x IS NOT NULL THEN x ELSE k
+ *   NULLIF(x, k)                            WHEN x = k THEN NULL ELSE x
+ * with results as translate_case_result takes them, of int2 / int4 / int8 or float8.  *type = the argument's type.  false
+ * (the reference's executor runs the query) for any other form, or when the pool or the arm table is full.
+ */
+static bool
+translate_case_arg(Node *arg, TupleDesc tupdesc, CgScanDesc *desc, Oid *type)
+{
+	const int a = desc->naggs, first = desc->ncase_arms;
+	CgCaseArm *arm;
+	if (IsA(arg, CaseExpr))
+	{
+		CaseExpr *ce = (CaseExpr *) arg;
+		*type = ce->casetype;
+		Var *subject = ce->arg != NULL ? strip_to_var((Node *) ce->arg) : NULL;
+		if (!case_type_supported(*type) || (ce->arg != NULL && subject == NULL))
+			return false;
+		ListCell *lc;
+		foreach(lc, ce->args)
+		{
+			CaseWhen *w = (CaseWhen *) lfirst(lc);
+			if ((arm = next_arm(desc)) == NULL)
+				return false;
+			if (ce->arg != NULL)
+			{
+				/* the simple form: the planner wrote each WHEN as "CaseTestExpr = Const" */
+				OpExpr *op = IsA(w->expr, OpExpr) ? (OpExpr *) w->expr : NULL;
+				if (op == NULL || list_length(op->args) != 2 || !IsA((Node *) linitial(op->args), CaseTestExpr) ||
+					!IsA((Node *) lsecond(op->args), Const) ||
+					!case_equality_atom(subject, (Const *) lsecond(op->args), op->opno, tupdesc, desc, arm))
+					return false;
+			}
+			else if (!translate_where((Node *) w->expr, tupdesc, desc, desc->filter_quals, &desc->nfilter_quals, CG_MAX_FILTER_QUALS, arm->when,
+									  &arm->nwhen))
+				return false;
+			if (!translate_case_result((Node *) w->result, *type, tupdesc, arm))
+				return false;
+		}
+		/* [PG] a CASE without ELSE has a NULL Const as its defresult */
+		if (ce->defresult != NULL && ((arm = next_arm(desc)) == NULL || !translate_case_result((Node *) ce->defresult, *type, tupdesc, arm)))
+			return false;
+	}
+	else if (IsA(arg, CoalesceExpr))
+	{
+		CoalesceExpr *co = (CoalesceExpr *) arg;
+		*type = co->coalescetype;
+		Var *x = list_length(co->args) == 2 ? strip_to_var((Node *) linitial(co->args)) : NULL;
+		if (!case_type_supported(*type) || x == NULL || x->varattno <= 0 || x->varattno > tupdesc->natts || desc->nfilter_quals >= CG_MAX_FILTER_QUALS ||
+			(arm = next_arm(desc)) == NULL)
+			return false;
+		CgQual *q = &desc->filter_quals[desc->nfilter_quals];
+		q->column = x->varattno - 1;
+		q->op = CG_OP_IS_NOT_NULL;
+		q->konst = 0;
+		arm->when[arm->nwhen++] = (int8_t) desc->nfilter_quals++;
+		if (!translate_case_result((Node *) linitial(co->args), *type, tupdesc, arm) || (arm = next_arm(desc)) == NULL ||
+			!translate_case_result((Node *) lsecond(co->args), *type, tupdesc, arm) || arm->form != CG_CASE_CONST)
+			return false;
+	}
+	else if (IsA(arg, NullIfExpr))
+	{
+		NullIfExpr *ni = (NullIfExpr *) arg;
+		*type = ni->opresulttype;
+		Var *x = list_length(ni->args) == 2 ? strip_to_var((Node *) linitial(ni->args)) : NULL;
+		Node *k = list_length(ni->args) == 2 ? (Node *) lsecond(ni->args) : NULL;
+		if (!case_type_supported(*type) || k == NULL || !IsA(k, Const) || (arm = next_arm(desc)) == NULL ||
+			!case_equality_atom(x, (Const *) k, ni->opno, tupdesc, desc, arm))
+			return false;
+		arm->form = CG_CASE_NULL;
+		if ((arm = next_arm(desc)) == NULL || !translate_case_result((Node *) x, *type, tupdesc, arm))
+			return false;
+	}
+	else
+		return false;
+	desc->case_first[a] = first;
+	desc->case_narms[a] = desc->ncase_arms - first;
+	return desc->case_narms[a] > 0;
+}
+
 /* the most accumulator words the library can lay out for the aggregate list (include/citus_gpu.h, CG_MAX_WORDS): word 0
  * plus per aggregate its widest form, whatever the term bounds turn out to be */
 static int
@@ -443,35 +588,52 @@ translate_aggref(Aggref *agg, TupleDesc tupdesc, CgScanDesc *desc, GpuOutColumn 
 		desc->naggs++;
 		return true;
 	}
+	/* the argument: a bare column, or a conditional expression whose arms read columns and constants (translate_case_arg);
+	 * vtype = its type either way */
 	Var *var = strip_to_var(arg);
-	int attlen, type_class;
-	if (var == NULL || var->varattno <= 0 || var->varattno > tupdesc->natts || !type_is_supported(var->vartype, &attlen, &type_class))
-		return false;
-	spec->nfactors = 1;
-	spec->column[0] = var->varattno - 1;
-	spec->is_float = type_class == CG_TYPE_FLOAT;
-	spec->a[0] = 0;
-	if (spec->is_float) { double one = 1.0; memcpy(&spec->b[0], &one, sizeof one); }
-	else spec->b[0] = 1;
+	const bool is_case = var == NULL;
+	Oid vtype;
+	desc->case_narms[desc->naggs] = 0;
+	if (is_case)
+	{
+		if (!translate_case_arg(arg, tupdesc, desc, &vtype))
+			return false;
+		spec->nfactors = 0;
+		spec->is_float = vtype == FLOAT8OID;
+	}
+	else
+	{
+		int attlen, type_class;
+		if (var->varattno <= 0 || var->varattno > tupdesc->natts || !type_is_supported(var->vartype, &attlen, &type_class))
+			return false;
+		vtype = var->vartype;
+		spec->nfactors = 1;
+		spec->column[0] = var->varattno - 1;
+		spec->is_float = type_class == CG_TYPE_FLOAT;
+		spec->a[0] = 0;
+		if (spec->is_float) { double one = 1.0; memcpy(&spec->b[0], &one, sizeof one); }
+		else spec->b[0] = 1;
+	}
 	if (strcmp(name, "count") == 0)
 	{
-		spec->kind = CG_AGG_COUNT; spec->is_float = 0; spec->b[0] = 1;
+		spec->kind = CG_AGG_COUNT;
+		if (!is_case) { spec->is_float = 0; spec->b[0] = 1; }
 		out->kind = GPU_OUT_COUNT; out->type = INT8OID;
 	}
 	else if (strcmp(name, "sum") == 0)
 	{
 		spec->kind = CG_AGG_SUM;
-		if (spec->is_float) { out->kind = GPU_OUT_SUM_FLOAT8; out->type = var->vartype == FLOAT4OID ? FLOAT4OID : FLOAT8OID; }
-		else if (var->vartype == INT8OID) { out->kind = GPU_OUT_SUM_NUMERIC; out->type = NUMERICOID; }   /* [PG] sum(int8) is numeric */
-		else if (var->vartype == INT4OID || var->vartype == INT2OID) { out->kind = GPU_OUT_SUM_INT8; out->type = INT8OID; }
+		if (spec->is_float) { out->kind = GPU_OUT_SUM_FLOAT8; out->type = vtype == FLOAT4OID ? FLOAT4OID : FLOAT8OID; }
+		else if (vtype == INT8OID) { out->kind = GPU_OUT_SUM_NUMERIC; out->type = NUMERICOID; }   /* [PG] sum(int8) is numeric */
+		else if (vtype == INT4OID || vtype == INT2OID) { out->kind = GPU_OUT_SUM_INT8; out->type = INT8OID; }
 		else return false;
-		if (var->vartype == FLOAT4OID) return false;          /* [PG] sum(float4) accumulates in float4: not what the kernels do */
+		if (vtype == FLOAT4OID) return false;          /* [PG] sum(float4) accumulates in float4: not what the kernels do */
 	}
 	else if (strcmp(name, "min") == 0 || strcmp(name, "max") == 0 || strcmp(name, "any_value") == 0)
 	{
 		/* any_value(x): any non-NULL input -- the minimum is one */
 		spec->kind = name[1] == 'a' ? CG_AGG_MAX : CG_AGG_MIN;
-		out->kind = GPU_OUT_MINMAX; out->type = var->vartype;
+		out->kind = GPU_OUT_MINMAX; out->type = vtype;
 	}
 	else if (strcmp(name, "var_pop") == 0 || strcmp(name, "var_samp") == 0 || strcmp(name, "variance") == 0 ||
 			 strcmp(name, "stddev_pop") == 0 || strcmp(name, "stddev_samp") == 0 || strcmp(name, "stddev") == 0)
@@ -479,7 +641,7 @@ translate_aggref(Aggref *agg, TupleDesc tupdesc, CgScanDesc *desc, GpuOutColumn 
 		/* over int2 / int4 / int8 PostgreSQL keeps N, sum(x) and sum(x^2) as exact integers and the result is numeric: one
 		 * state for all six names, the name picks the final function (cg_numeric_var_out).  A float argument keeps the
 		 * reference's executor (float8_accum cannot be matched bit for bit) */
-		if (var->vartype != INT2OID && var->vartype != INT4OID && var->vartype != INT8OID)
+		if (vtype != INT2OID && vtype != INT4OID && vtype != INT8OID)
 			return false;
 		const bool pop = strcmp(name, "var_pop") == 0 || strcmp(name, "stddev_pop") == 0;
 		spec->kind = CG_AGG_VARIANCE;
@@ -489,7 +651,7 @@ translate_aggref(Aggref *agg, TupleDesc tupdesc, CgScanDesc *desc, GpuOutColumn 
 	else if (strcmp(name, "bit_and") == 0 || strcmp(name, "bit_or") == 0)
 	{
 		/* bare int2 / int4 / int8 column; the result has the argument's type (words hold it sign-extended) */
-		if (var->vartype != INT2OID && var->vartype != INT4OID && var->vartype != INT8OID)
+		if (is_case || (vtype != INT2OID && vtype != INT4OID && vtype != INT8OID))
 			return false;
 		spec->kind = name[4] == 'a' ? CG_AGG_BIT_AND : CG_AGG_BIT_OR;
 		out->kind = GPU_OUT_MINMAX; out->type = var->vartype;

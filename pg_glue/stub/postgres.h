@@ -128,7 +128,8 @@ List *list_delete_ptr(List *list, void *datum);
 
 /* ---- nodes ---- */
 typedef enum NodeTag { T_Invalid = 0, T_Var, T_Const, T_OpExpr, T_BoolExpr, T_Aggref, T_TargetEntry, T_RelabelType, T_CustomScan, T_CustomScanState,
-					   T_CustomPath, T_Query, T_NullTest, T_FuncExpr, T_ScalarArrayOpExpr } NodeTag;
+					   T_CustomPath, T_Query, T_NullTest, T_FuncExpr, T_ScalarArrayOpExpr, T_CaseExpr, T_CaseWhen, T_CaseTestExpr,
+					   T_CoalesceExpr, T_NullIfExpr } NodeTag;
 typedef struct Node { NodeTag type; } Node;
 #define nodeTag(nodeptr) (((const Node *) (nodeptr))->type)
 #define IsA(nodeptr, _type_) (nodeTag(nodeptr) == T_##_type_)
@@ -146,6 +147,11 @@ typedef struct RelabelType { Expr xpr; Expr *arg; Oid resulttype; } RelabelType;
 typedef struct ScalarArrayOpExpr { Expr xpr; Oid opno; Oid opfuncid; Oid hashfuncid; Oid negfuncid; bool useOr; Oid inputcollid; List *args; int location; } ScalarArrayOpExpr;
 typedef enum NullTestType { IS_NULL, IS_NOT_NULL } NullTestType;
 typedef struct NullTest { Expr xpr; Expr *arg; NullTestType nulltesttype; bool argisrow; int location; } NullTest;
+typedef struct CaseExpr { Expr xpr; Oid casetype; Oid casecollid; Expr *arg; List *args; Expr *defresult; int location; } CaseExpr;
+typedef struct CaseWhen { Expr xpr; Expr *expr; Expr *result; int location; } CaseWhen;
+typedef struct CaseTestExpr { Expr xpr; Oid typeId; int32 typeMod; Oid collation; } CaseTestExpr;
+typedef struct CoalesceExpr { Expr xpr; Oid coalescetype; Oid coalescecollid; List *args; int location; } CoalesceExpr;
+typedef OpExpr NullIfExpr;                      /* [PG] an OpExpr of the "=" operator, tagged T_NullIfExpr */
 typedef struct Aggref { Expr xpr; Oid aggfnoid; Oid aggtype; List *args; List *aggorder; List *aggdistinct; Expr *aggfilter; bool aggstar; char aggkind; } Aggref;
 typedef struct TargetEntry { Expr xpr; Expr *expr; AttrNumber resno; char *resname; unsigned ressortgroupref; bool resjunk; } TargetEntry;
 typedef struct SortGroupClause { NodeTag type; unsigned tleSortGroupRef; Oid eqop; } SortGroupClause;
