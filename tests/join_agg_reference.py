@@ -9,8 +9,7 @@ are equal when their int64 values are equal; a NULL key joins nothing, on either
 other.  The rows come out probe row by probe row, each probe row's matches in build-row order; a join has no order, so
 callers compare multisets (or aggregates).
 
-The joined columns feed the existing aggregate references unchanged (reference.aggregate,
-column_compare_reference.aggregate, bool_bit_reference.aggregate, variance_reference.aggregate).
+The joined columns feed the exact aggregate reference unchanged (reference.aggregate).
 """
 from __future__ import annotations
 

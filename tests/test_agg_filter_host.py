@@ -1,7 +1,8 @@
 """Aggregate FILTER (WHERE ...) on the host side, without a GPU: the descriptor make_desc builds, the checks of the new
 CgScanDesc fields, the generated kernels of every kind with filters, chunk-group skipping and bounds that ignore
-filters, and the composition the GPU tests take their expected answers from."""
+filters, and FILTER in the exact reference against its composition from aggregates without filters."""
 import ctypes as C
+import dataclasses
 
 import numpy as np
 import pytest
@@ -19,30 +20,6 @@ def cg():
     from citus_b200 import capi, columnar
     capi.lib()
     return columnar
-
-
-def as_tree(where):
-    """a WHERE / FILTER in any accepted form -> a tree the reference evaluates (None = no condition)"""
-    if isinstance(where, tuple) and where and where[0] in ("and", "or"):
-        return where
-    if isinstance(where, tuple):
-        return ("and", where)
-    return ("and",) + tuple(where) if where else None
-
-
-def filtered_reference(cols, nulls, where, group_cols, aggs, float_cols=()):
-    """PostgreSQL's FILTER by composition: the groups are those of WHERE alone; aggregate j of a group is the reference
-    aggregate over ("and", WHERE, FILTER_j), or no input (count 0, SQL NULL) where that has no row of the group"""
-    res = ref.aggregate(cols, nulls, where, group_cols, aggs, float_cols)
-    w = as_tree(where)
-    for j, a in enumerate(aggs):
-        if getattr(a, "filter", None) is None:
-            continue
-        f = as_tree(a.filter)
-        sub = ref.aggregate(cols, nulls, ("and", w, f) if w else f, group_cols, [a], float_cols)
-        for key, per in res.groups.items():
-            per[j] = sub.groups[key][0] if key in sub.groups else ref.AggResult()
-    return res
 
 
 def compile_check(cg, d, cols, kmin, kmax, rows, nullable=0):
@@ -162,7 +139,7 @@ def test_chunk_mask_and_bounds_ignore_filters(cg):
         assert cg.relation_bounds(rel, d) == cg.relation_bounds(rel, plain)
 
 
-# --------------------------------------------------------------------------- the composition the GPU tests use
+# --------------------------------------------------------------------------- FILTER in the exact reference
 def test_composition_reference_on_hand_made_tables():
     class A:
         def __init__(self, kind, factors=(), is_float=False, filter=None):
@@ -174,7 +151,7 @@ def test_composition_reference_on_hand_made_tables():
     cols, nulls = [k, x, y], [None, xn, None]
     aggs = [A(0, filter=(2, "=", 1)), A(1, [(1, 0, 1)], filter=(2, "=", 1)), A(2, [(1, 0, 1)], filter=(2, "=", 1)),
             A(3, [(1, 0, 1)], filter=("or", (1, ">", 4), (2, "=", 1))), A(0), A(4, [(1, 0, 1)], filter=(1, ">", 1000))]
-    r = filtered_reference(cols, nulls, [(0, "<", 3)], [0], aggs)
+    r = ref.aggregate(cols, nulls, [(0, "<", 3)], [0], aggs)
     assert set(r.groups) == {(1,), (2,)}                          # group 2 exists though every filter on y rejects it
     g1, g2 = r.groups[(1,)], r.groups[(2,)]
     assert [g1[0].count, g1[1].count, g1[2].count, g1[2].sum] == [2, 1, 1, 9]   # the NULL x of row 1 is no input of count(x)
@@ -183,10 +160,81 @@ def test_composition_reference_on_hand_made_tables():
     assert g1[5].count == 0 and g1[5].max is None                 # a filter that matches nothing: NULL
     # a filter row that would overflow is no input: no overflow
     big = [2**62, 3, 2**62]
-    r = filtered_reference([[0, 0, 0], big], None, [], [], [A(2, [(1, 0, 1), (1, 0, 1)], filter=(1, "<", 10))])
+    r = ref.aggregate([[0, 0, 0], big], None, [], [], [A(2, [(1, 0, 1), (1, 0, 1)], filter=(1, "<", 10))])
     assert not ref.overflows(r) and r.groups[()][0].sum == 9
-    r = filtered_reference([[0, 0, 0], big], None, [], [], [A(2, [(1, 0, 1), (1, 0, 1)], filter=(1, ">", 10))])
+    r = ref.aggregate([[0, 0, 0], big], None, [], [], [A(2, [(1, 0, 1), (1, 0, 1)], filter=(1, ">", 10))])
     assert ref.overflows(r)
     # the plain aggregate over zero accepted rows keeps its group from WHERE
-    r = filtered_reference(cols, nulls, [], [], [A(0, filter=(0, ">", 9)), A(2, [(1, 0, 1)], filter=(0, ">", 9))])
+    r = ref.aggregate(cols, nulls, [], [], [A(0, filter=(0, ">", 9)), A(2, [(1, 0, 1)], filter=(0, ">", 9))])
     assert r.groups[()][0].count == 0 and r.groups[()][1].count == 0
+
+
+ATTLENS, FC, SCALES = [2, 4, 8, 8, 8, 8], (3,), {4: 2}     # edge_relation's columns; column 4 read as numeric(p, 2)
+
+
+def random_language(rng, n=300, forms=("const", "in", "null", "column")):
+    """(cols, nulls, atom, agg): an edge_relation of n rows, a random atom of one of `forms` over it (edge constants of
+    its chunks, IN lists with and without NULL, IS [NOT] NULL, column-to-column atoms) and agg(kind, filter), a random
+    aggregate of that kind with that FILTER"""
+    from citus_b200 import columnar
+    cols, nulls = edge_relation(rng, n, 120, 30)
+    pools = constant_pools(ref.skip_minmax(cols, nulls, 120, 30, FC), ATTLENS, FC)
+    ints = (0, 1, 2, 4, 5)
+
+    def pick(seq):
+        return seq[int(rng.integers(0, len(seq)))]
+
+    def atom():
+        c, form = int(rng.integers(0, 6)), pick(forms)
+        if form == "in":
+            elems = [pick(pools[c]) for _ in range(int(rng.integers(0, 5)))] + ([None] if rng.random() < 0.3 else [])
+            return (c, pick(("in", "not in")), tuple(elems))
+        if form == "null":
+            return (c, pick(("is null", "is not null")))
+        if form == "column":
+            return (c, pick(OPS), columnar.Col(3 if c == 3 else pick(ints)))
+        return (c, pick(OPS), pick(pools[c]))
+
+    def agg(kind, filter=None):
+        if kind == ref.COUNT_STAR:
+            return columnar.Agg(kind, filter=filter)
+        if kind in (ref.BOOL_AND, ref.BOOL_OR):
+            return columnar.Agg(kind, filter=filter, arg=random_tree(rng, atom, 3))
+        is_float = kind in (ref.COUNT, ref.SUM, ref.MIN, ref.MAX) and rng.random() < 0.3
+        col = 3 if is_float else pick(ints)
+        if kind in (ref.BIT_AND, ref.BIT_OR) or rng.random() < 0.5:
+            return columnar.Agg(kind, [(col, 0, 1)], is_float, filter=filter)
+        return columnar.Agg(kind, [(col, int(rng.integers(-3, 4)), int(rng.integers(-2, 3)))], is_float, filter=filter)
+    return cols, nulls, atom, agg
+
+
+def map_atoms(tree, fn):
+    """the condition as a tree with every atom replaced by fn(atom); None stays None"""
+    tree = ref.as_tree(tree)
+    if tree is None:
+        return None
+    return (tree[0],) + tuple(map_atoms(a, fn) if a[0] in ("and", "or") else fn(a) for a in tree[1:])
+
+
+def test_filter_equals_its_composition_for_every_kind():
+    """aggregate j with FILTER_j equals aggregate j without it over (WHERE AND FILTER_j), inside the groups of WHERE
+    alone (no input where that leaves a group no row), for every kind and atom form"""
+    rng = np.random.default_rng(20261016)
+    for trial in range(120):
+        if trial % 40 == 0:
+            cols, nulls, atom, agg = random_language(rng)
+        where = random_tree(rng, atom, 4) if trial % 5 else []
+        group = [[], [5], [0]][trial % 3]
+        aggs = [agg(int(k), random_tree(rng, atom, 3) if rng.random() < 0.7 else None) for k in rng.integers(0, 10, 4)]
+        plain = [dataclasses.replace(a, filter=None) for a in aggs]
+        got = ref.aggregate(cols, nulls, where, group, aggs, FC, SCALES)
+        want = ref.aggregate(cols, nulls, where, group, plain, FC, SCALES)
+        w = ref.as_tree(where)
+        for j, a in enumerate(aggs):
+            if a.filter is None:
+                continue
+            f = ref.as_tree(a.filter)
+            sub = ref.aggregate(cols, nulls, ("and", w, f) if w else f, group, [plain[j]], FC, SCALES)
+            for key, per in want.groups.items():
+                per[j] = sub.groups[key][0] if key in sub.groups else ref.AggResult()
+        assert repr(got) == repr(want), (where, group, aggs)

@@ -8,7 +8,6 @@ import os
 import numpy as np
 import pytest
 
-import bool_bit_reference as bref
 import reference as ref
 from test_agg_filter_host import compile_check
 from test_where_reference import constant_pools, edge_relation, random_tree
@@ -197,9 +196,9 @@ def bool_agg_queries():
     """the six bool_agg.out queries: (WHERE, GROUP BY, aggregates); every(p) is bool_and(p)"""
     ID, VAL, FLAG, KIND = range(4)
     flag = (FLAG, "=", 1)
-    three = [A(bref.BOOL_AND, arg=flag), A(bref.BOOL_OR, arg=flag), A(bref.BOOL_AND, arg=flag)]
-    expr = [A(bref.BOOL_OR, arg=("or", (VAL, ">", 2), (ID, "<", 2))), A(bref.BOOL_AND, arg=(VAL, "<", 3))]
-    bits = [A(bref.BIT_AND, [(VAL, 0, 1)]), A(bref.BIT_OR, [(VAL, 0, 1)])]
+    three = [A(ref.BOOL_AND, arg=flag), A(ref.BOOL_OR, arg=flag), A(ref.BOOL_AND, arg=flag)]
+    expr = [A(ref.BOOL_OR, arg=("or", (VAL, ">", 2), (ID, "<", 2))), A(ref.BOOL_AND, arg=(VAL, "<", 3))]
+    bits = [A(ref.BIT_AND, [(VAL, 0, 1)]), A(ref.BIT_OR, [(VAL, 0, 1)])]
     return [([], [], three), ([], [KIND], three), ([], [], expr), ([], [KIND], expr), ([flag], [], bits), ([], [FLAG], bits)]
 
 
@@ -211,7 +210,7 @@ def golden_rows(result, group_cols, aggs):
         for a, st in zip(aggs, per):
             if st.value is None:
                 cells.append("")
-            elif a.kind in (bref.BOOL_AND, bref.BOOL_OR):
+            elif a.kind in (ref.BOOL_AND, ref.BOOL_OR):
                 cells.append("t" if st.value else "f")
             else:
                 cells.append(str(st.value))
@@ -223,7 +222,7 @@ def test_reference_reproduces_the_bool_agg_goldens():
     g, cols = bool_agg_case()
     assert len(g["queries"]) == 6
     for (sql, want), (where, group, aggs) in zip(g["queries"], bool_agg_queries()):
-        got = golden_rows(bref.aggregate(cols, None, where, group, aggs), group, aggs)
+        got = golden_rows(ref.aggregate(cols, None, where, group, aggs), group, aggs)
         assert sorted(got) == sorted(want), sql
 
 
@@ -234,13 +233,13 @@ def test_reference_three_valued_bool_aggregates_by_hand():
     x = [5, 0, -1, 0]
     y = [0, 1, 1, 0]
     cols, nulls = [k, x, y], [None, [0, 1, 0, 1], None]
-    aggs = [A(bref.BOOL_AND, arg=(1, ">", 0)), A(bref.BOOL_OR, arg=(1, ">", 0)), A(bref.BOOL_OR, arg=("or", (1, ">", 0), (2, "=", 1))),
-            A(bref.BOOL_AND, arg=("and", (1, ">", 0), (2, "=", 1))), A(bref.BIT_AND, [(1, 0, 1)]), A(bref.BIT_OR, [(1, 0, 1)])]
-    r = bref.aggregate(cols, nulls, [], [0], aggs)
+    aggs = [A(ref.BOOL_AND, arg=(1, ">", 0)), A(ref.BOOL_OR, arg=(1, ">", 0)), A(ref.BOOL_OR, arg=("or", (1, ">", 0), (2, "=", 1))),
+            A(ref.BOOL_AND, arg=("and", (1, ">", 0), (2, "=", 1))), A(ref.BIT_AND, [(1, 0, 1)]), A(ref.BIT_OR, [(1, 0, 1)])]
+    r = ref.aggregate(cols, nulls, [], [0], aggs)
     g1, g2 = r.groups[(1,)], r.groups[(2,)]
     assert [(s.count, s.value) for s in g1] == [(1, True), (1, True), (2, True), (1, False), (1, 5), (1, 5)]
     assert [(s.count, s.value) for s in g2] == [(1, False), (1, False), (1, True), (2, False), (1, -1), (1, -1)]
-    r = bref.aggregate([[0, 0], [0, 0]], [None, [1, 1]], [], [], aggs[:2] + aggs[4:])     # every row UNKNOWN / NULL: no input
+    r = ref.aggregate([[0, 0], [0, 0]], [None, [1, 1]], [], [], aggs[:2] + aggs[4:])     # every row UNKNOWN / NULL: no input
     assert all(s.count == 0 and s.value is None for s in r.groups[()])
-    r = bref.aggregate([[0, 0, 0], [-2**63, -1, 2**63 - 1]], None, [], [], aggs[4:])
+    r = ref.aggregate([[0, 0, 0], [-2**63, -1, 2**63 - 1]], None, [], [], aggs[4:])
     assert [s.value for s in r.groups[()]] == [0, -1]

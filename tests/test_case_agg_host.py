@@ -1,5 +1,5 @@
-"""CASE aggregate arguments (columnar.Case) on the host side, without a GPU: tests/case_agg_reference.py against a
-row-at-a-time loop, the descriptor make_desc writes, every refusal of a CASE descriptor, cg_relation_bounds of CASE
+"""CASE aggregate arguments (columnar.Case) on the host side, without a GPU: tests/reference.py against a
+row-at-a-time loop and against FILTER, the descriptor make_desc writes, every refusal of a CASE descriptor, cg_relation_bounds of CASE
 aggregates against the skip lists, and the generated kernels of every kind and form with CASE arms, their source shape,
 and one source for one shape whatever its constants."""
 import ctypes as C
@@ -8,7 +8,6 @@ import itertools
 import numpy as np
 import pytest
 
-import case_agg_reference as caseref
 import reference as ref
 from test_in_null_atoms_host import compile_check
 
@@ -43,7 +42,7 @@ def test_reference_against_a_row_loop(cg):
         case = Case([((1, "<", k1), 2), (("or", (1, ">", k2), (2, "is null")), Const(k3))],
                     **({} if trial % 5 == 0 else {"else_": els}))
         aggs = [cg.sum_(case), cg.count(case), cg.min_(case), cg.max_(case, filter=(0, "<>", 1))]
-        got = caseref.aggregate(cols, nulls, [], [0], aggs)
+        got = ref.aggregate(cols, nulls, [], [0], aggs)
 
         def value(r):
             x1 = None if nulls[1][r] else int(cols[1][r])
@@ -71,11 +70,34 @@ def test_reference_evaluates_only_the_chosen_arm():
     big = [(0, 0, 2**40)]             # 2^40 * x leaves int64 for |x| >= 2^23
     case = cgm.Case([((1, "=", 1), big)], else_=cgm.Const(0))
     cols = [[2**30, 2**30], [0, 1]]
-    r = caseref.aggregate(cols, [None, None], [], [], [cgm.sum_(case)])
+    r = ref.aggregate(cols, [None, None], [], [], [cgm.sum_(case)])
     assert r.groups[()][0].overflow
-    r = caseref.aggregate([cols[0][:1], cols[1][:1]], [None, None], [], [], [cgm.sum_(case)])
+    r = ref.aggregate([cols[0][:1], cols[1][:1]], [None, None], [], [], [cgm.sum_(case)])
     assert not r.groups[()][0].overflow and r.groups[()][0].sum == 0
 
+
+
+def test_case_without_else_equals_a_filter():
+    """CASE WHEN p THEN e END (no ELSE) as the argument of count, sum, min, max and variance equals the aggregate of e
+    FILTER (WHERE p): a row whose p is FALSE or UNKNOWN is no input on both sides"""
+    import dataclasses
+    from citus_b200.columnar import Case
+    from test_agg_filter_host import FC, SCALES, random_language
+    from test_where_reference import random_tree
+    rng = np.random.default_rng(20261020)
+    for trial in range(120):
+        if trial % 40 == 0:
+            cols, nulls, atom, agg = random_language(rng)
+        where = random_tree(rng, atom, 3) if trial % 4 else []
+        cases, filters = [], []
+        for k in rng.integers(0, 5, 4):
+            kind = [ref.COUNT, ref.SUM, ref.MIN, ref.MAX, ref.VARIANCE][int(k)]
+            e, p = agg(kind), random_tree(rng, atom, 3)
+            cases.append(dataclasses.replace(e, factors=[], case=Case([(p, e.factors)])))
+            filters.append(dataclasses.replace(e, filter=p))
+        got = ref.aggregate(cols, nulls, where, [5], cases, FC, SCALES)
+        want = ref.aggregate(cols, nulls, where, [5], filters, FC, SCALES)
+        assert repr(got) == repr(want), (where, cases)
 
 # --------------------------------------------------------------------------- descriptor
 def test_make_desc_writes_the_arms(cg):

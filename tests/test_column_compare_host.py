@@ -1,6 +1,6 @@
 """Column-to-column atoms (column, op, Col(other)) on the host side, without a GPU: the descriptor make_desc builds, the
-checks of the comparison classes, chunk-group skipping and cg_relation_bounds against tests/column_compare_reference.py
-over random trees that mix column atoms with the other atoms, the generated kernels of every kind and form, and the
+checks of the comparison classes, chunk-group skipping and cg_relation_bounds against tests/reference.py
+over random trees that mix column atoms with the other atoms, column atoms against a precomputed 1 / 0 / NULL column, the generated kernels of every kind and form, and the
 generated source of query shapes without column atoms, which must stay byte for byte what it was."""
 import ctypes as C
 import hashlib
@@ -9,7 +9,6 @@ import math
 import numpy as np
 import pytest
 
-import column_compare_reference as cref
 import reference as ref
 from test_in_null_atoms_host import PINNED, compile_check, existing_shapes
 from test_variance_host import PARENT_SOURCE, existing_jit_shapes
@@ -91,7 +90,10 @@ def test_both_columns_count_toward_the_column_limit(cg):
 
 # --------------------------------------------------------------------------- reference rows
 def test_reference_row_semantics():
-    v = cref.atom_value
+    from citus_b200.columnar import Col
+
+    def v(op, x, x_null, y, y_null, is_float, sx=0, sy=0):
+        return ref.atom_value((0, op, Col(1)), [x, y], [x_null, y_null], (0, 1) if is_float else (), {0: sx, 1: sy})
     assert v("<", 1, False, 2, False, False) is True and v(">=", 1, False, 2, False, False) is False
     assert v("<", 1, True, 2, False, False) is None and v("<>", 1, False, 2, True, False) is None
     assert v("=", math.nan, False, math.nan, False, True) is True
@@ -101,6 +103,39 @@ def test_reference_row_semantics():
     assert v(">", INT64_MIN, False, INT64_MIN, False, False, 18, 0) is True           # INT64_MIN > INT64_MIN * 10^18
     assert v("=", 5, False, 500, False, False, 0, 2) is True                          # 5 = 5.00
 
+
+
+def test_column_atoms_equal_a_precomputed_column():
+    """a column atom answers as "v = 1" over a column v holding the atom's three-valued result per row (1 / 0 / NULL), in
+    WHERE, FILTER and bool_* arguments, integer-like sides at their numeric scales"""
+    import dataclasses
+    from test_agg_filter_host import FC, SCALES, map_atoms, random_language
+    rng = np.random.default_rng(20261018)
+    for trial in range(120):
+        if trial % 40 == 0:
+            cols, nulls, atom, agg = random_language(rng, forms=("const", "column", "column", "in"))
+            n = len(cols[0])
+            rows = [[float(c[r]) if i in FC else int(c[r]) for i, c in enumerate(cols)] for r in range(n)]
+            isnull = [[bool(z[r]) if z is not None else False for z in nulls] for r in range(n)]
+        virtual_cols, virtual_nulls, index = [], [], {}
+
+        def virtual(a):
+            if type(a[2] if len(a) > 2 else None).__name__ != "Col":
+                return a
+            if a not in index:
+                v = [ref.atom_value(a, rows[r], isnull[r], FC, SCALES) for r in range(n)]
+                index[a] = len(cols) + len(virtual_cols)
+                virtual_cols.append([int(bool(x)) for x in v])
+                virtual_nulls.append([x is None for x in v])
+            return (index[a], "=", 1)
+        where = random_tree(rng, atom, 4)
+        aggs = [agg(int(k), random_tree(rng, atom, 3) if rng.random() < 0.5 else None) for k in rng.integers(0, 10, 3)]
+        mapped = [dataclasses.replace(a, filter=map_atoms(a.filter, virtual), arg=map_atoms(a.arg, virtual)) for a in aggs]
+        mapped_where = map_atoms(where, virtual)
+        got = ref.aggregate(cols, nulls, where, [5], aggs, FC, SCALES)
+        want = ref.aggregate(list(cols) + virtual_cols, list(nulls) + virtual_nulls, mapped_where, [5], mapped, FC, SCALES)
+        assert repr(got) == repr(want), where
+        assert index or trial % 40
 
 # --------------------------------------------------------------------------- chunk-group skipping and bounds
 def test_selected_chunk_mask_and_relation_bounds_against_reference(cg):
@@ -142,7 +177,7 @@ def test_selected_chunk_mask_and_relation_bounds_against_reference(cg):
         except capi.CitusGpuError as e:
             assert e.code == capi.CG_EUNSUPPORTED
             continue
-        want = cref.selected_chunk_mask(cols, nulls, where, stripe_rows, chunk_rows, float_cols=fc, minmax=minmax)
+        want = ref.selected_chunk_mask(cols, nulls, where, stripe_rows, chunk_rows, float_cols=fc, minmax=minmax)
         got = library_mask(cg, rel, d)
         assert got == want, f"seed {seed} where {where}"
         refuted += ref.chunks_filtered(want)
@@ -152,7 +187,7 @@ def test_selected_chunk_mask_and_relation_bounds_against_reference(cg):
     # an AND with a refuting arm is refuted, an OR with a column-atom arm is not
     m = [library_mask(cg, rel, cg.make_desc(t, [], [cg.count_star()])) for t in trees[:3]]
     assert all(all(s) for s in m[0])
-    want_and = cref.selected_chunk_mask(cols, nulls, trees[1], stripe_rows, chunk_rows, float_cols=fc, minmax=minmax)
+    want_and = ref.selected_chunk_mask(cols, nulls, trees[1], stripe_rows, chunk_rows, float_cols=fc, minmax=minmax)
     assert m[1] == want_and
     assert all(all(s) for s in m[2])
     # and the plain constant atom alone refutes what the AND refutes

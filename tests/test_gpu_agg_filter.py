@@ -1,6 +1,6 @@
-"""Aggregate FILTER (WHERE ...) in the fused scan against the exact reference, on every kernel family.  The expected
-answers are composed from tests/reference.py: the groups come from WHERE alone, aggregate j of a group is the reference
-aggregate over (WHERE AND FILTER_j), and a group without such rows has count 0 / SQL NULL."""
+"""Aggregate FILTER (WHERE ...) in the fused scan against the exact reference (tests/reference.py), on every kernel
+family: the groups come from WHERE alone, a row its FILTER does not find TRUE is no input of that aggregate, and a group
+without such rows has count 0 / SQL NULL."""
 import dataclasses
 import math
 
@@ -8,42 +8,20 @@ import numpy as np
 import pytest
 
 import reference as ref
-from test_agg_filter_host import filtered_reference
 from test_gpu_exact import NEG_NAN, assert_matches_reference, gpu_run
 from test_where_reference import constant_pools, random_tree
+from gpu_harness import cg, kernel_family, FAMILIES  # noqa: F401  (fixtures)
 
 pytestmark = pytest.mark.gpu
 
-FAMILIES = ["jit", "jit_always", "aot", "general"]
 OPS = ("<", "<=", "=", ">=", ">", "<>")
 SHAPES = [dict(group_cols=[]), dict(group_cols=[0]), dict(group_cols=[0, 1]), dict(group_cols=[2], expected_groups=4096, force_hash=True)]
 
 
-@pytest.fixture(scope="module")
-def cg():
-    import torch
-    assert torch.cuda.is_available(), "these tests need an H100"
-    from citus_b200 import build
-    build.build()
-    from citus_b200 import columnar
-    columnar.init(0)
-    return columnar
-
-
-@pytest.fixture
-def kernel_family(cg):
-    def use(name):
-        cg.set_option("jit", {"jit": 1, "jit_always": 2, "aot": 0, "general": 0}[name])
-        cg.set_option("force_general", 1 if name == "general" else 0)
-    yield use
-    cg.set_option("jit", 1)
-    cg.set_option("force_general", 0)
-
-
 def check(cg, rel, cols, nulls, where, group_cols, aggs, n, float_cols=(), **kw):
-    """the scan equals the composed reference; the WHERE counters equal those of the same query without filters"""
+    """the scan equals the reference; the WHERE counters equal those of the same query without filters"""
     from citus_b200 import capi
-    want = filtered_reference(cols, nulls, where, group_cols, aggs, float_cols)
+    want = ref.aggregate(cols, nulls, where, group_cols, aggs, float_cols)
     if ref.overflows(want):
         with pytest.raises(capi.CitusGpuError) as e:
             gpu_run(cg, rel, where, group_cols, aggs, float_cols=float_cols, **kw)
@@ -164,7 +142,7 @@ def test_argument_errors_only_on_accepted_rows(cg, kernel_family, family):
         # bound 1000: only the rows the filter rejects break it
         agg = [cg.sum_(1, filter=("and", (1, ">=", -1000), (1, "<=", 1000))), cg.count_star()]
         st, got, _ = gpu_run(cg, rel, [], group, agg, bounds=[1000, 0], force_hash=hash_, expected_groups=16)
-        assert_matches_reference(st, got, filtered_reference(cols, None, [], group, agg), agg, n)
+        assert_matches_reference(st, got, ref.aggregate(cols, None, [], group, agg), agg, n)
         with pytest.raises(capi.CitusGpuError) as e:
             gpu_run(cg, rel, [], group, [cg.sum_(1, filter=(1, ">", -5000)), cg.count_star()], bounds=[1000, 0], force_hash=hash_,
                     expected_groups=16)
@@ -204,7 +182,7 @@ def test_filter_only_column_is_staged(cg, kernel_family, family):
     for dma in (False, True):
         for group in ([], [0]):
             st, got = scan_relation(cg, rel, where, group, aggs, dma)
-            assert_matches_reference(st, got, filtered_reference(cols, None, where, group, aggs), aggs, n)
+            assert_matches_reference(st, got, ref.aggregate(cols, None, where, group, aggs), aggs, n)
             st2, _ = scan_relation(cg, rel, where, group, same_cols, dma)
             assert st.h2d_bytes == st2.h2d_bytes and st.h2d_bytes > 0
             assert (st.chunk_groups_filtered, st.rows_removed_by_filter, st.rows_scanned) == \
@@ -234,7 +212,7 @@ def test_q1_shape_with_filters_packing_on_and_off(cg, oracle, kernel_family, fam
     rel = cg.Relation.from_image(tab.pages(), tab.stripes_array(), tab.nodes_array(), [-1] * 6 + [4], [NUM2] * 4 + [3, 3, 0])
     aggs = [cg.sum_(0), cg.sum_(1), cg.Agg(2, [(1, 0, 1), (2, 100, -1)]), cg.count_star(),
             cg.count_star(filter=(2, ">", 5)), cg.sum_(1, filter=(6, ">=", -1000)), cg.sum_(0, filter=("or", (4, "=", 65), (3, "<", 3)))]
-    want = filtered_reference(cols, None, [(6, "<=", 1500)], [4, 5], aggs)
+    want = ref.aggregate(cols, None, [(6, "<=", 1500)], [4, 5], aggs)
     for packing in (True, False):
         a = [dataclasses.replace(x) for x in aggs]
         dsc = cg.make_desc([(6, "<=", 1500)], [4, 5], a, expected_groups=16)
@@ -271,7 +249,7 @@ def test_export_merge_and_fetch_merge_values_round_trips(cg):
               cg.count(1, filter=(2, ">", 0.0)), cg.count_star()],
              [cg.count_star(filter=(0, "<", 3)), cg.sum_(1, filter=(0, ">=", 3))]]
     for aggs in lists:
-        want = filtered_reference(cols, None, [], [0], aggs, (2,))
+        want = ref.aggregate(cols, None, [], [0], aggs, (2,))
         for force_hash in (False, True):
             d = cg.make_desc([], [0], aggs, float_cols=(2,), expected_groups=16)
             kmin, kmax = (0, 5) if not force_hash else (0, -1)

@@ -1,6 +1,6 @@
 """bit_and / bit_or / bool_and / bool_or (every) in the fused scan against the exact reference, on every kernel family.
-The expected answers come from tests/bool_bit_reference.py (built on tests/reference.py), FILTER by composition:
-groups come from WHERE alone, aggregate j is the reference aggregate over (WHERE AND FILTER_j).  bool_and / bool_or
+The expected answers come from tests/reference.py: groups come from WHERE alone, and a row its FILTER does not find
+TRUE is no input of that aggregate.  bool_and / bool_or
 evaluate their predicate under three-valued logic (an UNKNOWN row is no input); every value is compared exactly."""
 import dataclasses
 import math
@@ -11,39 +11,17 @@ import traceback
 import numpy as np
 import pytest
 
-import bool_bit_reference as bref
 import reference as ref
 from test_bool_bit_agg_host import bool_agg_case
 from test_gpu_agg_filter import mixed_relation, scan_relation
 from test_gpu_exact import gpu_run
 from test_where_reference import constant_pools, random_tree
+from gpu_harness import cg, kernel_family, FAMILIES  # noqa: F401  (fixtures)
 
 pytestmark = pytest.mark.gpu
 
-FAMILIES = ["jit", "jit_always", "aot", "general"]
 OPS = ("<", "<=", "=", ">=", ">", "<>")
 SHAPES = [dict(group_cols=[]), dict(group_cols=[0]), dict(group_cols=[0, 1]), dict(group_cols=[2], expected_groups=4096, force_hash=True)]
-
-
-@pytest.fixture(scope="module")
-def cg():
-    import torch
-    assert torch.cuda.is_available(), "these tests need an H100"
-    from citus_b200 import build
-    build.build()
-    from citus_b200 import columnar
-    columnar.init(0)
-    return columnar
-
-
-@pytest.fixture
-def kernel_family(cg):
-    def use(name):
-        cg.set_option("jit", {"jit": 1, "jit_always": 2, "aot": 0, "general": 0}[name])
-        cg.set_option("force_general", 1 if name == "general" else 0)
-    yield use
-    cg.set_option("jit", 1)
-    cg.set_option("force_general", 0)
 
 
 def assert_exact(st, got, want, aggs, nrows):
@@ -77,8 +55,8 @@ def assert_exact(st, got, want, aggs, nrows):
 
 
 def check(cg, rel, cols, nulls, where, group_cols, aggs, n, float_cols=(), **kw):
-    """the scan equals the composed reference; the WHERE counters equal those of the count(*)-only query"""
-    want = bref.filtered(cols, nulls, where, group_cols, aggs, float_cols)
+    """the scan equals the reference; the WHERE counters equal those of the count(*)-only query"""
+    want = ref.aggregate(cols, nulls, where, group_cols, aggs, float_cols)
     st, got, layout = gpu_run(cg, rel, where, group_cols, aggs, float_cols=float_cols, **kw)
     assert_exact(st, got, want, aggs, n)
     st0, _, _ = gpu_run(cg, rel, where, group_cols, [cg.count_star()], float_cols=float_cols, **kw)
@@ -263,7 +241,7 @@ def test_count_bounded_sum_and_bit_or_packing_on_and_off(cg, kernel_family, fami
     cols = [rng.integers(0, 3000, n), rng.integers(0, 100, n), rng.integers(-10**6, 10**6, n)]
     rel = cg.Relation.write([8, 8, 8], cols, chunk_row_limit=5000)
     aggs = [cg.sum_(2), cg.count_star(), cg.bit_or(2)]
-    want = bref.aggregate(cols, None, [(1, "<", 50)], [0], aggs)
+    want = ref.aggregate(cols, None, [(1, "<", 50)], [0], aggs)
     d = cg.make_desc([(1, "<", 50)], [0], aggs)
     kmin, kmax, bounds, rows = cg.relation_bounds(rel, d)
     a2 = [dataclasses.replace(a, term_abs_bound=b) for a, b in zip(aggs, bounds)]
@@ -290,13 +268,13 @@ def test_argument_only_columns_through_every_staging_path(cg, kernel_family, fam
     rel = cg.Relation.write([8, 8, 8, 8], cols, chunk_row_limit=5000)
     where = [(1, "<", 400_000)]
     aggs = [cg.count_star(), cg.bool_or((2, ">", 45)), cg.bool_and((3, ">", 1000)), cg.bit_or(1)]
-    want = bref.filtered(cols, None, where, [0], aggs)
+    want = ref.aggregate(cols, None, where, [0], aggs)
     st, got, _ = gpu_run(cg, rel, where, [0], aggs)
     assert_exact(st, got, want, aggs, n)
     for dma in (False, True):
         for group in ([], [0]):
             st, got = scan_relation(cg, rel, where, group, aggs, dma)
-            assert_exact(st, got, bref.filtered(cols, None, where, group, aggs), aggs, n)
+            assert_exact(st, got, ref.aggregate(cols, None, where, group, aggs), aggs, n)
             assert st.h2d_bytes > 0 and st.chunk_groups_filtered > 0
 
 
@@ -318,7 +296,7 @@ def test_layout_export_merge_and_fetch_merge_values_round_trips(cg):
     rels = [cg.Relation.write([8, 8, 8], [c[h] for c in cols], [None, z[h], None], type_classes=[0, 0, 1]) for h in halves]
     aggs = [cg.bit_and(1), cg.bit_or(1, filter=(0, "<", 4)), cg.bool_and((1, ">", -9 * 10**11)), cg.bool_or(("and", (2, ">", 2.0), (1, "<", 0))),
             cg.count_star(), cg.bool_or((1, ">", 0), filter=(0, "=", 5))]
-    want = bref.filtered(cols, nulls, [], [0], aggs, (2,))
+    want = ref.aggregate(cols, nulls, [], [0], aggs, (2,))
     for force_hash in (False, True):
         d = cg.make_desc([], [0], aggs, float_cols=(2,), expected_groups=16)
         kmin, kmax = (0, 5) if not force_hash else (0, -1)
@@ -375,7 +353,7 @@ def _combine_worker(rank, world, port, out):
         halves = [slice(0, n // 2), slice(n // 2, n)]
         rel = cg.Relation.write([8, 8, 8], [c[halves[rank]] for c in cols], chunk_row_limit=5000)
         aggs = [cg.count_star(), cg.bit_and(1), cg.bit_or(1), cg.bool_and((2, "<", 98)), cg.bool_or((1, ">", 999_000_000))]
-        want = bref.filtered(cols, None, [], [0], aggs)
+        want = ref.aggregate(cols, None, [], [0], aggs)
         for mode in (1, 0):
             cg.set_option("peer_window", mode)
             for kmin, kmax in ((0, 1999), (0, -1)):

@@ -1,4 +1,4 @@
-"""CASE aggregate arguments in the fused scan and the join aggregate, exact against tests/case_agg_reference.py on every
+"""CASE aggregate arguments in the fused scan and the join aggregate, exact against tests/reference.py on every
 kernel family: random CASE trees with NULLs in WHEN and THEN columns, every ELSE form, groups where every row chose NULL
 next to groups that chose ELSE 0, overflow and bound violations in chosen and unchosen arms, CASE with FILTER, every table
 kind with packing on and off, the three staging paths, float sums, min and max with NaN, variance, an export / merge /
@@ -11,16 +11,12 @@ import os
 import numpy as np
 import pytest
 
-import case_agg_reference as caseref
 import join_agg_reference as jref
 import reference as ref
-import variance_reference as vref
-from test_gpu_agg_filter import cg, kernel_family  # noqa: F401  (fixtures)
 from test_gpu_exact import NEG_NAN
+from gpu_harness import cg, kernel_family, FAMILIES  # noqa: F401  (fixtures)
 
 pytestmark = pytest.mark.gpu
-
-FAMILIES = ["jit", "jit_always", "aot", "general"]
 
 
 def run(cg, rel, where, group_cols, aggs, float_cols=(), use_bounds=True, force_hash=False, e2e=False, packing=True,
@@ -87,7 +83,7 @@ def assert_exact(st, got, want, aggs, nrows):
 
 def check(cg, rel, cols, nulls, where, group_cols, aggs, n, float_cols=(), **kw):
     from citus_b200 import capi
-    want = caseref.aggregate(cols, nulls, where, group_cols, aggs, float_cols)
+    want = ref.aggregate(cols, nulls, where, group_cols, aggs, float_cols)
     if ref.overflows(want):
         with pytest.raises(capi.CitusGpuError) as e:
             run(cg, rel, where, group_cols, aggs, float_cols=float_cols, **kw)
@@ -286,11 +282,11 @@ def test_variance_over_case_to_exact_text(cg, kernel_family, family):
     aggs = [cg.variance(case)]
     for use_bounds in (True, False):
         got = check(cg, rel, cols, nulls, [], [0], aggs, n, use_bounds=use_bounds)
-        want = caseref.aggregate(cols, nulls, [], [0], aggs)
+        want = ref.aggregate(cols, nulls, [], [0], aggs)
         for key, per in want.groups.items():
             w, gg = per[0], got[key][0]
             for final in (capi.CG_VAR_POP, capi.CG_VAR_SAMP, capi.CG_STDDEV_POP, capi.CG_STDDEV_SAMP):
-                assert cg.numeric_var_out(final, gg["count"], gg["sum"], gg["sumsq"], 0) == vref.var_out(final, w.count, w.sum, w.sumsq, 0), \
+                assert cg.numeric_var_out(final, gg["count"], gg["sum"], gg["sumsq"], 0) == ref.var_out(final, w.count, w.sum, w.sumsq, 0), \
                     (key, final)
 
 
@@ -322,7 +318,7 @@ def test_export_merge_fetch_round_trip(cg):
         a.free()
         b.free()
     # b holds its own scan plus a's exported rows: counts and sums twice, min and max once
-    want = caseref.aggregate(cols, nulls, [], [0], aggs, float_cols=(6,))
+    want = ref.aggregate(cols, nulls, [], [0], aggs, float_cols=(6,))
     for (key,), (s, c, lo, hi) in want.groups.items():
         g = got[key]
         assert [g[j]["count"] for j in range(4)] == [2 * s.count, 2 * c.count, 2 * lo.count, 2 * hi.count]
@@ -350,7 +346,7 @@ def test_join_aggregate_arms_mix_build_and_probe(cg, mode):
     aggs = [cg.sum_(case), cg.count(case), cg.min_(case, filter=(4, "<>", 0)), cg.max_(case), cg.variance(case)]
     group = [] if mode == "plain" else [4]
     where = [(3, ">", -40)]
-    want = caseref.aggregate(jcols, jnulls, where, group, aggs)
+    want = ref.aggregate(jcols, jnulls, where, group, aggs)
     d = cg.make_desc(where, group, aggs, expected_groups=16 if mode == "hash" else 0)
     colspec = [(8, 0)] * 5
     kmin, kmax = (0, 4) if mode == "dense" else (0, -1)

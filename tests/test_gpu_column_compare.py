@@ -1,5 +1,5 @@
 """Column-to-column atoms (column, op, Col(other)) in the fused scan against the exact reference
-(tests/column_compare_reference.py), on every kernel family: groups and aggregates, rows scanned, rows removed by the
+(tests/reference.py), on every kernel family: groups and aggregates, rows scanned, rows removed by the
 filter and chunk groups removed by the filter, in WHERE, in FILTERs and in bool_and / bool_or arguments, over every
 same-class pair of column types, NULLs on either side, NaN / +-0.0 / +-inf, numeric scale alignment beyond 64 bits, and
 the TPC-H Q12 predicates over the lineitem fixture."""
@@ -10,12 +10,12 @@ import math
 import numpy as np
 import pytest
 
-import column_compare_reference as cref
 import reference as ref
 from test_gpu_agg_filter import mixed_relation
 from test_gpu_bool_bit_agg import assert_exact
-from test_gpu_in_null_atoms import FAMILIES, OPS, keyed, small_tree, typed_relation
+from test_gpu_in_null_atoms import OPS, keyed, small_tree, typed_relation
 from test_where_reference import constant_pools
+from gpu_harness import cg, kernel_family, FAMILIES  # noqa: F401  (fixtures)
 
 pytestmark = pytest.mark.gpu
 
@@ -25,27 +25,6 @@ BPCHAR1 = 3
 
 def NUMERIC(s):
     return 2 | (s << 8)
-
-
-@pytest.fixture(scope="module")
-def cg():
-    import torch
-    assert torch.cuda.is_available(), "these tests need an H100"
-    from citus_b200 import build
-    build.build()
-    from citus_b200 import columnar
-    columnar.init(0)
-    return columnar
-
-
-@pytest.fixture
-def kernel_family(cg):
-    def use(name):
-        cg.set_option("jit", {"jit": 1, "jit_always": 2, "aot": 0, "general": 0}[name])
-        cg.set_option("force_general", 1 if name == "general" else 0)
-    yield use
-    cg.set_option("jit", 1)
-    cg.set_option("force_general", 0)
 
 
 def run(cg, rel, where, group, aggs, float_cols=(), stage="shard", expected_groups=0, force_hash=False, packing=True):
@@ -88,8 +67,8 @@ def check(cg, rel, cols, nulls, where, group, aggs, stripe_rows, chunk_rows, flo
     n = len(cols[0])
     ck = (key, repr(where), tuple(group), repr(aggs))
     if key is None or ck not in _WANT:
-        want = cref.aggregate(cols, nulls, where, group, aggs, float_cols, scales)
-        mask = cref.selected_chunk_mask(cols, nulls, where, stripe_rows, chunk_rows, float_cols=float_cols)
+        want = ref.aggregate(cols, nulls, where, group, aggs, float_cols, scales)
+        mask = ref.selected_chunk_mask(cols, nulls, where, stripe_rows, chunk_rows, float_cols=float_cols)
         _WANT[ck] = (want, mask)
     want, mask = _WANT[ck]
     st, got = run(cg, rel, where, group, aggs, float_cols, **kw)

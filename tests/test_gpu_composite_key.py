@@ -1,7 +1,7 @@
 """Composite GROUP BY keys (CgScanDesc.composite_key) in the fused scan against the exact reference, on every kernel
 family: one to four key columns of every integer-like type (bool, int1, int2, int4, int8, char(1), numeric(12, 2)),
 negative values and NULLs in every key column, in the small-domain, direct-indexed and hash table kinds.  The expected
-answers come from tests/bool_bit_reference.py (reference.py plus FILTER by composition), whose groups are keyed by the
+answers come from tests/reference.py, whose groups are keyed by the
 tuple of key values with None for NULL -- the shape GpuColumnarAgg.groups() decodes composite codes into."""
 import ctypes
 import dataclasses
@@ -12,12 +12,12 @@ import traceback
 import numpy as np
 import pytest
 
-import bool_bit_reference as bref
+import reference as ref
 from test_gpu_bool_bit_agg import assert_exact
+from gpu_harness import cg, kernel_family, FAMILIES  # noqa: F401  (fixtures)
 
 pytestmark = pytest.mark.gpu
 
-FAMILIES = ["jit", "jit_always", "aot", "general"]
 BPCHAR1, NUMERIC2 = 3, 2 | (2 << 8)
 ATTLENS = [1, 1, 2, 4, 8, -1, -1, 8, 8]
 TYPES = [0, 0, 0, 0, 0, BPCHAR1, NUMERIC2, 0, 1]
@@ -25,27 +25,6 @@ FLOAT_COLS = (8,)
 # key columns -> the table kind they give with the aggregates below
 GROUPINGS = [([0, 1], "small"), ([2, 3], "dense"), ([5, 0], "dense"), ([1, 2, 3], "dense"), ([4, 3], "hash"), ([6], "hash"),
              ([0, 5, 6, 2], "hash")]
-
-
-@pytest.fixture(scope="module")
-def cg():
-    import torch
-    assert torch.cuda.is_available(), "these tests need an H100"
-    from citus_b200 import build
-    build.build()
-    from citus_b200 import columnar
-    columnar.init(0)
-    return columnar
-
-
-@pytest.fixture
-def kernel_family(cg):
-    def use(name):
-        cg.set_option("jit", {"jit": 1, "jit_always": 2, "aot": 0, "general": 0}[name])
-        cg.set_option("force_general", 1 if name == "general" else 0)
-    yield use
-    cg.set_option("jit", 1)
-    cg.set_option("force_general", 0)
 
 
 def make_rows(seed, n):
@@ -89,7 +68,7 @@ _REFERENCE = {}
 def reference(cols, nulls, where, group, aggs, key):
     k = (key, repr(where), tuple(group), repr(aggs))
     if k not in _REFERENCE:
-        _REFERENCE[k] = bref.filtered(cols, nulls, where, group, aggs, FLOAT_COLS)
+        _REFERENCE[k] = ref.aggregate(cols, nulls, where, group, aggs, FLOAT_COLS)
     return _REFERENCE[k]
 
 
@@ -227,7 +206,7 @@ def test_shards_fold_into_one_partial_under_union_bounds(cg, oracle, kernel_fami
                 assert e.value.code == capi.CG_EINVAL
         finally:
             agg.free()
-        want = bref.filtered(cols, nulls, [], group, aggs, FLOAT_COLS)
+        want = ref.aggregate(cols, nulls, [], group, aggs, FLOAT_COLS)
         assert set(got) == set(want.groups)
         for key, per in want.groups.items():
             assert [g["count"] for g in got[key]] == [w.count for w in per], (group, key)
@@ -328,7 +307,7 @@ def _worker(rank, world, port, out):
                 agg.scan_shard(cg.Shard(rel), want_stats=False)
                 cgd.combine_partials(agg, dst=0)
                 if rank == 0:
-                    want = bref.filtered(cols, nulls, [], group, aggs, FLOAT_COLS)
+                    want = ref.aggregate(cols, nulls, [], group, aggs, FLOAT_COLS)
                     got = agg.groups()
                     assert set(got) == set(want.groups), (pw, group)
                     for key, per in want.groups.items():
@@ -409,7 +388,7 @@ def test_packing_engages_and_its_overflow_is_detected(cg, kind):
         got = agg.groups()
     finally:
         agg.free()
-    want = bref.aggregate([k0, k1, v], None, [], [0, 1], aggs)
+    want = ref.aggregate([k0, k1, v], None, [], [0, 1], aggs)
     assert set(got) == set(want.groups)
     for key, per in want.groups.items():
         assert (got[key][0]["sum"], got[key][1]["count"]) == (per[0].sum, per[1].count), key

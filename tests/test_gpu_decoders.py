@@ -9,21 +9,11 @@ import numpy as np
 import pytest
 
 import decoder_corpus as dc
+from gpu_harness import cg  # noqa: F401  (fixtures)
 
 pytestmark = pytest.mark.gpu
 
 NUM2 = 2 | (2 << 8)          # numeric(p, 2)
-
-
-@pytest.fixture(scope="module")
-def cg():
-    import torch
-    assert torch.cuda.is_available(), "these tests need an H100"
-    from citus_b200 import build
-    build.build()
-    from citus_b200 import columnar
-    columnar.init(0)
-    return columnar
 
 
 # decoder form -> cg_set_option values

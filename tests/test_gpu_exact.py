@@ -12,33 +12,12 @@ import numpy as np
 import pytest
 
 import reference as ref
+from gpu_harness import cg, kernel_family, FAMILIES  # noqa: F401  (fixtures)
 
 pytestmark = pytest.mark.gpu
 
-FAMILIES = ["jit", "jit_always", "aot", "general"]
 NEG_NAN = struct.unpack("<d", struct.pack("<Q", 0xFFF8000000000000))[0]
 INT64_MIN, INT64_MAX = -2**63, 2**63 - 1
-
-
-@pytest.fixture(scope="module")
-def cg():
-    import torch
-    assert torch.cuda.is_available(), "these tests need an H100"
-    from citus_b200 import build
-    build.build()
-    from citus_b200 import columnar
-    columnar.init(0)
-    return columnar
-
-
-@pytest.fixture
-def kernel_family(cg):
-    def use(name):
-        cg.set_option("jit", {"jit": 1, "jit_always": 2, "aot": 0, "general": 0}[name])
-        cg.set_option("force_general", 1 if name == "general" else 0)
-    yield use
-    cg.set_option("jit", 1)
-    cg.set_option("force_general", 0)
 
 
 def gpu_run(cg, rel, where, group_cols, aggs, float_cols=(), use_bounds=True, force_hash=False, e2e=False,

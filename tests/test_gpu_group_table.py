@@ -15,10 +15,10 @@ import numpy as np
 import pytest
 
 import group_table_reference as gt
+from gpu_harness import kernel_family, FAMILIES  # noqa: F401  (fixtures)
 
 pytestmark = pytest.mark.gpu
 
-FAMILIES = ["jit", "jit_always", "aot", "general"]
 DENSE, HASH = "dense", "hash"
 I64_MIN, I64_MAX = gt.I64_MIN, gt.I64_MAX
 I32_MIN, I32_MAX = -(1 << 31), (1 << 31) - 1
@@ -42,16 +42,6 @@ def cg():
         shard.free()
     for cache in (_RELS, _SHIFT_RELS, _BOUNDARY_RELS, _EXPECT, _LIFE, _CAP, _LIMIT_RELS):
         cache.clear()
-
-
-@pytest.fixture
-def kernel_family(cg):
-    def use(name):
-        cg.set_option("jit", {"jit": 1, "jit_always": 2, "aot": 0, "general": 0}[name])
-        cg.set_option("force_general", 1 if name == "general" else 0)
-    yield use
-    cg.set_option("jit", 1)
-    cg.set_option("force_general", 0)
 
 
 def capi():

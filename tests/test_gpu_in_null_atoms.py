@@ -1,4 +1,4 @@
-"""IN / NOT IN lists and IS [NOT] NULL atoms in the fused scan against the exact reference (tests/in_null_reference.py), on
+"""IN / NOT IN lists and IS [NOT] NULL atoms in the fused scan against the exact reference (tests/reference.py), on
 every kernel family: groups and aggregates, rows scanned, rows removed by the filter and chunk groups removed by the
 filter, in WHERE, in FILTERs and in bool_and / bool_or arguments, over every column type the atoms take."""
 import dataclasses
@@ -6,39 +6,17 @@ import dataclasses
 import numpy as np
 import pytest
 
-import in_null_reference as iref
 import reference as ref
 from test_gpu_agg_filter import mixed_relation
 from test_gpu_bool_bit_agg import assert_exact
 from test_gpu_composite_key import ATTLENS, TYPES, table
 from test_where_reference import constant_pools
+from gpu_harness import cg, kernel_family, FAMILIES  # noqa: F401  (fixtures)
 
 pytestmark = pytest.mark.gpu
 
-FAMILIES = ["jit", "jit_always", "aot", "general"]
 OPS = ("<", "<=", "=", ">=", ">", "<>")
 INT64_MIN, INT64_MAX = -2**63, 2**63 - 1
-
-
-@pytest.fixture(scope="module")
-def cg():
-    import torch
-    assert torch.cuda.is_available(), "these tests need an H100"
-    from citus_b200 import build
-    build.build()
-    from citus_b200 import columnar
-    columnar.init(0)
-    return columnar
-
-
-@pytest.fixture
-def kernel_family(cg):
-    def use(name):
-        cg.set_option("jit", {"jit": 1, "jit_always": 2, "aot": 0, "general": 0}[name])
-        cg.set_option("force_general", 1 if name == "general" else 0)
-    yield use
-    cg.set_option("jit", 1)
-    cg.set_option("force_general", 0)
 
 
 def keyed(groups, group_cols):
@@ -93,8 +71,8 @@ def check(cg, rel, cols, nulls, where, group, aggs, stripe_rows, chunk_rows, flo
     n = len(cols[0])
     ck = (key, repr(where), tuple(group), repr(aggs))
     if key is None or ck not in _WANT:
-        want = iref.aggregate(cols, nulls, where, group, aggs, float_cols)
-        mask = iref.selected_chunk_mask(cols, nulls, where, stripe_rows, chunk_rows, float_cols=float_cols)
+        want = ref.aggregate(cols, nulls, where, group, aggs, float_cols)
+        mask = ref.selected_chunk_mask(cols, nulls, where, stripe_rows, chunk_rows, float_cols=float_cols)
         _WANT[ck] = (want, mask)
     want, mask = _WANT[ck]
     st, got = run(cg, rel, where, group, aggs, float_cols, **kw)
@@ -326,7 +304,7 @@ def test_back_to_back_asynchronous_scans_with_different_lists(cg, kernel_family)
         sh.free()
     # each list alone against the reference
     for where in wheres:
-        want1 = iref.aggregate(cols, None, where, [0], aggs)
+        want1 = ref.aggregate(cols, None, where, [0], aggs)
         p = partial_for(where)
         for rel in rels:
             p.scan_relation(rel)

@@ -1,6 +1,5 @@
 """cg_join_aggregate against the exact references: the numpy equi-join of tests/join_agg_reference.py, aggregated by
-tests/column_compare_reference.py (WHERE trees, IN lists, IS NULL, column atoms, FILTER, bit_* / bool_*) and
-tests/variance_reference.py.  Covered: the plain aggregate against cg_join_count_sum on a C4-shaped input with a
+tests/reference.py (WHERE trees, IN lists, IS NULL, column atoms, FILTER, bit_* / bool_*, variance).  Covered: the plain aggregate against cg_join_count_sum on a C4-shaped input with a
 3000 x 3000 key, INT64_MIN and NULL keys; every group key form on dense and hash tables; every aggregate kind; WHERE
 trees with a cross-side column atom; accumulation over two calls and an export / merge round trip; the one-GPU
 repartition exchange followed by one call per partition; the refusals."""
@@ -10,12 +9,11 @@ import types
 import numpy as np
 import pytest
 
-import column_compare_reference as cref
 import join_agg_reference as jref
 import partition_reference as pr
 import reference as ref
-import variance_reference as vref
 from test_gpu_bool_bit_agg import assert_exact
+from gpu_harness import cg  # noqa: F401  (fixtures)
 
 pytestmark = pytest.mark.gpu
 
@@ -32,17 +30,6 @@ COLS = [(8, INT), (8, INT), (4, INT), (-1, NUMERIC(2)), (8, FLOAT),
         (8, INT), (8, INT), (4, INT), (-1, NUMERIC(3)), (8, FLOAT)]
 FLOATS = (4, 9)
 SCALES = {3: 2, 8: 3}
-
-
-@pytest.fixture(scope="module")
-def cg():
-    import torch
-    assert torch.cuda.is_available(), "these tests need an H100"
-    from citus_b200 import build
-    build.build()
-    from citus_b200 import columnar
-    columnar.init(0)
-    return columnar
 
 
 def _dev(a, dtype=np.int64):
@@ -116,7 +103,7 @@ def run(cg, b, p, where, group, aggs, kmin=0, kmax=-1, composite=False, key_boun
 
 def check(cg, b, p, where, group, aggs, **kw):
     jc, jn = joined(b, p)
-    want = cref.aggregate(jc, jn, where, group, aggs, FLOATS, SCALES)
+    want = ref.aggregate(jc, jn, where, group, aggs, FLOATS, SCALES)
     agg, st = run(cg, b, p, where, group, aggs, **kw)
     try:
         got = keyed(agg.groups(), group, kw.get("composite", False))
@@ -237,7 +224,7 @@ def test_var_samp_over_numeric(cg, sides, group):
     b, p = sides
     aggs = [cg.count_star(), cg.variance(3), cg.variance(1, filter=(6, ">", 0))]
     jc, jn = joined(b, p)
-    want = vref.filtered(jc, jn, [], group, aggs, FLOATS)
+    want = ref.aggregate(jc, jn, [], group, aggs, FLOATS)
     agg, st = run(cg, b, p, [], group, aggs, **(dict(kmin=0, kmax=49) if group else {}))
     try:
         got = keyed(agg.groups(), group, False)
@@ -250,7 +237,7 @@ def test_var_samp_over_numeric(cg, sides, group):
             assert (g["count"], g["sum"], g["sumsq"]) == (w.count, w.sum, w.sumsq), (key, a)
             if w.count > 1:
                 assert cg.numeric_var_out(1, g["count"], g["sum"], g["sumsq"], 2 if a == 1 else 0) == \
-                    vref.var_out(1, w.count, w.sum, w.sumsq, 2 if a == 1 else 0)
+                    ref.var_out(1, w.count, w.sum, w.sumsq, 2 if a == 1 else 0)
 
 
 # --------------------------------------------------------------------------- 4. WHERE trees
@@ -283,7 +270,7 @@ def test_two_calls_and_export_merge(cg):
     j1, j2 = joined(b1, p1), joined(b2, p2)
     jc = [np.concatenate([a, c]) for a, c in zip(j1[0], j2[0])]
     jn = [None if a is None else np.concatenate([a, c]) for a, c in zip(j1[1], j2[1])]
-    want = cref.aggregate(jc, jn, [], group, aggs, FLOATS, SCALES)
+    want = ref.aggregate(jc, jn, [], group, aggs, FLOATS, SCALES)
     agg, st1 = run(cg, b1, p1, [], group, aggs, expected_groups=64)
     other = None
     try:
@@ -368,7 +355,7 @@ def test_exchange_then_join_aggregate(cg, comm):
     finally:
         agg.free()
     jc, jn = jref.join([bk, bx, bg], None, 0, [pk, py, ph], None, 0)
-    want = cref.aggregate(jc, jn, where, [2], aggs)
+    want = ref.aggregate(jc, jn, where, [2], aggs)
     assert set(got) == set(want.groups)
     for key, per in want.groups.items():
         for a, w in enumerate(per):
@@ -413,7 +400,7 @@ def test_refusals_leave_the_partial_untouched(cg, sides):
             agg.desc = other
         # nothing of the above reached the partial: one valid call gives the reference
         jc, jn = joined(b, p)
-        want = cref.aggregate(jc, jn, [], group, aggs, FLOATS, SCALES)
+        want = ref.aggregate(jc, jn, [], group, aggs, FLOATS, SCALES)
         st = agg.join_aggregate(b.ptrs(), 0, b.n, p.ptrs(), 0, p.n, b.null_ptrs(), p.null_ptrs())
         assert_exact(st, keyed(agg.groups(), group, False), want, aggs, len(jc[0]))
         # an empty side is a no-op

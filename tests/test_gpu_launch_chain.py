@@ -9,25 +9,15 @@ import dataclasses
 import numpy as np
 import pytest
 
-import in_null_reference as iref
+import reference as ref
 from test_gpu_scan import assert_same_groups, oracle_table, to_oracle_aggs
+from gpu_harness import cg  # noqa: F401  (fixtures)
 
 pytestmark = pytest.mark.gpu
 
 ROWS = 120_000            # per shard: 12 chunk groups of 10 000 rows
 NSHARDS = 6
 NKEYS = 5_000             # a direct-indexed table too large for the shared-memory kernel
-
-
-@pytest.fixture(scope="module")
-def cg():
-    import torch
-    assert torch.cuda.is_available(), "these tests need an H100"
-    from citus_b200 import build
-    build.build()
-    from citus_b200 import columnar
-    columnar.init(0)
-    return columnar
 
 
 @pytest.fixture
@@ -154,7 +144,7 @@ def test_in_list_change_between_shards(cg):
         agg.desc = d
         sh = cg.Shard(rel)
         agg.scan_shard(sh, want_stats=False)
-        r = iref.aggregate(list(cols), [None, None, vn], where, [0], aggs)
+        r = ref.aggregate(list(cols), [None, None, vn], where, [0], aggs)
         for k, per in r.groups.items():
             acc = want.setdefault(k[0], [[0, 0] for _ in aggs])
             for a, st in enumerate(per):

@@ -5,21 +5,11 @@ them, and plans of more than three columns, which take the plain arena; widths 0
 partial; and WHERE lists that skip chunk groups."""
 import numpy as np
 import pytest
+from gpu_harness import cg  # noqa: F401  (fixtures)
 
 pytestmark = pytest.mark.gpu
 
 ROWS = 100_000 + 37          # 11 chunk groups, the last one short
-
-
-@pytest.fixture(scope="module")
-def cg():
-    import torch
-    assert torch.cuda.is_available(), "these tests need an H100"
-    from citus_b200 import build
-    build.build()
-    from citus_b200 import columnar
-    columnar.init(0)
-    return columnar
 
 
 def make_rel(cg, seed, nulls=False, key_base=0, nkeys=5000):

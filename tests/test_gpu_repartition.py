@@ -10,23 +10,13 @@ import numpy as np
 import pytest
 
 import partition_reference as pr
+from gpu_harness import cg  # noqa: F401  (fixtures)
 
 pytestmark = pytest.mark.gpu
 
 PS = [1, 2, 3, 7, 32, 255, 256, 257, 1000, 1024]
 CHUNK_ROWS = 2048 * 4096          # the offset scan's chunk of 2048 blocks of 4096 rows
 W = 64                             # hash values searched on either side of every interval boundary
-
-
-@pytest.fixture(scope="module")
-def cg():
-    import torch
-    assert torch.cuda.is_available(), "these tests need an H100"
-    from citus_b200 import build
-    build.build()
-    from citus_b200 import columnar
-    columnar.init(0)
-    return columnar
 
 
 def _dev(a, dtype=np.int64):

@@ -10,6 +10,7 @@ import numpy as np
 import pytest
 
 import reference as ref
+from gpu_harness import cg, kernel_family  # noqa: F401  (fixtures)
 
 pytestmark = pytest.mark.gpu
 
@@ -19,17 +20,6 @@ FLOAT_RTOL = 1e-12
 def pgdate(s):
     y, m, d = map(int, s.split("-"))
     return (datetime.date(y, m, d) - datetime.date(2000, 1, 1)).days
-
-
-@pytest.fixture(scope="module")
-def cg():
-    import torch
-    assert torch.cuda.is_available(), "these tests need an H100"
-    from citus_b200 import build
-    build.build()
-    from citus_b200 import columnar
-    columnar.init(0)
-    return columnar
 
 
 def oracle_table(oracle, rel, chunk_row_limit=10000):
@@ -669,17 +659,6 @@ def test_join_count_sum_matches_row_at_a_time_join(cg, oracle):
 
 
 # --------------------------------------------------------------------------- NULL-bearing chunk groups on the fast paths
-@pytest.fixture
-def kernel_family(cg):
-    """runs a test body once per kernel family through the same C-ABI calls"""
-    def use(name):
-        cg.set_option("jit", {"jit": 1, "jit_always": 2, "aot": 0, "general": 0}[name])
-        cg.set_option("force_general", 1 if name == "general" else 0)
-    yield use
-    cg.set_option("jit", 1)
-    cg.set_option("force_general", 0)
-
-
 @pytest.mark.parametrize("family", ["jit", "jit_always", "aot", "general"])
 @pytest.mark.parametrize("path", ["shard", "e2e", "dma"])
 def test_c2_with_nulls_on_every_kernel_family(cg, oracle, kernel_family, family, path):

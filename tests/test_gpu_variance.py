@@ -1,7 +1,7 @@
 """var_pop / var_samp / stddev_pop / stddev_samp in the fused scan against the exact reference, on every kernel family.
-The GPU keeps the exact state (N, sum(x), sum(x^2)) of CG_AGG_VARIANCE; tests/variance_reference.py computes the same
-state from the rows (on top of tests/reference.py, FILTER by composition) and the final functions from their
-definition.  Every word is compared exactly, and the final text through cg_numeric_var_out."""
+The GPU keeps the exact state (N, sum(x), sum(x^2)) of CG_AGG_VARIANCE; tests/reference.py computes the same
+state from the rows and the final functions from their definition.  Every word is compared exactly, and the final text
+through cg_numeric_var_out."""
 import dataclasses
 import json
 import os
@@ -10,36 +10,14 @@ import numpy as np
 import pytest
 
 import reference as ref
-import variance_reference as vref
+from gpu_harness import cg, kernel_family, FAMILIES  # noqa: F401  (fixtures)
 
 pytestmark = pytest.mark.gpu
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-FAMILIES = ["jit", "jit_always", "aot", "general"]
 INT64_MIN, INT64_MAX = -(1 << 63), (1 << 63) - 1
 NUMERIC2 = 2 | (2 << 8)
 VARIANCE = 9
-
-
-@pytest.fixture(scope="module")
-def cg():
-    import torch
-    assert torch.cuda.is_available(), "these tests need an H100"
-    from citus_b200 import build
-    build.build()
-    from citus_b200 import columnar
-    columnar.init(0)
-    return columnar
-
-
-@pytest.fixture
-def kernel_family(cg):
-    def use(name):
-        cg.set_option("jit", {"jit": 1, "jit_always": 2, "aot": 0, "general": 0}[name])
-        cg.set_option("force_general", 1 if name == "general" else 0)
-    yield use
-    cg.set_option("jit", 1)
-    cg.set_option("force_general", 0)
 
 
 def keyed(d, group_cols, got):
@@ -116,7 +94,7 @@ def assert_exact(cg, got, want, aggs, scales=None):
                 scale = scales[a] if scales else 0
                 for final in range(4):
                     assert cg.numeric_var_out(final, g["count"], g["sum"], g["sumsq"], scale) == \
-                        vref.var_out(final, w.count, w.sum, w.sumsq, scale), (key, a, final)
+                        ref.var_out(final, w.count, w.sum, w.sumsq, scale), (key, a, final)
 
 
 def var_words(nlimbs_sum, qlimbs):
@@ -151,7 +129,7 @@ def test_every_key_form_with_nulls_where_and_filter(cg, kernel_family, family):
             cg.sum_(3), cg.variance(2, filter=(5, ">=", 1))]
     for where in ([], [(1, "<", 2)], ("or", (2, ">", 0), (4, "<", 0))):
         for shape in SHAPES:
-            want = vref.filtered(cols, nulls, where, shape["group_cols"], aggs)
+            want = ref.aggregate(cols, nulls, where, shape["group_cols"], aggs)
             for use_bounds in (True, False):
                 _, got, _ = run(cg, rel, where, aggs=aggs, use_bounds=use_bounds, **shape)
                 assert_exact(cg, got, want, aggs)
@@ -175,7 +153,7 @@ def test_one_two_and_four_limb_forms(cg, kernel_family, family):
                             (2, 0, var_words(2, 4)), (2, 2**40, var_words(1, 4))):
         aggs = [cg.count_star(), cg.variance(c)]
         for group in ([], [0]):
-            want = vref.aggregate(cols, None, [], group, aggs)
+            want = ref.aggregate(cols, None, [], group, aggs)
             _, got, layout = run(cg, rel, [], group, aggs, bounds=[0, bound])
             assert layout[0] == 1 + words, (c, bound, layout)
             assert_exact(cg, got, want, aggs)
@@ -205,12 +183,12 @@ def test_numeric_column_compressed_shards_and_several_shards(cg, oracle, kernel_
     aggs = [cg.count_star(), cg.variance(1), cg.variance(2, filter=(0, "<>", 1))]
     for rels, cs in (([p[0] for p in parts], None), ([p[1] for p in parts], None)):
         for i, p in enumerate(parts):
-            want = vref.filtered(p[2], p[3], [], [0], aggs)
+            want = ref.aggregate(p[2], p[3], [], [0], aggs)
             _, got, _ = run(cg, rels[i], [], [0], aggs)
             assert_exact(cg, got, want, aggs, scales=[0, 2, 0] if rels[i] is p[0] else None)
         cols = [np.concatenate([p[2][c] for p in parts]) for c in range(3)]
         nulls = [np.concatenate([p[3][c] for p in parts]) for c in range(3)]
-        want = vref.filtered(cols, nulls, [], [0], aggs)
+        want = ref.aggregate(cols, nulls, [], [0], aggs)
         _, got, _ = run(cg, rels, [], [0], aggs)
         assert_exact(cg, got, want, aggs)
 
@@ -222,7 +200,7 @@ def test_scan_relation_end_to_end(cg, kernel_family, family):
     aggs = [cg.variance(4), cg.count_star(), cg.variance(2, filter=(1, "=", 0))]
     for e2e in ("pageable", "dma"):
         for shape in SHAPES[:3]:
-            want = vref.filtered(cols, nulls, [(0, "<>", 3)], shape["group_cols"], aggs)
+            want = ref.aggregate(cols, nulls, [(0, "<>", 3)], shape["group_cols"], aggs)
             _, got, _ = run(cg, rel, [(0, "<>", 3)], aggs=aggs, e2e=e2e, **shape)
             assert_exact(cg, got, want, aggs)
 
@@ -236,7 +214,7 @@ def test_contestant_golden_on_the_gpu(cg, kernel_family):
         kernel_family(family)
         _, got, _ = run(cg, rel, [], [], [cg.variance(0), cg.sum_(0)])
         v = got[()][0]
-        assert cg.numeric_var_out(vref.STDDEV_SAMP, v["count"], v["sum"], v["sumsq"], 0) == g["stddev_samp"]
+        assert cg.numeric_var_out(ref.STDDEV_SAMP, v["count"], v["sum"], v["sumsq"], 0) == g["stddev_samp"]
         assert cg.numeric_div_out(got[()][1]["sum"], 0, got[()][1]["count"]) == g["avg"]
 
 
@@ -269,7 +247,7 @@ def test_export_merge_rows_round_trip_and_the_carry_chain(cg):
         b.merge_rows(keys.data_ptr(), kn.data_ptr(), words.data_ptr(), rows)
         b.merge_rows(keys.data_ptr(), kn.data_ptr(), words.data_ptr(), rows)
         ga, gb = a.groups(), b.groups()
-        want = vref.aggregate(cols, None, [], [0], aggs)
+        want = ref.aggregate(cols, None, [], [0], aggs)
         assert_exact(cg, {(k,): v for k, v in ga.items()}, want, aggs)
         for k in ga:
             assert gb[k][0]["count"] == 2 * ga[k][0]["count"] and gb[k][0]["sum"] == 2 * ga[k][0]["sum"]
@@ -360,4 +338,4 @@ def test_bound_violated_by_the_data_is_an_error(cg, kernel_family, family):
             aggs = [cg.variance(c), cg.count_star()]
             _, got, layout = run(cg, rel, [], group, aggs, bounds=[good, 0])
             assert layout[0] == 1 + var_words(sl, ql)
-            assert_exact(cg, got, vref.aggregate(cols, None, [], group, aggs), aggs)
+            assert_exact(cg, got, ref.aggregate(cols, None, [], group, aggs), aggs)

@@ -9,33 +9,13 @@ import numpy as np
 import pytest
 
 import reference as ref
-from test_gpu_exact import FAMILIES, assert_matches_reference
+from test_gpu_exact import assert_matches_reference
 from test_where_reference import HAND_DATUMS, INT64_MAX, INT64_MIN, LIMITS, OPS, constant_pools, image_with_datums, random_tree
+from gpu_harness import cg, kernel_family, FAMILIES  # noqa: F401  (fixtures)
 
 pytestmark = pytest.mark.gpu
 
 BPCHAR1 = 3
-
-
-@pytest.fixture(scope="module")
-def cg():
-    import torch
-    assert torch.cuda.is_available(), "these tests need an H100"
-    from citus_b200 import build
-    build.build()
-    from citus_b200 import columnar
-    columnar.init(0)
-    return columnar
-
-
-@pytest.fixture
-def kernel_family(cg):
-    def use(name):
-        cg.set_option("jit", {"jit": 1, "jit_always": 2, "aot": 0, "general": 0}[name])
-        cg.set_option("force_general", 1 if name == "general" else 0)
-    yield use
-    cg.set_option("jit", 1)
-    cg.set_option("force_general", 0)
 
 
 class Table:

@@ -1,6 +1,6 @@
 """IN / NOT IN lists and IS [NOT] NULL atoms on the host side, without a GPU: the descriptor make_desc builds (the list
-table), the checks of the new fields, chunk-group skipping and cg_relation_bounds against tests/in_null_reference.py over
-random trees that mix the new atoms with the comparison atoms, the generated kernels of every kind and form, and the
+table), the checks of the new fields, chunk-group skipping and cg_relation_bounds against tests/reference.py over
+random trees that mix the new atoms with the comparison atoms, IN lists against their OR of equalities, the generated kernels of every kind and form, and the
 generated source of the existing query shapes, which must stay byte for byte what it was."""
 import ctypes as C
 import hashlib
@@ -9,7 +9,6 @@ import math
 import numpy as np
 import pytest
 
-import in_null_reference as iref
 import reference as ref
 from test_where_reference import OPS, constant_pools, edge_relation, library_mask, random_tree
 
@@ -116,21 +115,60 @@ def test_list_and_null_test_columns_count_toward_the_column_limit(cg):
 
 # --------------------------------------------------------------------------- reference rows
 def test_reference_row_semantics():
-    assert iref.atom_value((0, "in", (1, 2)), 1, False, False) is True
-    assert iref.atom_value((0, "in", (1, 2)), 3, False, False) is False
-    assert iref.atom_value((0, "in", (1, None)), 3, False, False) is None
-    assert iref.atom_value((0, "in", (1, None)), 1, False, False) is True
-    assert iref.atom_value((0, "in", (1,)), 0, True, False) is None
-    assert iref.atom_value((0, "not in", (1, 2)), 3, False, False) is True
-    assert iref.atom_value((0, "not in", (1, None)), 3, False, False) is None
-    assert iref.atom_value((0, "not in", (1, None)), 1, False, False) is False
-    assert iref.atom_value((0, "not in", (1,)), 0, True, False) is None
-    assert iref.atom_value((0, "is null"), 0, True, False) is True and iref.atom_value((0, "is null"), 0, False, False) is False
-    assert iref.atom_value((0, "is not null"), 0, True, False) is False
-    assert iref.atom_value((0, "in", (math.nan,)), math.nan, False, True) is True
-    assert iref.atom_value((0, "in", (-0.0,)), 0.0, False, True) is True
-    assert iref.atom_value((0, "not in", (0.0,)), -0.0, False, True) is False
+    def v(atom, x, isnull, is_float):
+        return ref.atom_value(atom, [x], [isnull], (0,) if is_float else ())
+    assert v((0, "in", (1, 2)), 1, False, False) is True
+    assert v((0, "in", (1, 2)), 3, False, False) is False
+    assert v((0, "in", (1, None)), 3, False, False) is None
+    assert v((0, "in", (1, None)), 1, False, False) is True
+    assert v((0, "in", (1,)), 0, True, False) is None
+    assert v((0, "not in", (1, 2)), 3, False, False) is True
+    assert v((0, "not in", (1, None)), 3, False, False) is None
+    assert v((0, "not in", (1, None)), 1, False, False) is False
+    assert v((0, "not in", (1,)), 0, True, False) is None
+    assert v((0, "is null"), 0, True, False) is True and v((0, "is null"), 0, False, False) is False
+    assert v((0, "is not null"), 0, True, False) is False
+    assert v((0, "in", (math.nan,)), math.nan, False, True) is True
+    assert v((0, "in", (-0.0,)), 0.0, False, True) is True
+    assert v((0, "not in", (0.0,)), -0.0, False, True) is False
 
+
+
+def test_in_lists_equal_their_or_of_equalities():
+    """a non-empty IN list without NULL elements answers as the OR of its "=" atoms and NOT IN as the AND of its "<>" atoms, in
+    WHERE, FILTER and bool_* arguments, for the rows and for the chunk mask"""
+    import dataclasses
+    from test_agg_filter_host import FC, map_atoms, random_language
+
+    def expand(atom):
+        if atom[1] not in ("in", "not in"):
+            return atom
+        return ("or" if atom[1] == "in" else "and",) + tuple((atom[0], "=" if atom[1] == "in" else "<>", e) for e in atom[2])
+    rng = np.random.default_rng(20261017)
+    lists = 0
+    for trial in range(120):
+        if trial % 40 == 0:
+            cols, nulls, atom, agg = random_language(rng, forms=("const", "in", "in", "null"))
+            minmax = ref.skip_minmax(cols, nulls, 120, 30, FC)
+
+        def no_null_atom():
+            while True:
+                a = atom()
+                if a[1] not in ("in", "not in"):
+                    return a
+                if any(e is not None for e in a[2]):
+                    return a[:2] + (tuple(e for e in a[2] if e is not None),)
+        where = random_tree(rng, no_null_atom, 4)
+        aggs = [agg(int(k), random_tree(rng, no_null_atom, 3) if rng.random() < 0.5 else None) for k in rng.integers(0, 10, 3)]
+        aggs = [dataclasses.replace(a, arg=random_tree(rng, no_null_atom, 3)) if a.arg is not None else a for a in aggs]
+        lists += sum(a[1] in ("in", "not in") for a in ref._atoms(ref.as_tree(where)))
+        ors = [dataclasses.replace(a, filter=map_atoms(a.filter, expand), arg=map_atoms(a.arg, expand)) for a in aggs]
+        got = ref.aggregate(cols, nulls, where, [5], aggs, FC)
+        want = ref.aggregate(cols, nulls, map_atoms(where, expand), [5], ors, FC)
+        assert repr(got) == repr(want), where
+        assert ref.selected_chunk_mask(cols, nulls, where, 120, 30, FC, minmax=minmax) == \
+            ref.selected_chunk_mask(cols, nulls, map_atoms(where, expand), 120, 30, FC, minmax=minmax), where
+    assert lists > 50
 
 # --------------------------------------------------------------------------- chunk-group skipping and bounds
 def _list_atom(rng, pools, c, minmax_vals):
@@ -190,7 +228,7 @@ def test_selected_chunk_mask_and_relation_bounds_against_reference(cg):
         except capi.CitusGpuError as e:                         # more than 8 lists or 1024 values: refused, as documented
             assert e.code == capi.CG_EUNSUPPORTED
             continue
-        want = iref.selected_chunk_mask(cols7, nulls7, where, stripe_rows, chunk_rows, float_cols=fc, minmax=minmax)
+        want = ref.selected_chunk_mask(cols7, nulls7, where, stripe_rows, chunk_rows, float_cols=fc, minmax=minmax)
         got = library_mask(cg, rel7, d)
         assert got == want, f"seed {seed} where {where}"
         refuted += ref.chunks_filtered(want)
@@ -215,10 +253,10 @@ def test_in_list_over_four_chunk_groups_restates_citus_5803(cg):
     where = [(0, "in", (11, 20, 21))]
     d = cg.make_desc(where, [], [cg.count_star()])
     mask = library_mask(cg, rel, d)
-    want = iref.selected_chunk_mask([c], None, where, 4000, 1000)
+    want = ref.selected_chunk_mask([c], None, where, 4000, 1000)
     assert mask == want == [[True, True, False, False]]
     assert ref.chunks_filtered(want) == 2
-    res = iref.aggregate([c], None, where, [], [cg.count_star()])
+    res = ref.aggregate([c], None, where, [], [cg.count_star()])
     kept = ref.rows_kept(want, 4000, 4000, 1000)
     assert (kept, kept - res.rows_passed, res.rows_passed) == (2000, 1, 1999)
     assert cg.relation_bounds(rel, d)[3] == 2000

@@ -1,5 +1,6 @@
 """var_pop / var_samp / stddev_pop / stddev_samp on the host side, without a GPU: cg_numeric_var_out against the independent
-reference tests/variance_reference.py (the reference's goldens and seeded states at the edges), the descriptor checks of
+reference tests/reference.py (the reference's goldens and seeded states at the edges), the reference's variance state
+against its sum over the same argument, the descriptor checks of
 CG_AGG_VARIANCE, the generated kernels of variance plans, and the generated source of the plans without the kind, which
 must stay byte for byte what the parent commit's generator emitted."""
 import ctypes as C
@@ -10,11 +11,11 @@ import random
 
 import pytest
 
-import variance_reference as vref
+import reference as ref
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 INT64_MIN, INT64_MAX = -(1 << 63), (1 << 63) - 1
-FINALS = (vref.VAR_POP, vref.VAR_SAMP, vref.STDDEV_POP, vref.STDDEV_SAMP)
+FINALS = (ref.VAR_POP, ref.VAR_SAMP, ref.STDDEV_POP, ref.STDDEV_SAMP)
 
 
 @pytest.fixture(scope="module")
@@ -59,9 +60,9 @@ def test_contestant_stddev_samp_golden(cg):
     """SELECT avg(rating), stddev_samp(rating) FROM contestant (columnar_query.out): 433.746119785032"""
     g = golden()["contestant"]
     n, s, q = state(g["rating"])
-    assert vref.var_out(vref.STDDEV_SAMP, n, s, q, 0) == g["stddev_samp"] == "433.746119785032"
-    assert cg.numeric_var_out(vref.STDDEV_SAMP, n, s, q, 0) == g["stddev_samp"]
-    assert cg.numeric_var_out(vref.VAR_SAMP, n, s, q, 0) == vref.var_out(vref.VAR_SAMP, n, s, q, 0) == "188135.696428571429"
+    assert ref.var_out(ref.STDDEV_SAMP, n, s, q, 0) == g["stddev_samp"] == "433.746119785032"
+    assert cg.numeric_var_out(ref.STDDEV_SAMP, n, s, q, 0) == g["stddev_samp"]
+    assert cg.numeric_var_out(ref.VAR_SAMP, n, s, q, 0) == ref.var_out(ref.VAR_SAMP, n, s, q, 0) == "188135.696428571429"
 
 
 def test_aggdata_stddev_by_id_golden_is_null(cg):
@@ -75,13 +76,13 @@ def test_aggdata_stddev_by_id_golden_is_null(cg):
         assert want == ""
         n, s, q = state(by_id[i])
         assert n <= 1
-        for final in (vref.STDDEV_SAMP, vref.VAR_SAMP):
-            assert vref.var_out(final, n, s, q, 0) is None
+        for final in (ref.STDDEV_SAMP, ref.VAR_SAMP):
+            assert ref.var_out(final, n, s, q, 0) is None
             assert cg.numeric_var_out(final, n, s, q, 0) is None
 
 
 def check(cg, final, n, s, q, scale):
-    want = vref.var_out(final, n, s, q, scale)
+    want = ref.var_out(final, n, s, q, scale)
     got = cg.numeric_var_out(final, n, s, q, scale)
     assert got == want, (final, n, s, q, scale)
     return got
@@ -89,7 +90,7 @@ def check(cg, final, n, s, q, scale):
 
 def test_small_counts_and_constant_inputs(cg):
     for final in FINALS:
-        sample = final in (vref.VAR_SAMP, vref.STDDEV_SAMP)
+        sample = final in (ref.VAR_SAMP, ref.STDDEV_SAMP)
         assert check(cg, final, 0, 0, 0, 0) is None
         one = check(cg, final, 1, -7, 49, 0)
         assert (one is None) if sample else (one == "0")
@@ -147,19 +148,42 @@ def test_var_out_errors(cg):
     buf = C.create_string_buffer(64)
     isnull = C.c_int32()
     L = capi.lib()
-    assert L.cg_numeric_var_out(vref.STDDEV_SAMP, 8, 0, 18755, q, 0, buf, 64, C.byref(isnull)) == 0
+    assert L.cg_numeric_var_out(ref.STDDEV_SAMP, 8, 0, 18755, q, 0, buf, 64, C.byref(isnull)) == 0
     # the text of a tiny variance has many fraction digits: a buffer that is too small is CG_EINVAL
     n, s, qq = (1 << 62), (1 << 62) * 5 + 1, (1 << 62) * 25 + 11
-    need = len(vref.var_out(vref.VAR_POP, n, s, qq, 0)) + 1
+    need = len(ref.var_out(ref.VAR_POP, n, s, qq, 0)) + 1
     qs = (C.c_uint64 * 3)(qq & (2**64 - 1), qq >> 64, 0)
     small = C.create_string_buffer(need - 1)
-    assert L.cg_numeric_var_out(vref.VAR_POP, n, s >> 64, s & (2**64 - 1), qs, 0, small, need - 1, C.byref(isnull)) == capi.CG_EINVAL
+    assert L.cg_numeric_var_out(ref.VAR_POP, n, s >> 64, s & (2**64 - 1), qs, 0, small, need - 1, C.byref(isnull)) == capi.CG_EINVAL
     exact = C.create_string_buffer(need)
-    assert L.cg_numeric_var_out(vref.VAR_POP, n, s >> 64, s & (2**64 - 1), qs, 0, exact, need, C.byref(isnull)) == 0
-    assert exact.value.decode() == vref.var_out(vref.VAR_POP, n, s, qq, 0)
+    assert L.cg_numeric_var_out(ref.VAR_POP, n, s >> 64, s & (2**64 - 1), qs, 0, exact, need, C.byref(isnull)) == 0
+    assert exact.value.decode() == ref.var_out(ref.VAR_POP, n, s, qq, 0)
     for final, scale, cnt in ((4, 0, 2), (-1, 0, 2), (0, 31, 2), (0, -1, 2), (0, 0, -1)):
         assert L.cg_numeric_var_out(final, cnt, 0, 0, q, scale, buf, 64, C.byref(isnull)) == capi.CG_EINVAL
 
+
+
+def test_variance_counts_and_sums_like_sum():
+    """a variance aggregate's count, sum and overflow equal those of sum over the same argument, with FILTERs and WHERE
+    trees of every atom form; its sumsq is the sum of the squared inputs"""
+    import dataclasses
+
+    import numpy as np
+    from test_agg_filter_host import FC, SCALES, random_language
+    from test_where_reference import random_tree
+    rng = np.random.default_rng(20261019)
+    for trial in range(90):
+        if trial % 30 == 0:
+            cols, nulls, atom, agg = random_language(rng)
+        where = random_tree(rng, atom, 4)
+        group = [[], [5]][trial % 2]
+        aggs = [agg(ref.VARIANCE, random_tree(rng, atom, 3) if rng.random() < 0.5 else None) for _ in range(3)]
+        got = ref.aggregate(cols, nulls, where, group, aggs, FC, SCALES)
+        want = ref.aggregate(cols, nulls, where, group, [dataclasses.replace(a, kind=ref.SUM) for a in aggs], FC, SCALES)
+        assert set(got.groups) == set(want.groups)
+        for key, per in got.groups.items():
+            for v, s in zip(per, want.groups[key]):
+                assert (v.count, v.sum, v.overflow, v.sumsq) == (s.count, s.sum, s.overflow, s.sumsq), (where, key)
 
 # --------------------------------------------------------------------------- descriptors and generated kernels
 COLS = [(1, 0), (2, 0), (4, 0), (8, 0), (4, 1), (8, 1), (-1, 3), (-1, 2 | (2 << 8))]

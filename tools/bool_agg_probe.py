@@ -7,7 +7,7 @@ bench.py's C5 leg (SF100, 32 shards, HBM resident), Q1's WHERE and GROUP BY l_re
 
 (the synthetic lineitem has no l_linenumber; l_suppkey, int4, stands in for the bit aggregates' integer column),
 timed alternately in one process.  Prints per query the median ms per query and the fused kernel's device time, with
-the card and its power limit, and checks both queries' groups exactly against tests/bool_bit_reference.py on a sample.
+the card and its power limit, and checks both queries' groups exactly against tests/reference.py on a sample.
 
     python tools/bool_agg_probe.py [--rows 600000000] [--reps 10] [--sample-rows 150000] [--json FILE]
 """
@@ -34,7 +34,6 @@ build.build()
 from citus_b200 import capi  # noqa: E402
 from citus_b200 import columnar as cg  # noqa: E402
 
-import bool_bit_reference as bref  # noqa: E402
 import reference as ref  # noqa: E402
 
 
@@ -131,7 +130,7 @@ def main():
         part.scan_shard(cg.Shard(sample), want_stats=False)
         got = part.groups()
         part.free()
-        want = bref.aggregate(cols, None, q["quals"], q["group"], aggs)
+        want = ref.aggregate(cols, None, q["quals"], q["group"], aggs)
         ok = len(got) == len(want.groups)
         for k, per_got in got.items():
             key = ref.unpack_two_column_key(k)

@@ -14,7 +14,7 @@
               tools/join_aggregate_probe.py (count(*), sum(r.x), sum(s.y) GROUP BY r.g) on the same keys
 
 Prints per query the median over --reps warm runs (host clock around the launches and a device synchronise), with the
-card, its power limit and SM clock read in the same run.  Each query is checked against tests/case_agg_reference.py on a
+card, its power limit and SM clock read in the same run.  Each query is checked against tests/reference.py on a
 sample (the scans: the first stripe of one shard, 150 000 rows; the join: --sample-rows rows per side); the run fails
 when a check does.
 
@@ -41,7 +41,7 @@ from citus_b200 import capi  # noqa: E402
 from citus_b200 import columnar as cg  # noqa: E402
 from filter_probe import card, synth_columns  # noqa: E402
 
-import case_agg_reference as caseref  # noqa: E402
+import reference as ref  # noqa: E402
 import join_agg_reference as jref  # noqa: E402
 
 NSHARDS = 32
@@ -124,7 +124,7 @@ def scan_leg(cols_spec, queries, nrows, reps, seed, out):
             finally:
                 agg.free()
             cols = synth_columns(cols_spec, 0, sample.rows, seed)
-            want = caseref.aggregate(cols, None, q["where"], q["group"], aggs)
+            want = ref.aggregate(cols, None, q["where"], q["group"], aggs)
             ok = set(got) == {k[0] for k in want.groups}
             for (k,), pw in want.groups.items():
                 for a, w in enumerate(pw):
@@ -178,7 +178,7 @@ def join_leg(nrows, reps, sample_rows, out):
             got = agg.groups()
         finally:
             agg.free()
-        want = caseref.aggregate(jc, jn, q["where"], q["group"], q["aggs"])
+        want = ref.aggregate(jc, jn, q["where"], q["group"], q["aggs"])
         ok = set(got) == {k[0] for k in want.groups}
         for (k,), pw in want.groups.items():
             for a, w in enumerate(pw):

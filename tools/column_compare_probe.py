@@ -11,7 +11,7 @@
 
 timed alternately in one process.  Prints per query the median ms per query over the runs, the fused kernels' device
 time, the kernel family that ran (generated kernels launched per query; none = an ahead-of-time kernel) and the card with
-its power limit, and checks every query's groups against the exact reference (tests/column_compare_reference.py) on a
+its power limit, and checks every query's groups against the exact reference (tests/reference.py) on a
 sample.
 
     python tools/column_compare_probe.py [--rows 600000000] [--c2-rows 200000000] [--reps 10] [--sample-rows 150000] [--json FILE]
@@ -40,7 +40,7 @@ from citus_b200 import capi  # noqa: E402
 from citus_b200 import columnar as cg  # noqa: E402
 from filter_probe import _Env, card, synth_columns  # noqa: E402
 
-import column_compare_reference as cref  # noqa: E402
+import reference as ref  # noqa: E402
 
 DATE_LO, DATE_HI = -2922, -366                     # 1992-01-01 .. 1998-12-31 as days since 2000-01-01
 DATES = [(4, 0, DATE_LO, DATE_HI, 0)] * 3         # 0 l_shipdate, 1 l_commitdate, 2 l_receiptdate
@@ -125,7 +125,7 @@ def main():
         sh.free()
         got = part.groups()
         part.free()
-        want = cref.aggregate(cols, None, q["quals"], q["group"], aggs)
+        want = ref.aggregate(cols, None, q["quals"], q["group"], aggs)
         ok = st.rows_passed == want.rows_passed and {(k,) for k in got} == set(want.groups)
         for k, per_got in got.items():
             for a, (g, w) in enumerate(zip(per_got, want.groups.get((k,), []))):

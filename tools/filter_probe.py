@@ -7,7 +7,7 @@ HBM resident), Q1 as bench.py runs it and Q1 without sum(l_discount) (eight aggr
 
 (every column already staged for Q1), timed alternately in one process.  Prints per query the ms per query, the
 fused kernel's device time, bytes per row and the fraction of 3.35 TB/s, with the card and its power limit, and
-checks both queries' groups against the exact reference (tests/reference.py, FILTER by composition) on a sample.
+checks both queries' groups against the exact reference (tests/reference.py) on a sample.
 
     python tools/filter_probe.py [--rows 600000000] [--reps 10] [--sample-rows 150000] [--json FILE]
 """
@@ -67,18 +67,6 @@ def synth_columns(columns, first_row, nrows, seed):
     return out
 
 
-def composed(cols, where, group, aggs):
-    res = ref.aggregate(cols, None, where, group, aggs)
-    for j, a in enumerate(aggs):
-        if a.filter is None:
-            continue
-        f = a.filter if a.filter[0] in ("and", "or") else ("and", a.filter)
-        sub = ref.aggregate(cols, None, ("and", ("and",) + tuple(where), f), group, [a])
-        for key, per in res.groups.items():
-            per[j] = sub.groups[key][0] if key in sub.groups else ref.AggResult()
-    return res
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rows", type=int, default=600_000_000)
@@ -133,7 +121,7 @@ def main():
         part.scan_shard(cg.Shard(sample), want_stats=False)
         got = part.groups()
         part.free()
-        want = composed(cols, q["quals"], q["group"], aggs)
+        want = ref.aggregate(cols, None, q["quals"], q["group"], aggs)
         ok = len(got) == len(want.groups)
         for k, per_got in got.items():
             key = ref.unpack_two_column_key(k)

@@ -13,7 +13,7 @@ resident) and on C2 with 5 % NULLs in v:
     c2null_f the same plus count(*) FILTER (WHERE v IS NULL)
 
 timed alternately in one process.  Prints per query the ms per query and the fused kernel's device time with the card and
-its power limit, and checks every query's groups against the exact reference (tests/in_null_reference.py) on a sample.
+its power limit, and checks every query's groups against the exact reference (tests/reference.py) on a sample.
 
     python tools/in_list_probe.py [--rows 600000000] [--c2-rows 200000000] [--reps 10] [--sample-rows 150000] [--json FILE]
 """
@@ -40,7 +40,7 @@ from citus_b200 import capi  # noqa: E402
 from citus_b200 import columnar as cg  # noqa: E402
 from filter_probe import _Env, card, synth_columns  # noqa: E402
 
-import in_null_reference as iref  # noqa: E402
+import reference as ref  # noqa: E402
 
 C2_NULL = list(bench.C2_COLUMNS)
 C2_NULL[2] = (8, 0, -10**9, 10**9, 50000)           # 5 % NULLs in v, as bench.py's C2-NULL leg
@@ -153,7 +153,7 @@ def main():
         sh.free()
         got = part.groups()
         part.free()
-        want = iref.aggregate(cols, nulls, q["quals"], q["group"], aggs)
+        want = ref.aggregate(cols, nulls, q["quals"], q["group"], aggs)
         ok = st.rows_passed == want.rows_passed
         if q["group"]:
             ok &= {(k,) for k in got} == set(want.groups)

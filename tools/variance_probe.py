@@ -8,7 +8,7 @@
 timed alternately in one process.  Both variance aggregates are one CG_AGG_VARIANCE state each (N, sum(x), sum(x^2));
 with the skip lists' bounds their sum(x^2) is one word (l_quantity) and two 32-bit limbs (l_extendedprice).  Prints per
 query the median ms per query and the fused kernel's device time, with the card and its power limit, and checks both
-queries' groups exactly against tests/variance_reference.py on a sample, the final texts included.
+queries' groups exactly against tests/reference.py on a sample, the final texts included.
 
     python tools/variance_probe.py [--rows 600000000] [--reps 10] [--sample-rows 150000] [--json FILE]
 """
@@ -35,7 +35,6 @@ build.build()
 from citus_b200 import capi  # noqa: E402
 from citus_b200 import columnar as cg  # noqa: E402
 
-import variance_reference as vref  # noqa: E402
 import reference as ref  # noqa: E402
 
 
@@ -66,7 +65,7 @@ def synth_columns(columns, first_row, nrows, seed):
     return out
 
 
-FINAL = {3: vref.STDDEV_SAMP, 4: vref.VAR_POP}               # aggregate number in B -> its SQL final function
+FINAL = {3: ref.STDDEV_SAMP, 4: ref.VAR_POP}               # aggregate number in B -> its SQL final function
 
 
 def exact(g, w, kind, a):
@@ -77,9 +76,9 @@ def exact(g, w, kind, a):
         return True
     if g["sum"] != w.sum:
         return False
-    if kind == vref.VARIANCE:
+    if kind == ref.VARIANCE:
         return g["sumsq"] == w.sumsq and cg.numeric_var_out(FINAL[a], g["count"], g["sum"], g["sumsq"], 2) == \
-            vref.var_out(FINAL[a], w.count, w.sum, w.sumsq, 2)
+            ref.var_out(FINAL[a], w.count, w.sum, w.sumsq, 2)
     return True
 
 
@@ -138,7 +137,7 @@ def main():
         part.scan_shard(cg.Shard(sample), want_stats=False)
         got = part.groups()
         part.free()
-        want = vref.aggregate(cols, None, q["quals"], q["group"], aggs)
+        want = ref.aggregate(cols, None, q["quals"], q["group"], aggs)
         ok = len(got) == len(want.groups)
         for k, per_got in got.items():
             key = ref.unpack_two_column_key(k)
