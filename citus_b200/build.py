@@ -15,7 +15,7 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "lib", "libcitus_gpu.so")
 STAMP = LIB + ".flags"          # the compile flags the library was built with: other flags (another GPU target) rebuild it
-SOURCES = ["cg_scan.cu", "cg_decompress.cu", "cg_scan_fast.cu", "cg_scan_small.cu", "cg_partition.cu", "cg_join.cu", "cg_comm.cu", "cg_values.cu", "cg_varlena.cu", "cg_narrow.cu", "cg_host.cpp", "cg_plan.cpp", "cg_numeric.cpp", "cg_gen.cpp", "cg_jit.cpp"]
+SOURCES = ["cg_scan.cu", "cg_decompress.cu", "cg_scan_fast.cu", "cg_scan_small.cu", "cg_scan_rows.cu", "cg_partition.cu", "cg_join.cu", "cg_comm.cu", "cg_values.cu", "cg_varlena.cu", "cg_narrow.cu", "cg_host.cpp", "cg_plan.cpp", "cg_numeric.cpp", "cg_gen.cpp", "cg_jit.cpp"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",

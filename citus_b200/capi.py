@@ -167,6 +167,8 @@ SYMBOLS = [
     ("cg_partial_reset", C.c_int, [_P]),
     ("cg_partial_set_packing", C.c_int, [_P, C.c_int32]),
     ("cg_scan_shard", C.c_int, [_P, C.POINTER(CgScanDesc), _P, C.POINTER(CgScanStats)]),
+    ("cg_scan_shard_rows", C.c_int, [_P, C.POINTER(CgScanDesc), _P, C.c_int32, C.c_int64, _P, _P, C.POINTER(C.c_int64),
+                                     C.POINTER(CgScanStats)]),
     ("cg_relation_register", C.c_int, [C.POINTER(CgRelation)]),
     ("cg_relation_unregister", C.c_int, [C.POINTER(CgRelation)]),
     ("cg_scan_relation", C.c_int, [C.POINTER(CgRelation), C.POINTER(CgScanDesc), _P, C.POINTER(CgScanStats)]),

@@ -540,6 +540,19 @@ class Shard:
     def rows(self):
         return lib().cg_shard_rows(self.h)
 
+    def scan_rows(self, desc: CgScanDesc, atts, d_col_ptrs=None, d_null_ptrs=None, capacity=0, want_stats=True):
+        """cg_scan_shard_rows: SELECT atts FROM shard WHERE <desc's WHERE tree> in the shard's row order, into the caller's
+        device arrays (int64 values; a null list holds None or a device byte array per column, as join_aggregate takes
+        them).  capacity 0 only counts.  Returns (passing rows, stats)."""
+        atts_arr = (C.c_int32 * len(atts))(*atts)
+        cols = None if d_col_ptrs is None else (C.c_void_p * len(d_col_ptrs))(*d_col_ptrs)
+        nulls = None if d_null_ptrs is None else (C.c_void_p * len(d_null_ptrs))(*d_null_ptrs)
+        n = C.c_int64()
+        st = CgScanStats()
+        check(lib().cg_scan_shard_rows(self.h, C.byref(desc), atts_arr, len(atts), capacity, cols, nulls, C.byref(n),
+                                       C.byref(st) if want_stats else None))
+        return n.value, st
+
     def narrow_image(self, cg: int, att: int):
         """(base, width, words: uint64 array) of the narrow image of attribute att in chunk group cg; width 255 = none"""
         base, width, n = C.c_int64(), C.c_uint32(), C.c_uint64()

@@ -976,6 +976,7 @@ extern "C" void cg_shard_free(CgShard *sh)
 	cudaFree(sh->d_selected);
 	cudaFree(sh->d_narrow);
 	cudaFree(sh->d_packcols);
+	sh->row_sets.release();
 	delete sh;
 }
 
@@ -1160,35 +1161,36 @@ static int stats_end(CgContext *ctx, CgPartial *p, const unsigned long long befo
 	return CG_OK;
 }
 
-/* the plan's IN / NOT IN codes to the partial's device buffer.  Codes equal to the last ones written are already there (the
- * common case: one query over many shards).  Otherwise the copy is enqueued on the compute stream, so it runs after every
- * launch enqueued there before -- an earlier scan into this partial, still in flight, reads its own lists to the end -- and
- * before this scan's launches.  Its source is a pinned slot of a ring (a pageable source may make cudaMemcpyAsync wait
- * for the stream); a slot is reused only after its previous copy has run (its event). */
-static int upload_sets(CgContext *ctx, CgPartial *p, const std::vector<uint64_t> &codes, KPlan *plan)
+/* the plan's IN / NOT IN codes to the owner's device buffer (a partial's, or a shard's for its row scans).  Codes equal to
+ * the last ones written are already there (the common case: one query over many shards).  Otherwise the copy is enqueued on
+ * the compute stream, so it runs after every launch enqueued there before -- an earlier scan through this buffer, still in
+ * flight, reads its own lists to the end -- and before this scan's launches.  Its source is a pinned slot of a ring (a
+ * pageable source may make cudaMemcpyAsync wait for the stream); a slot is reused only after its previous copy has run (its
+ * event). */
+static int upload_sets(CgContext *ctx, CgSetBuf *owner, const std::vector<uint64_t> &codes, KPlan *plan)
 {
 	if (codes.empty()) return CG_OK;
 	const size_t cap = 2 * CG_MAX_IN_VALUES;
 	if (codes.size() > cap) return cg_set_error(CG_EINVAL, "%zu list codes", codes.size());
-	if (!p->d_sets && cudaMalloc(&p->d_sets, cap * sizeof(uint64_t)) != cudaSuccess)
+	if (!owner->d_sets && cudaMalloc(&owner->d_sets, cap * sizeof(uint64_t)) != cudaSuccess)
 	{
-		p->d_sets = nullptr;
+		owner->d_sets = nullptr;
 		return cg_set_error(CG_ENOMEM, "cudaMalloc for the IN lists failed");
 	}
-	plan->sets = p->d_sets;
-	if (codes == p->sets_last) return CG_OK;
-	const int slot = p->sets_slot;
-	p->sets_slot = (slot + 1) % CgPartial::kSetSlots;
-	if (!p->h_sets[slot]) CG_CUDA(cudaHostAlloc((void **) &p->h_sets[slot], cap * sizeof(uint64_t), cudaHostAllocDefault));
-	if (!p->sets_copied[slot]) CG_CUDA(cudaEventCreateWithFlags(&p->sets_copied[slot], cudaEventDisableTiming));
-	CG_CUDA(cudaEventSynchronize(p->sets_copied[slot]));       /* the slot's previous copy has read it */
-	memcpy(p->h_sets[slot], codes.data(), codes.size() * sizeof(uint64_t));
-	p->sets_last.clear();                                      /* the buffer's content is unknown until the copy is enqueued */
+	plan->sets = owner->d_sets;
+	if (codes == owner->last) return CG_OK;
+	const int slot = owner->slot;
+	owner->slot = (slot + 1) % CgSetBuf::kSlots;
+	if (!owner->h_sets[slot]) CG_CUDA(cudaHostAlloc((void **) &owner->h_sets[slot], cap * sizeof(uint64_t), cudaHostAllocDefault));
+	if (!owner->copied[slot]) CG_CUDA(cudaEventCreateWithFlags(&owner->copied[slot], cudaEventDisableTiming));
+	CG_CUDA(cudaEventSynchronize(owner->copied[slot]));        /* the slot's previous copy has read it */
+	memcpy(owner->h_sets[slot], codes.data(), codes.size() * sizeof(uint64_t));
+	owner->last.clear();                                       /* the buffer's content is unknown until the copy is enqueued */
 	int rc = cg_chain_end(ctx, ctx->compute);
 	if (rc) return rc;
-	CG_CUDA(cudaMemcpyAsync(p->d_sets, p->h_sets[slot], codes.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->compute));
-	CG_CUDA(cudaEventRecord(p->sets_copied[slot], ctx->compute));
-	p->sets_last = codes;
+	CG_CUDA(cudaMemcpyAsync(owner->d_sets, owner->h_sets[slot], codes.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->compute));
+	CG_CUDA(cudaEventRecord(owner->copied[slot], ctx->compute));
+	owner->last = codes;
 	return CG_OK;
 }
 
@@ -1291,7 +1293,7 @@ extern "C" int cg_scan_shard(const CgShard *sh, const CgScanDesc *desc, CgPartia
 	if (rc) return rc;
 	if (!selected.empty())
 	{
-		rc = upload_sets(ctx, into, codes, &plan);
+		rc = upload_sets(ctx, &into->sets, codes, &plan);
 		if (rc) return rc;
 		plan.arena = sh->d_arena;
 		plan.chunkcols = sh->d_chunkcols;
@@ -1346,6 +1348,160 @@ extern "C" int cg_scan_shard(const CgShard *sh, const CgScanDesc *desc, CgPartia
 		}
 	}
 	return stats_end(ctx, into, before, filtered, selected.size(), bytes, stats);
+}
+
+/*
+ * The row scan (include/citus_gpu.h states the contract).  Chunk-group skipping as cg_scan_shard does it, into a tile list
+ * of its own in shard order: the shard's cached selection is ordered [NULL-free | rest] for the aggregate kernels and is
+ * left as it is.  Scratch (tiles, bitmap, tile counts) is allocated in stream order; the only host synchronisation reads
+ * the total between the offset scan and the write pass.
+ */
+extern "C" int cg_scan_shard_rows(const CgShard *sh, const CgScanDesc *desc, const int32_t *atts, int32_t ncols, int64_t capacity,
+								  int64_t *const *d_cols, uint8_t *const *d_nulls, int64_t *nrows, CgScanStats *stats)
+{
+	CgContext *ctx = cg_ctx();
+	if (!ctx) return CG_EINVAL;
+	if (!sh || !desc || !atts || !nrows) return cg_set_error(CG_EINVAL, "NULL argument");
+	if (ncols < 1 || ncols > CG_MAX_ROW_COLS) return cg_set_error(CG_EINVAL, "%d output columns (1 .. %d)", ncols, CG_MAX_ROW_COLS);
+	if (capacity < 0) return cg_set_error(CG_EINVAL, "negative capacity %lld", (long long) capacity);
+	*nrows = 0;
+	if (stats) memset(stats, 0, sizeof *stats);
+	KPlan plan;
+	std::vector<uint64_t> codes;
+	int rc = cg_build_where_plan(desc, sh->columns.data(), sh->natts, &sh->slot_of_att, &plan, &codes);
+	if (rc) return rc;
+	KRowOut out;
+	memset(&out, 0, sizeof out);
+	out.ncols = ncols;
+	std::vector<bool> read(sh->staged.size(), false);          /* staged slots the write pass reads */
+	for (int c = 0; c < ncols; c++)
+	{
+		const int a = atts[c];
+		if (a < 0 || a >= sh->natts) return cg_set_error(CG_EINVAL, "output column %d: attribute %d out of range", c, a);
+		if (sh->slot_of_att[a] < 0) return cg_set_error(CG_EINVAL, "output column %d: attribute %d is not staged in this shard", c, a);
+		out.slot[c] = (uint8_t) sh->slot_of_att[a];
+		out.len[c] = (uint8_t) cg_decoded_len(sh->columns[a]);
+		out.isfloat[c] = (uint8_t) (sh->columns[a].type_class == CG_TYPE_FLOAT);
+		read[out.slot[c]] = true;
+	}
+	if (capacity > 0)
+	{
+		if (!d_cols) return cg_set_error(CG_EINVAL, "NULL output column array");
+		for (int c = 0; c < ncols; c++)
+			if (!d_cols[c]) return cg_set_error(CG_EINVAL, "NULL device pointer for output column %d", c);
+	}
+
+	/* SelectedChunkMask per stripe; the surviving chunk groups in shard order, cut into tiles */
+	const size_t ns = sh->staged.size();
+	std::vector<RowTile> tiles;
+	std::vector<uint8_t> mask;
+	int64_t nfiltered = 0, ncg = 0;
+	uint64_t nwords = 0, scanned = 0, bytes = 0;
+	uint32_t nullcols = 0;                                     /* output columns with NULLs in a surviving chunk group */
+	for (size_t si = 0; si < sh->stripes.size(); si++)
+	{
+		const CgStripe &s = sh->stripes[si];
+		mask.resize(s.chunk_count);
+		stripe_chunk_mask(s, sh->nodes.data(), sh->columns.data(), sh->natts, desc, mask.data(), &nfiltered);
+		for (uint32_t k = 0; k < s.chunk_count; k++)
+		{
+			if (!mask[k]) continue;
+			const uint64_t cg = sh->stripe_first_cg[si] + k;
+			const uint32_t rows = sh->cg_rows[cg];
+			ncg++;
+			scanned += rows;
+			for (uint32_t r0 = 0; r0 < rows; r0 += CG_ROW_TILE) tiles.push_back(RowTile{nwords + r0 / 64, (uint32_t) cg, r0});
+			nwords += (rows + 63) / 64;
+			for (int c = 0; c < ncols; c++)
+			{
+				const DevChunkCol &d = sh->h_chunkcols[cg * ns + out.slot[c]];
+				if (d.value_count != d.row_count) nullcols |= 1u << c;
+			}
+			for (int c = 0; c < plan.ncols; c++) bytes += sh->algorithmic_bytes_per_cg_col(cg, plan.slot[c]);
+			for (size_t slot = 0; slot < ns; slot++)
+				if (read[slot]) bytes += sh->algorithmic_bytes_per_cg_col(cg, (int) slot);
+		}
+	}
+	for (int c = 0; c < ncols && capacity > 0; c++)
+		if (((nullcols >> c) & 1u) && !(d_nulls && d_nulls[c]))
+			return cg_set_error(CG_EINVAL, "output column %d (attribute %d) has NULLs in a chunk group that is scanned: it needs a null array",
+								c, atts[c]);
+	if (stats)
+	{
+		stats->chunk_groups_filtered = nfiltered;
+		stats->chunk_groups_scanned = ncg;
+		stats->rows_scanned = (int64_t) scanned;
+		stats->rows_removed_by_filter = (int64_t) scanned;
+		stats->bytes_scanned = (int64_t) bytes;
+	}
+	if (tiles.empty()) return CG_OK;
+
+	/* one stream-ordered allocation: tiles | tile counts, then offsets | total | bitmap */
+	const int64_t ntiles = (int64_t) tiles.size();
+	auto a256 = [](size_t x) { return (x + 255) & ~(size_t) 255; };
+	const size_t tb = a256(tiles.size() * sizeof(RowTile)), cb = a256((size_t) ntiles * 8), ob = 256;
+	rc = cg_chain_end(ctx, ctx->compute);
+	if (rc) return rc;
+	CgAsyncBuf mem;
+	if (mem.alloc(tb + cb + ob + nwords * 8, ctx->compute) != cudaSuccess)
+	{
+		cudaGetLastError();
+		return cg_set_error(CG_ENOMEM, "cudaMallocAsync of %zu bytes for the row scan failed", tb + cb + ob + (size_t) nwords * 8);
+	}
+	uint8_t *d = mem.as<uint8_t>();
+	RowTile *d_tiles = (RowTile *) d;
+	unsigned long long *d_counts = (unsigned long long *) (d + tb);
+	unsigned long long *d_tot = (unsigned long long *) (d + tb + cb);
+	uint64_t *d_bitmap = (uint64_t *) (d + tb + cb + ob);
+	CG_CUDA(cudaMemcpyAsync(d_tiles, tiles.data(), tiles.size() * sizeof(RowTile), cudaMemcpyHostToDevice, ctx->compute));
+	rc = upload_sets(ctx, &const_cast<CgShard *>(sh)->row_sets, codes, &plan);
+	if (rc) return rc;
+	plan.arena = sh->d_arena;
+	plan.chunkcols = sh->d_chunkcols;
+	plan.nstaged = (int32_t) ns;
+	if (stats) CG_CUDA(cudaEventRecord(ctx->ev_a, ctx->compute));
+	rc = cg_launch_rows_select(ctx, plan, d_tiles, ntiles, d_bitmap, d_counts, ctx->compute);
+	if (rc) return rc;
+	CgAsyncBuf chunk_buf;
+	rc = partition_scan_blocks(ctx, d_counts, d_tot, ntiles, 1, &chunk_buf);
+	if (rc) return rc;
+	if (stats) CG_CUDA(cudaEventRecord(ctx->ev_b, ctx->compute));
+	unsigned long long total = 0;
+	CG_CUDA(cudaMemcpyAsync(&total, d_tot, sizeof total, cudaMemcpyDeviceToHost, ctx->compute));
+	CG_CUDA(cudaStreamSynchronize(ctx->compute));
+	*nrows = (int64_t) total;
+	if (stats)
+	{
+		float ms = 0;
+		CG_CUDA(cudaEventElapsedTime(&ms, ctx->ev_a, ctx->ev_b));
+		stats->kernel_ms = ms;
+		stats->rows_passed = (int64_t) total;
+		stats->rows_removed_by_filter = (int64_t) (scanned - total);
+	}
+	if ((int64_t) total > capacity)
+		return capacity == 0 ? CG_OK : cg_set_error(CG_EINVAL, "%llu rows pass the WHERE tree, more than the capacity %lld", total, (long long) capacity);
+	if (total == 0) return CG_OK;
+	out.arena = sh->d_arena;
+	out.chunkcols = sh->d_chunkcols;
+	out.nstaged = (int32_t) ns;
+	for (int c = 0; c < ncols; c++)
+	{
+		out.cols[c] = d_cols[c];
+		out.nulls[c] = d_nulls ? d_nulls[c] : nullptr;
+	}
+	if (stats) CG_CUDA(cudaEventRecord(ctx->ev_a, ctx->compute));
+	rc = cg_launch_rows_write(ctx, out, d_tiles, ntiles, d_bitmap, d_counts, ctx->compute);
+	if (rc) return rc;
+	if (stats)
+	{
+		/* with stats the call waits for the write pass too, to time it */
+		CG_CUDA(cudaEventRecord(ctx->ev_b, ctx->compute));
+		CG_CUDA(cudaEventSynchronize(ctx->ev_b));
+		float ms = 0;
+		CG_CUDA(cudaEventElapsedTime(&ms, ctx->ev_a, ctx->ev_b));
+		stats->kernel_ms += ms;
+	}
+	return CG_OK;
 }
 
 /* the comparison class of a join key column (0 = float, not a join key) and its numeric scale */
@@ -1415,7 +1571,7 @@ extern "C" int cg_join_aggregate(const CgJoinSide *build, const CgJoinSide *prob
 	unsigned long long before[3];
 	rc = stats_begin(ctx, into, stats, before);
 	if (rc) return rc;
-	rc = upload_sets(ctx, into, codes, &plan);
+	rc = upload_sets(ctx, &into->sets, codes, &plan);
 	if (rc) return rc;
 	if (stats)
 	{
@@ -1631,7 +1787,7 @@ extern "C" int cg_scan_relation(const CgRelation *rel, const CgScanDesc *desc, C
 	if (rc) return rc;
 	rc = before_scan(ctx, into);
 	if (rc) return rc;
-	rc = upload_sets(ctx, into, codes, &plan);
+	rc = upload_sets(ctx, &into->sets, codes, &plan);
 	if (rc) return rc;
 
 	std::vector<std::vector<uint8_t>> select(rel->nstripes);

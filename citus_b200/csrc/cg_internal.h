@@ -136,6 +136,34 @@ static inline __host__ __device__ uint64_t cg_narrow_words(uint32_t rows, uint32
 	return (uint64_t) ((rows + 63u) / 64u) * width;
 }
 
+/* the device copy of a plan's IN / NOT IN codes (2 * CG_MAX_IN_VALUES words, allocated by the first scan with a list):
+ * written with cudaMemcpyAsync on the compute stream before a launch whose codes differ from the last ones written
+ * (last), so that the copy is ordered behind every earlier launch that reads the buffer (cg_set_stream synchronises the
+ * old stream before switching).  The copies come from a ring of pinned slots: a slot is rewritten once the copy recorded
+ * in its event has run, so the host does not wait behind the stream's earlier kernels.  A partial owns one for its
+ * scans, a shard one for its row scans (cg_scan_shard_rows) */
+struct CgSetBuf
+{
+	uint64_t *d_sets = nullptr;
+	std::vector<uint64_t> last;
+	static const int kSlots = 4;
+	uint64_t *h_sets[kSlots] = {nullptr, nullptr, nullptr, nullptr};
+	cudaEvent_t copied[kSlots] = {nullptr, nullptr, nullptr, nullptr};
+	int slot = 0;
+	void release()
+	{
+		cudaFree(d_sets);
+		d_sets = nullptr;
+		for (int i = 0; i < kSlots; i++)
+		{
+			if (copied[i]) { cudaEventSynchronize(copied[i]); cudaEventDestroy(copied[i]); }
+			if (h_sets[i]) cudaFreeHost(h_sets[i]);
+			copied[i] = nullptr; h_sets[i] = nullptr;
+		}
+		last.clear();
+	}
+};
+
 struct CgShard
 {
 	int natts = 0;
@@ -176,6 +204,8 @@ struct CgShard
 	DevPackCol *d_packcols = nullptr;        /* [nchunkgroups][nstaged] */
 	std::vector<DevPackCol> h_packcols;
 	std::vector<uint8_t> slot_narrow;        /* per staged slot: 1 = the column has images */
+	/* the IN-list codes of the row scans (cg_scan_shard_rows); they never touch the selection cache above */
+	CgSetBuf row_sets;
 	uint64_t algorithmic_bytes_per_cg_col(uint64_t cg, int slot) const
 	{
 		const DevChunkCol &c = h_chunkcols[cg * staged.size() + slot];
@@ -507,17 +537,8 @@ struct CgPartial
 	/* pinned host buffer the result rows are fetched through */
 	uint8_t *h_out = nullptr;
 	size_t h_out_cap = 0;
-	/* the codes of the IN / NOT IN lists of the scan in flight (2 * CG_MAX_IN_VALUES words, allocated by the first scan with a
-	 * list): written with cudaMemcpyAsync on the compute stream before a launch whose codes differ from the last ones
-	 * written (sets_last), so that the copy is ordered behind every earlier launch that reads the buffer (cg_set_stream
-	 * synchronises the old stream before switching).  The copies come from a ring of pinned slots: a slot is rewritten once
-	 * the copy recorded in its event has run, so the host does not wait behind the stream's earlier kernels */
-	uint64_t *d_sets = nullptr;
-	std::vector<uint64_t> sets_last;
-	static const int kSetSlots = 4;
-	uint64_t *h_sets[kSetSlots] = {nullptr, nullptr, nullptr, nullptr};
-	cudaEvent_t sets_copied[kSetSlots] = {nullptr, nullptr, nullptr, nullptr};
-	int sets_slot = 0;
+	/* the codes of the IN / NOT IN lists of the scan in flight */
+	CgSetBuf sets;
 };
 
 /* cg_scan.cu */
@@ -628,6 +649,38 @@ int cg_partition_route_scatter_async(const int64_t *d_keys, const uint8_t *d_nul
  * a plan column's slot is its joined-row attribute: build columns first, then probe columns), on `stream` */
 int cg_launch_join_aggregate(CgContext *ctx, const KPlan &plan, const CgJoinSide *const sides[2], cudaStream_t stream);
 
+/* cg_scan_rows.cu: the row scan (cg_scan_shard_rows).  A tile is CG_ROW_TILE rows of one chunk group starting at row0 (a
+ * multiple of it); its selection bits are the bitmap words [word, word + ceil(rows / 64)) */
+#define CG_ROW_TILE 2048
+#define CG_MAX_ROW_COLS 16
+struct RowTile
+{
+	uint64_t word;
+	uint32_t cg;
+	uint32_t row0;
+};
+/* the projected columns of a row scan: staged slot, decoded width and float flag of every output column, and the caller's
+ * device arrays (nulls[c] may be NULL when the column has no NULLs in the chunk groups scanned) */
+struct KRowOut
+{
+	const uint8_t *arena;
+	const DevChunkCol *chunkcols;
+	int32_t nstaged;
+	int32_t ncols;
+	uint8_t slot[CG_MAX_ROW_COLS];
+	uint8_t len[CG_MAX_ROW_COLS];
+	uint8_t isfloat[CG_MAX_ROW_COLS];
+	int64_t *cols[CG_MAX_ROW_COLS];
+	uint8_t *nulls[CG_MAX_ROW_COLS];
+};
+/* pass 1: the WHERE tree of plan (arena, chunkcols and nstaged set; selected unused) over every tile: bitmap bits and the
+ * passing rows of every tile in counts[t] */
+int cg_launch_rows_select(CgContext *ctx, const KPlan &plan, const RowTile *tiles, int64_t ntiles, uint64_t *bitmap,
+						  unsigned long long *counts, cudaStream_t stream);
+/* pass 3: the passing rows of every tile to offsets[t] + their rank in the tile */
+int cg_launch_rows_write(CgContext *ctx, const KRowOut &out, const RowTile *tiles, int64_t ntiles, const uint64_t *bitmap,
+						 const unsigned long long *offsets, cudaStream_t stream);
+
 /* cg_comm.cu */
 void cg_comm_set_peer_window(int on);
 
@@ -647,6 +700,10 @@ void cg_shard_build_narrow(CgContext *ctx, CgShard *sh);
 int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts,
 				  const std::vector<int32_t> *slot_of_att, CgPartial *partial, KPlan *plan,
 				  bool *all8, std::vector<uint64_t> *set_codes = nullptr);
+/* the WHERE half of cg_build_plan alone, for a descriptor without aggregates, group columns, FILTER or CASE (the row scan):
+ * plan columns, atoms, IN-list codes, column atoms and the tree; no group table */
+int cg_build_where_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts, const std::vector<int32_t> *slot_of_att,
+						KPlan *plan, std::vector<uint64_t> *set_codes);
 /* what of the IN lists a WHERE list reads, for comparing two WHERE lists (empty without IN / NOT IN atoms) */
 std::vector<int64_t> cg_where_lists(const CgScanDesc *desc);
 

@@ -614,12 +614,8 @@ extern "C" void cg_partial_free(CgPartial *p)
 {
 	if (!p) return;
 	cudaFree(p->d_table); cudaFree(p->d_stats); cudaFree(p->d_out_keys); cudaFree(p->d_out_words); cudaFree(p->d_packed);
-	cudaFree(p->d_out_nulls); cudaFree(p->d_out_count); cudaFree(p->d_sets);
-	for (int i = 0; i < CgPartial::kSetSlots; i++)
-	{
-		if (p->sets_copied[i]) { cudaEventSynchronize(p->sets_copied[i]); cudaEventDestroy(p->sets_copied[i]); }
-		if (p->h_sets[i]) cudaFreeHost(p->h_sets[i]);
-	}
+	cudaFree(p->d_out_nulls); cudaFree(p->d_out_count);
+	p->sets.release();
 	if (p->h_out) cudaFreeHost(p->h_out);
 	if (p->h_ret) cudaFreeHost(p->h_ret);
 	delete p;
@@ -670,8 +666,157 @@ static bool same_case(const CgScanDesc *x, const CgScanDesc *y, int a)
 
 /*
  * Kernel plan: deduplicated projection (columnar_customscan.c:1813-1851 ColumnarAttrNeeded:
- * only the columns the quals, group keys and aggregate arguments reference are read).
+ * only the columns the quals, group keys and aggregate arguments reference are read).  Plan columns are numbered in first
+ * use: the WHERE atoms' columns first, so the WHERE half (where()) is the same for an aggregate scan and a row scan.
  */
+struct PlanBuilder
+{
+	const CgScanDesc *desc;
+	const CgColumnDesc *columns;
+	int natts;
+	const std::vector<int32_t> *slot_of_att;
+	KPlan *plan;
+	int pcol_of_att[256];
+	int ncols = 0;
+	/* IN / NOT IN lists: every list's codes once per kind (integer / float), back to back */
+	std::vector<uint64_t> codes;
+	int list_at[CG_MAX_IN_LISTS][2];
+
+	PlanBuilder(const CgScanDesc *d, const CgColumnDesc *c, int n, const std::vector<int32_t> *s, KPlan *p)
+		: desc(d), columns(c), natts(n), slot_of_att(s), plan(p)
+	{
+		memset(plan, 0, sizeof *plan);
+		for (int i = 0; i < 256; i++) pcol_of_att[i] = -1;
+		for (int l = 0; l < CG_MAX_IN_LISTS; l++) list_at[l][0] = list_at[l][1] = -1;
+	}
+
+	/* the plan column of attribute att, added on first use */
+	int use(int att, int *pc)
+	{
+		if (pcol_of_att[att] >= 0) { *pc = pcol_of_att[att]; return CG_OK; }
+		if (ncols == CG_KMAX_COLS) return cg_set_error(CG_EUNSUPPORTED, "query reads more than %d columns", CG_KMAX_COLS);
+		int slot = slot_of_att ? (*slot_of_att)[att] : att;
+		if (slot < 0) return cg_set_error(CG_EINVAL, "column %d is not staged in this shard", att);
+		plan->slot[ncols] = (uint8_t) slot;
+		plan->len[ncols] = (uint8_t) cg_decoded_len(columns[att]);       /* a varlena column reaches the kernels decoded to a fixed width */
+		plan->isfloat[ncols] = (uint8_t) (columns[att].type_class == CG_TYPE_FLOAT);
+		pcol_of_att[att] = ncols;
+		*pc = ncols++;
+		return CG_OK;
+	}
+
+	/* integer atoms in range form: pass iff ((x >= lo && x <= hi) != neg); float atoms keep op + constant (a float4
+	 * column's values are promoted to float8, the constant already is float8 bits) */
+	static void atom_range(const CgQual &q, int64_t *lo_out, int64_t *hi_out, uint8_t *neg_out)
+	{
+		int64_t k = q.konst, lo = INT64_MIN, hi = INT64_MAX;
+		bool neg = false;
+		if (cg_op_is_column(q.op)) { *lo_out = *hi_out = 0; *neg_out = 0; return; }     /* no constant: KCmp instead */
+		switch (q.op)
+		{
+			case CG_OP_LT: if (k == INT64_MIN) { lo = 1; hi = 0; } else hi = k - 1; break;
+			case CG_OP_LE: hi = k; break;
+			case CG_OP_EQ: lo = hi = k; break;
+			case CG_OP_GE: lo = k; break;
+			case CG_OP_GT: if (k == INT64_MAX) { lo = 1; hi = 0; } else lo = k + 1; break;
+			default: lo = hi = k; neg = true; break;
+		}
+		*lo_out = lo; *hi_out = hi; *neg_out = neg;
+	}
+
+	/* IN / NOT IN lists: each atom's list as sorted, distinct codes in its column's order (cg_set_code); the atoms of one
+	 * list on columns of one kind (integer / float) share them.  A list of NULLs only has no code (len 0): no row is found
+	 * in it, and nnull decides. */
+	void set_of(const CgQual &q, bool isfloat, KSet *ks)
+	{
+		memset(ks, 0, sizeof *ks);
+		if (!op_is_list(q.op)) return;
+		const CgInList &L = desc->in_lists[q.konst];
+		int &at = list_at[q.konst][isfloat];
+		std::vector<uint64_t> c;
+		for (int i = 0; i < L.nvalues; i++) c.push_back(cg_set_code(desc->in_values[L.first + i], isfloat));
+		std::sort(c.begin(), c.end());
+		c.erase(std::unique(c.begin(), c.end()), c.end());
+		if (at < 0)
+		{
+			at = (int) codes.size();
+			codes.insert(codes.end(), c.begin(), c.end());
+		}
+		ks->off = (uint16_t) at;
+		ks->len = (uint16_t) c.size();
+		int steps = 0;
+		while ((1u << steps) < c.size()) steps++;
+		ks->steps = (uint8_t) steps;
+		ks->nnull = (uint8_t) (L.nnulls > 0);
+	}
+
+	/* column atoms: the other column is a plan column too; integer-like sides of different scales align on the larger one */
+	int cmp_of(const CgQual &q, KCmp *kc)
+	{
+		memset(kc, 0, sizeof *kc);
+		kc->mul = 1;
+		if (!cg_op_is_column(q.op)) return CG_OK;
+		int pc = 0, rc;
+		if ((rc = use((int) q.konst, &pc))) return rc;
+		kc->col2 = (uint8_t) pc;
+		const CgColumnDesc &x = columns[q.column], &y = columns[q.konst];
+		if (cmp_class(x) != CMP_INTEGER) return CG_OK;
+		const int sx = cg_type_class(x) == CG_TYPE_NUMERIC ? cg_type_scale(x) : 0;
+		const int sy = cg_type_class(y) == CG_TYPE_NUMERIC ? cg_type_scale(y) : 0;
+		kc->right = (uint8_t) (sx > sy);
+		for (int i = 0; i < (sx > sy ? sx - sy : sy - sx); i++) kc->mul *= 10;      /* <= 10^18 */
+		return CG_OK;
+	}
+
+	/* the WHERE half: atoms, lists, column atoms and the tree */
+	int where()
+	{
+		int rc;
+		plan->nquals = desc->nquals;
+		for (int q = 0; q < desc->nquals; q++)
+		{
+			int pc = 0;
+			if ((rc = use(desc->quals[q].column, &pc))) return rc;
+			plan->qcol[q] = (uint8_t) pc;
+			plan->qop[q] = (uint8_t) desc->quals[q].op;
+			plan->qk[q] = desc->quals[q].konst;
+			atom_range(desc->quals[q], &plan->qlo[q], &plan->qhi[q], &plan->qneg[q]);
+			set_of(desc->quals[q], plan->isfloat[pc], &plan->qset[q]);
+			if ((rc = cmp_of(desc->quals[q], &plan->qcc[q]))) return rc;
+		}
+		plan->slices = 1; plan->slice_rows = 1u << 30; plan->max_cg_rows = 0;
+		plan->nqexpr = desc->nqual_expr;
+		for (int i = 0; i < desc->nqual_expr; i++) plan->qexpr[i] = desc->qual_expr[i];
+		return CG_OK;
+	}
+
+	/* the plan columns and the list codes (KPlan.sets is left NULL for the caller to point at their device copy) */
+	void finish(std::vector<uint64_t> *set_codes, bool *all8)
+	{
+		plan->sets = nullptr;
+		if (set_codes) set_codes->swap(codes);
+		plan->ncols = ncols;
+		bool a8 = true;
+		for (int c = 0; c < ncols; c++) if (plan->len[c] != 8) a8 = false;
+		*all8 = a8;
+	}
+};
+
+int cg_build_where_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts, const std::vector<int32_t> *slot_of_att,
+						KPlan *plan, std::vector<uint64_t> *set_codes)
+{
+	if (desc->naggs != 0 || desc->ngroup_cols != 0 || desc->composite_key != 0 || cg_desc_uses_pool(desc) || desc->ncase_arms != 0)
+		return cg_set_error(CG_EINVAL, "a row scan takes a WHERE tree only: no aggregates, group columns, FILTER, CASE or composite key");
+	int rc = validate_desc(desc, columns, natts);
+	if (rc) return rc;
+	if (natts > 256) return cg_set_error(CG_EUNSUPPORTED, "more than 256 attributes");
+	PlanBuilder b(desc, columns, natts, slot_of_att, plan);
+	if ((rc = b.where())) return rc;
+	bool all8;
+	b.finish(set_codes, &all8);
+	return CG_OK;
+}
+
 int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts,
 				  const std::vector<int32_t> *slot_of_att, CgPartial *partial, KPlan *plan, bool *all8,
 				  std::vector<uint64_t> *set_codes)
@@ -695,107 +840,14 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 				partial->desc.key_col_max[g] != desc->key_col_max[g])
 				return cg_set_error(CG_EINVAL, "partial aggregate was created for other composite key columns or bounds (column %d)", g);
 
-	memset(plan, 0, sizeof *plan);
-	int pcol_of_att[256];
-	if (natts > 256) return cg_set_error(CG_EUNSUPPORTED, "more than 256 attributes");
-	for (int c = 0; c < natts; c++) pcol_of_att[c] = -1;
-	int ncols = 0;
-	auto use = [&](int att) -> int {
-		if (pcol_of_att[att] >= 0) return pcol_of_att[att];
-		if (ncols == CG_KMAX_COLS) return -1;
-		int slot = slot_of_att ? (*slot_of_att)[att] : att;
-		if (slot < 0) return -2;
-		plan->slot[ncols] = (uint8_t) slot;
-		plan->len[ncols] = (uint8_t) cg_decoded_len(columns[att]);       /* a varlena column reaches the kernels decoded to a fixed width */
-		plan->isfloat[ncols] = (uint8_t) (columns[att].type_class == CG_TYPE_FLOAT);
-		pcol_of_att[att] = ncols;
-		return ncols++;
-	};
-#define USE_OR_FAIL(dst, att)                                                                       \
-	do {                                                                                            \
-		int pc__ = use(att);                                                                        \
-		if (pc__ == -1) return cg_set_error(CG_EUNSUPPORTED, "query reads more than %d columns", CG_KMAX_COLS); \
-		if (pc__ == -2) return cg_set_error(CG_EINVAL, "column %d is not staged in this shard", att);  \
-		dst = pc__;                                                                                 \
-	} while (0)
-
-	/* integer atoms in range form: pass iff ((x >= lo && x <= hi) != neg); float atoms keep op + constant (a float4
-	 * column's values are promoted to float8, the constant already is float8 bits) */
-	auto atom_range = [](const CgQual &q, int64_t *lo_out, int64_t *hi_out, uint8_t *neg_out) {
-		int64_t k = q.konst, lo = INT64_MIN, hi = INT64_MAX;
-		bool neg = false;
-		if (cg_op_is_column(q.op)) { *lo_out = *hi_out = 0; *neg_out = 0; return; }     /* no constant: KCmp instead */
-		switch (q.op)
-		{
-			case CG_OP_LT: if (k == INT64_MIN) { lo = 1; hi = 0; } else hi = k - 1; break;
-			case CG_OP_LE: hi = k; break;
-			case CG_OP_EQ: lo = hi = k; break;
-			case CG_OP_GE: lo = k; break;
-			case CG_OP_GT: if (k == INT64_MAX) { lo = 1; hi = 0; } else lo = k + 1; break;
-			default: lo = hi = k; neg = true; break;
-		}
-		*lo_out = lo; *hi_out = hi; *neg_out = neg;
-	};
-	/* IN / NOT IN lists: each atom's list as sorted, distinct codes in its column's order (cg_set_code); the atoms of one
-	 * list on columns of one kind (integer / float) share them.  A list of NULLs only has no code (len 0): no row is found
-	 * in it, and nnull decides. */
-	std::vector<uint64_t> codes;
-	int list_at[CG_MAX_IN_LISTS][2];
-	for (int l = 0; l < CG_MAX_IN_LISTS; l++) list_at[l][0] = list_at[l][1] = -1;
-	auto set_of = [&](const CgQual &q, bool isfloat, KSet *ks) {
-		memset(ks, 0, sizeof *ks);
-		if (!op_is_list(q.op)) return;
-		const CgInList &L = desc->in_lists[q.konst];
-		int &at = list_at[q.konst][isfloat];
-		std::vector<uint64_t> c;
-		for (int i = 0; i < L.nvalues; i++) c.push_back(cg_set_code(desc->in_values[L.first + i], isfloat));
-		std::sort(c.begin(), c.end());
-		c.erase(std::unique(c.begin(), c.end()), c.end());
-		if (at < 0)
-		{
-			at = (int) codes.size();
-			codes.insert(codes.end(), c.begin(), c.end());
-		}
-		ks->off = (uint16_t) at;
-		ks->len = (uint16_t) c.size();
-		int steps = 0;
-		while ((1u << steps) < c.size()) steps++;
-		ks->steps = (uint8_t) steps;
-		ks->nnull = (uint8_t) (L.nnulls > 0);
-	};
-	/* column atoms: the other column is a plan column too; integer-like sides of different scales align on the larger one */
-	auto cmp_of = [&](const CgQual &q, KCmp *kc) -> int {
-		memset(kc, 0, sizeof *kc);
-		kc->mul = 1;
-		if (!cg_op_is_column(q.op)) return CG_OK;
-		int pc; USE_OR_FAIL(pc, (int) q.konst);
-		kc->col2 = (uint8_t) pc;
-		const CgColumnDesc &x = columns[q.column], &y = columns[q.konst];
-		if (cmp_class(x) != CMP_INTEGER) return CG_OK;
-		const int sx = cg_type_class(x) == CG_TYPE_NUMERIC ? cg_type_scale(x) : 0;
-		const int sy = cg_type_class(y) == CG_TYPE_NUMERIC ? cg_type_scale(y) : 0;
-		kc->right = (uint8_t) (sx > sy);
-		for (int i = 0; i < (sx > sy ? sx - sy : sy - sx); i++) kc->mul *= 10;      /* <= 10^18 */
-		return CG_OK;
-	};
-	plan->nquals = desc->nquals;
-	for (int q = 0; q < desc->nquals; q++)
-	{
-		int pc; USE_OR_FAIL(pc, desc->quals[q].column);
-		plan->qcol[q] = (uint8_t) pc;
-		plan->qop[q] = (uint8_t) desc->quals[q].op;
-		plan->qk[q] = desc->quals[q].konst;
-		atom_range(desc->quals[q], &plan->qlo[q], &plan->qhi[q], &plan->qneg[q]);
-		set_of(desc->quals[q], plan->isfloat[pc], &plan->qset[q]);
-		if ((rc = cmp_of(desc->quals[q], &plan->qcc[q]))) return rc;
-	}
-	plan->slices = 1; plan->slice_rows = 1u << 30; plan->max_cg_rows = 0;
-	plan->nqexpr = desc->nqual_expr;
-	for (int i = 0; i < desc->nqual_expr; i++) plan->qexpr[i] = desc->qual_expr[i];
+	if (natts > 256) { memset(plan, 0, sizeof *plan); return cg_set_error(CG_EUNSUPPORTED, "more than 256 attributes"); }
+	PlanBuilder b(desc, columns, natts, slot_of_att, plan);
+	if ((rc = b.where())) return rc;
 	plan->ngroup = desc->ngroup_cols;
 	for (int g = 0; g < desc->ngroup_cols; g++)
 	{
-		int pc; USE_OR_FAIL(pc, desc->group_cols[g]);
+		int pc = 0;
+		if ((rc = b.use(desc->group_cols[g], &pc))) return rc;
 		plan->gcol[g] = (uint8_t) pc;
 	}
 	if (desc->composite_key)
@@ -811,7 +863,8 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 		plan->aggs[a] = partial->aggs[a];
 		for (int f = 0; f < desc->aggs[a].nfactors; f++)
 		{
-			int pc; USE_OR_FAIL(pc, desc->aggs[a].column[f]);
+			int pc = 0;
+			if ((rc = b.use(desc->aggs[a].column[f], &pc))) return rc;
 			plan->aggs[a].pcol[f] = (int8_t) pc;
 		}
 	}
@@ -838,7 +891,8 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 				k.nfactors = (int8_t) A.nfactors;
 				for (int f = 0; f < A.nfactors; f++)
 				{
-					int pc; USE_OR_FAIL(pc, A.column[f]);
+					int pc = 0;
+					if ((rc = b.use(A.column[f], &pc))) return rc;
 					k.pcol[f] = (int8_t) pc;
 					k.a[f] = A.a[f];
 					k.b[f] = A.b[f];
@@ -853,13 +907,14 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 		plan->nfquals = desc->nfilter_quals;
 		for (int q = 0; q < desc->nfilter_quals; q++)
 		{
-			int pc; USE_OR_FAIL(pc, desc->filter_quals[q].column);
+			int pc = 0;
+			if ((rc = b.use(desc->filter_quals[q].column, &pc))) return rc;
 			plan->fcol[q] = (uint8_t) pc;
 			plan->fop[q] = (uint8_t) desc->filter_quals[q].op;
 			plan->fk[q] = desc->filter_quals[q].konst;
-			atom_range(desc->filter_quals[q], &plan->flo[q], &plan->fhi[q], &plan->fneg[q]);
-			set_of(desc->filter_quals[q], plan->isfloat[pc], &plan->fset[q]);
-			if ((rc = cmp_of(desc->filter_quals[q], &plan->fcc[q]))) return rc;
+			PlanBuilder::atom_range(desc->filter_quals[q], &plan->flo[q], &plan->fhi[q], &plan->fneg[q]);
+			b.set_of(desc->filter_quals[q], plan->isfloat[pc], &plan->fset[q]);
+			if ((rc = b.cmp_of(desc->filter_quals[q], &plan->fcc[q]))) return rc;
 		}
 		for (int a = 0; a < desc->naggs; a++)
 		{
@@ -869,12 +924,7 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 			for (int i = 0; i < desc->narg_expr[a]; i++) plan->argexpr[a][i] = desc->arg_expr[a][i];
 		}
 	}
-	plan->sets = nullptr;
-	if (set_codes) set_codes->swap(codes);
-	plan->ncols = ncols;
-	bool a8 = true;
-	for (int c = 0; c < ncols; c++) if (plan->len[c] != 8) a8 = false;
-	*all8 = a8;
+	b.finish(set_codes, all8);
 
 	plan->mode = partial->mode;
 	plan->nwords = partial->nwords;
@@ -894,7 +944,6 @@ int cg_build_plan(const CgScanDesc *desc, const CgColumnDesc *columns, int natts
 	plan->pack_word = partial->pack_word;
 	return CG_OK;
 }
-
 
 /*
  * Specialised-kernel eligibility: 8-byte integer columns only; the WHERE list reduces to at

@@ -491,6 +491,41 @@ int cg_partial_set_packing(CgPartial *p, int32_t enable);
  * given (counters need the kernel to finish). */
 int cg_scan_shard(const CgShard *shard, const CgScanDesc *desc, CgPartial *into, CgScanStats *stats);
 
+/* Row-emitting scan of one staged shard:
+ *     SELECT atts[0 .. ncols) FROM shard WHERE <desc's WHERE tree>        in the shard's row order
+ * the filter query of a repartition join's map task (worker_partition_query_result,
+ * executor/partitioned_intermediate_results.c:115-298), with the rows left in device columns.
+ *   WHERE.  desc supplies the WHERE part only: quals, qual_expr, IN lists, IS [NOT] NULL atoms, column atoms and
+ *   enable_qual_pushdown, with the rules of cg_scan_shard (a row passes only when the tree is TRUE under three-valued
+ *   logic; chunk-group skipping is SelectedChunkMask over the skip nodes).  A desc with aggregates, group columns, FILTER
+ *   or predicate-argument trees, CASE arms or a composite key is CG_EINVAL.  The WHERE columns count toward the kernels'
+ *   column limit (8) as for a scan (CG_EUNSUPPORTED over it).
+ *   Order.  Stripes in order, chunk groups in order, rows in order: the order in which ColumnarScan hands rows to
+ *   PartitionedResultDestReceiver, so cg_partition_copy_serialize over these rows writes the reference's files.
+ *   Columns.  1 .. 16 output columns (the COPY serializer's limit); an attribute may appear more than once; one that is
+ *   out of range or not staged in the shard is CG_EINVAL.  d_cols[c] receives the values of atts[c] in CgJoinSide's form:
+ *   integers sign-extended to int64, bool 0 / 1, char(1) as the unsigned byte, numeric(p, s) as value * 10^s, float4 /
+ *   float8 as float8 bits; a NULL's value slot holds 0.
+ *   NULLs.  d_nulls may be NULL, and so may any d_nulls[c]; a given null array receives one byte per output row, 1 for
+ *   NULL and 0 otherwise.  With capacity > 0, d_nulls[c] is required when atts[c] has NULLs in a chunk group that
+ *   survives skipping (value_count != row_count in its skip node): a missing one is CG_EINVAL before anything is
+ *   launched.
+ *   Capacity.  *nrows = the number of passing rows.  capacity = 0 writes nothing (size the arrays, call again); a capacity
+ *   below *nrows is CG_EINVAL with *nrows set and no output byte written.  d_cols and every d_cols[c] must be device
+ *   pointers when capacity > 0.
+ *   Synchronisation.  The call waits once for the host to read the total; the writes are enqueued on the library's
+ *   compute stream (cg_set_stream), so the next library call on it -- routing, the exchange, a join -- sees them.  With
+ *   stats the call also waits for the writes.  The row scan ends a chain of scan launches like any other enqueue, and
+ *   leaves the shard's chunk-group selection for cg_scan_shard as it was.
+ *   Stats (may be NULL): rows_scanned (rows of the surviving chunk groups), rows_removed_by_filter, rows_passed,
+ *   chunk_groups_filtered, chunk_groups_scanned, bytes_scanned = the algorithmic bytes of the WHERE columns plus those of
+ *   the distinct projected columns over the surviving chunk groups, kernel_ms = device time of the row kernels.
+ *   A shard without rows, or one whose chunk groups are all skipped, gives *nrows = 0 and CG_OK.
+ * Not covered: host pages (cg_scan_relation's transient form; stage first), narrow images, expressions in the
+ * projection. */
+int cg_scan_shard_rows(const CgShard *shard, const CgScanDesc *desc, const int32_t *atts, int32_t ncols, int64_t capacity,
+					   int64_t *const *d_cols, uint8_t *const *d_nulls, int64_t *nrows, CgScanStats *stats);
+
 /* End-to-end call on HOST buffers: stage + scan.  This is what a GpuColumnarAgg CustomScan
  * node calls once per shard task.  Pageable pages (shared_buffers as it is today) are
  * de-framed by host threads into pinned blocks and sent with cudaMemcpyAsync; pages in
